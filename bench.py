@@ -1,14 +1,15 @@
 #!/usr/bin/env python
-"""bench.py -- acquisition steps/sec of the CODA hot path on B200 (BASELINE.json metric).
+"""bench.py -- acquisition steps/sec of the CODA hot path on an H100 (BASELINE.json metric).
 
     python bench.py --gpus 1 --steps 50 --warmup 5                 # our arm, one JSON line
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
            --master-port P bench.py --gpus N --steps K --warmup W  # N-axis sharded over N GPUs
     python bench.py --impl reference --steps 2 --warmup 1          # reference algorithm on the host cores
+    python bench.py --steps 50 --warmup 5 --dump-outputs DIR       # also write the last timed step's outputs as .npy
 
 One step = get_next_item_to_label() -> oracle(idx) -> add_label() -> get_best_model_prediction()
-(reference main.py:91-94).  Workload: synthetic M=256, N=1e6, C=100 (BASELINE.json configs[2]),
-strong scaling: the N axis is split over the ranks.
+(reference main.py:91-94).  Workload: synthetic M=256, N=5e5, C=100 (BASELINE.json configs[2] at half the items: the
+51 GB fp32 slab fits an 80 GB H100 beside the row cache), strong scaling: the N axis is split over the ranks.
 
   value  steps/s of the host-free device loop (labels resident in HBM; pick = arg-max, first index on equal values),
          CUDA-event timed, max over ranks;
@@ -33,7 +34,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 WORKLOADS = {
-    "cfg3": dict(H=256, N=1_000_000, C=100),     # BASELINE.json configs[2] / configs[3]
+    "cfg3": dict(H=256, N=500_000, C=100),       # BASELINE.json configs[2] / configs[3], N halved for 80 GB
     "cfg2": dict(H=64, N=50_000, C=10),          # BASELINE.json configs[1] (parity config)
     "mini": dict(H=32, N=20_000, C=10),          # smoke-sized
     # BASELINE.json configs[4]: 16.4 TB as dense fp32 -- runs from the compact top-K slab (98 GB over 8 GPUs); perf-only,
@@ -42,7 +43,7 @@ WORKLOADS = {
     "cfg5mini": dict(H=1024, N=131_072, C=1000, K=4, compact=True),
     "cfg5shard": dict(H=1024, N=500_000, C=1000, K=4, compact=True),     # what one of the 8 GPUs of cfg5 holds
 }
-METRIC = "acquisition steps/sec (M=256,N=1e6,C=100)"
+METRIC = "acquisition steps/sec (M=256,N=5e5,C=100)"
 
 
 def parse():
@@ -62,12 +63,14 @@ def parse():
     ap.add_argument("--dense", action="store_true", help="worst-case synthetic slab (wrong class uniform)")
     ap.add_argument("--no-dense-extra", dest="dense_extra", action="store_false",
                     help="skip the dense worst-case slab that the N=1 run reports under modes.dense_slab")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the device loop returned in them as DIR/<name>.npy")
     return ap.parse_args()
 
 
 # ---------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason sampler running DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clock / throttle-reason sampler running DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -239,8 +242,8 @@ REFERENCE_BUDGET_S = 75.0     # wall-clock budget of all timed + warm-up samples
 
 
 def run_reference(args):
-    """--impl reference: the reference's CPU algorithm (oracle port; the Python reference cannot travel to
-    the GPU box) on this box's host cores.  Rank 0 only.  Whole run: set-up (~10-30 s) + <= REFERENCE_BUDGET_S."""
+    """--impl reference: the reference's CPU algorithm (oracle port; the Python reference is not part of this
+    project) on the host cores.  Rank 0 only.  Whole run: set-up (~10-30 s) + <= REFERENCE_BUDGET_S."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -318,6 +321,25 @@ def algorithmic_bytes(eng):
     }
 
 
+def dump_outputs(sel, out_dir, steps):
+    """What the timed device loop handed back, as .npy: the pick, its EIG and the isclose-tie flag of each timed step,
+    and after the last one the per-item EIG, P(best) and the best model (float32 / float64).  Written by rank 0: picks,
+    P(best) and the best model are global, the per-item EIG is rank 0's shard of the items (all of them on one GPU)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    idx, q, tie = sel.history()
+    out = {
+        "picks": idx[-steps:].astype(np.float64),
+        "pick_eig": q[-steps:].astype(np.float32),
+        "ties": tie[-steps:].astype(np.float32),
+        "eig": sel.eig.detach().cpu().numpy().astype(np.float32),
+        "pbest": sel.get_pbest().detach().cpu().numpy().astype(np.float32),
+        "best_model": np.asarray([int(sel.engine.best_model[0])], dtype=np.float64),
+    }
+    for name, arr in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
+
+
 def main():
     args = parse()
     if args.impl == "reference":
@@ -358,8 +380,9 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (6650.0, "fallback")
-    tf_peak = peaks.get("bf16_tflops_sustained", 1400.0)
+    # fallbacks: NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 dense BF16 TFLOP/s at 700 W)
+    hbm_peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (3350.0, "datasheet")
+    tf_peak = peaks.get("bf16_tflops_sustained", 989.0)
 
     def barrier():
         if world > 1:
@@ -475,13 +498,6 @@ def main():
                         algorithmic_flops_per_launch=flops)
         else:
             base.update(bound="hbm", achieved=None, peak=hbm_peak, unit="GB/s", frac=None)
-        try:    # measured DRAM traffic of the same kernel/config from the committed ncu capture (not measurable live)
-            tr = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic_r2.json")))
-            ent = tr.get(f"{args.workload}/{world}/{mode}", {}).get(base["kernel"])
-            if ent:
-                base["traffic"], base["traffic_source"] = ent, "profiles/r2_step_kernels_ncu.txt"
-        except Exception:
-            pass
         return base
 
     # ---- our arm -------------------------------------------------------------------------------------
@@ -492,6 +508,8 @@ def main():
     graph_loop.exchange = None
     ms, launches = graph_loop(sel, labels_dev, args.warmup, args.steps)
     exchange = graph_loop.exchange
+    if args.dump_outputs and rank == 0:
+        dump_outputs(sel, args.dump_outputs, args.steps)
     value = args.steps / (ms / 1e3)
     picks_dev = sel.history()[0][-(args.steps):].tolist()
     ties_dev = int(sel.history()[2].sum())
@@ -523,7 +541,7 @@ def main():
     kernels = kernel_table(prof)
 
     def marginals_full(eng):
-        """The construction / recompute_all pass (coda.py:227-229) on this shard: the tcgen05 kernel beside the fp32 SIMT
+        """The construction / recompute_all pass (coda.py:227-229) on this shard: the wgmma kernel beside the fp32 SIMT
         kernel, CUDA events around one launch each (U is rewritten with the same values the steps maintained)."""
         if eng.compact is not None or not eng._pi_tc:
             return None
@@ -592,7 +610,7 @@ def main():
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {
                 "workload": workload_string(args, wl, world),
-                "mode": info["mode"], "l2": "per-step working set (row cache + U + slab gather) >> 126 MB L2; no flush needed",
+                "mode": info["mode"], "l2": "per-step working set (row cache + U + slab gather) >> 50 MB L2; no flush needed",
                 "loop": "CUDA graph, one replay per step; shards exchange through peer memory inside the step kernels",
                 "tie_rule_value": "arg-max, first index (device loop); isclose ties in the timed run: %d" % ties_dev,
                 "tie_rule_e2e": "random.choice (coda.py:308)",

@@ -1,6 +1,6 @@
 """Drop-in ``coda`` package: the names the reference's drivers import (coda/__init__.py:1-3),
 served by ``coda_b200``.  Put this repository before the reference on PYTHONPATH and
-``main.py --method coda`` runs on the sm_100a kernels unchanged (see INTEGRATION.md)."""
+``main.py --method coda`` runs on the sm_90a kernels unchanged (see INTEGRATION.md)."""
 from coda_b200.selector import CODA
 from coda_b200.datasets import Dataset
 from coda_b200.oracle import Oracle

@@ -1,4 +1,4 @@
-"""coda_b200: the CODA active-model-selection acquisition hot path on B200 (sm_100a)."""
+"""coda_b200: the CODA active-model-selection acquisition hot path on H100 (sm_90a)."""
 import os as _os
 
 # Several shards driven by one process each use their own streams and wait for each other inside kernels: give every

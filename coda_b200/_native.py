@@ -1,7 +1,7 @@
 """ctypes binding of libcoda_b200.so (the C ABI in include/coda_b200.h).
 
 There is no CPU fallback: importing works anywhere (so the symbol table can be checked
-without a GPU), but every compute entry point needs an sm_100 device and ``require_device``
+without a GPU), but every compute entry point needs an sm_90 device and ``require_device``
 fails loudly without one.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library (sm_100a only) in-tree: coda_b200/lib/libcoda_b200.so."""
+"""Build the C-ABI shared library (sm_90a only) in-tree: coda_b200/lib/libcoda_b200.so."""
 from __future__ import annotations
 
 import hashlib
@@ -13,7 +13,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libcoda_b200.so")
 SOURCES = ["api.cu", "xchg.cu", "slab.cu", "tables.cu", "pairs.cu", "pairs_tc.cu", "pi_tc.cu", "gain.cu", "step.cu", "compact.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -69,7 +69,7 @@ def _build_locked(stamp, dig, verbose):
             sys.stderr.write(log[-1])
             raise RuntimeError(f"nvcc failed on {src}")
         objs.append(obj)
-    cmd = [_nvcc(), "-shared", "-o", tmp_lib, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [_nvcc(), "-shared", "-o", tmp_lib, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     log.append(f"$ {' '.join(cmd)}\n{r.stdout}{r.stderr}")
     if r.returncode != 0:

@@ -15,10 +15,10 @@ void coda_set_error(const char* fmt, ...) {
 int coda_sm_count() {
   static thread_local int cached_dev = -1, cached = 0;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev != cached_dev) {
     cudaDeviceProp p;
-    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 148;
+    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 132;
     cached = p.multiProcessorCount;
     cached_dev = dev;
   }
@@ -40,8 +40,8 @@ extern "C" int coda_b200_device_check(void) {
   CODA_CUDA_OK(cudaGetDevice(&dev));
   cudaDeviceProp p;
   CODA_CUDA_OK(cudaGetDeviceProperties(&p, dev));
-  if (p.major != 10) {
-    coda_set_error("device %d is sm_%d%d; this library is built for sm_100a only", dev, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    coda_set_error("device %d is sm_%d%d; this library is built for sm_90a only", dev, p.major, p.minor);
     return CODA_B200_ECUDA;
   }
   return CODA_B200_OK;

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the coda_b200 kernels (sm_100a only).
+// Shared device/host helpers for the coda_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -133,6 +133,21 @@ __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src
           smem_u32(smem_dst)),
       "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
+}
+
+// ---- Hopper warpgroup MMA (wgmma) ---------------------------------------------------------------
+// Shared-memory matrix descriptor, no swizzle (layout type 0), K-major: the operand is stored as 8-row x 16-byte core
+// matrices; LBO = byte distance between core matrices adjacent along K, SBO = between core matrices adjacent along M / N.
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// generic-proxy shared-memory stores -> visible to wgmma / bulk copies (async proxy)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // ---- arg-max records ---------------------------------------------------------------------------

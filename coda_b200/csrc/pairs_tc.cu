@@ -1,19 +1,21 @@
-// pair_rows on the 5th-generation tensor cores (tcgen05 + TMEM), for Hp = 32..256 models.
+// pair_rows on the Hopper tensor cores (wgmma, fp32 accumulators in registers), for Hp = 32..256 models.
 //
 // Same arithmetic as k_pair_rows (pairs.cu) for a tile of 128 same-class pairs, cast as two GEMMs:
 //
 //   phase A   logD[128 x 256] = Z[128 x Hp] . dL_c[Hp x 256]             K = Hp (models)
 //             Z in {0,1} is exact in bf16; dL is split into 3 bf16 limbs (24 mantissa bits) -> 3 MMAs
-//   epilogue  D = exp(logD)  (TMEM -> registers -> exp -> two bf16 limbs -> shared memory, A-operand layout)
+//   epilogue  D = exp(logD)  (registers -> exp -> two bf16 limbs -> shared memory, A-operand layout)
 //   phase B   prob_k[128 x Hp] = D[128 x 256] . G_k[256 x Hp],  k = miss, hit    K = 256 (quadrature nodes)
 //             D = Dhi + Dlo, G = Ghi + Glo (bf16 limbs); Dhi.Ghi + Dhi.Glo + Dlo.Ghi -> 3 MMAs per table
-//   epilogue  thread <-> pair (TMEM lane): select hit/miss column by the pair's mask bit, normalise over
-//             models (coda.py:114), information gain (coda.py:274-276), cached row write.
+//   epilogue  select hit/miss column by the pair's mask bit, normalise over models (coda.py:114), information gain
+//             (coda.py:274-276), cached row write.
 //
-// Operands are staged by 1-D bulk TMA (cp.async.bulk, no tensor map): the class tables are stored in HBM
-// already in the UMMA "no-swizzle, K-major" core-matrix order (8 rows x 16 bytes per core, see tables.cu), so
-// one K-chunk of all limbs is a single contiguous blob.  Accumulators live in TMEM (512 columns: logD / prob
-// miss in [0,256), prob hit in [256,512)); one CTA per SM, 128 threads, one elected thread issues TMA + MMA.
+// Two consumer warpgroups, one per 64 pairs of the tile; every MMA is a wgmma m64n32k16 (one 32-model / 32-node column
+// block; 32 models are also one word of the pair's mask).  Operands are staged by 1-D bulk TMA (cp.async.bulk, no tensor
+// map): the class tables are stored in HBM already in the no-swizzle K-major core-matrix order (8 rows x 16 bytes per
+// core, see tables.cu), so one K-chunk of all limbs is a single contiguous blob.  The accumulators of phase B for both
+// tables over all Hp columns would not fit the register file at Hp > 128, so phase B then runs in two passes over
+// column halves (the G stream is read twice; it is per class and stays in L2 across the class's tiles).
 #include "common.cuh"
 
 #include <cuda_bf16.h>
@@ -25,9 +27,9 @@ constexpr int TC_NODES = 256;    // quadrature nodes
 constexpr int KA = 32;           // models per phase-A chunk
 constexpr int KB = 16;           // nodes per phase-B chunk
 constexpr int STAGES_A = 3;
-constexpr int TC_THREADS = 512;   // 16 warps: warp w works on TMEM lane quadrant w % 4 (hardware rule) and column part w / 4
-constexpr int TC_PARTS = TC_THREADS / 128;
 constexpr int STAGES_B = 3;
+constexpr int TC_THREADS = 256;  // 2 warpgroups x 64 pairs
+constexpr int NBMAX = 4;         // 32-column blocks per phase-B pass
 
 struct TcArgs {
   const int4* tiles;             // (class, first pid, count <= 128, unused)
@@ -46,53 +48,18 @@ struct TcArgs {
   int H, Hp, W;
 };
 
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // cute::UMMA::SmemDescriptor (mma_sm100_desc.hpp): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
-  // version = 1 [46,48), layout_type = SWIZZLE_NONE (0) [61,64)
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         (1ull << 46);
-}
-
-__device__ __forceinline__ uint32_t instr_desc_bf16(int n) {
-  // cute::UMMA::InstrDescriptor: c_format F32 (1) [4,6), a/b_format BF16 (1) [7,10) [10,13), K-major both,
-  // n_dim = N >> 3 [17,23), m_dim = M >> 4 [24,29)
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-}
-
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// D[64 x 32] (+)= A[64 x 16] . B[16 x 32]^T, both operands bf16 in shared memory (K-major), fp32 accumulators
+__device__ __forceinline__ void mma_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
 }
 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
@@ -105,12 +72,16 @@ __device__ __forceinline__ uint32_t core_off(int r, int k, int rows) {
   return (uint32_t)(((k >> 3) * (rows >> 3) + (r >> 3)) * 128 + (r & 7) * 16 + (k & 7) * 2);
 }
 
+// accumulator fragment of wgmma m64nN (fp32): register 4 j + 2 i + e holds row (16 warp + lane / 4 + 8 i),
+// column (8 j + 2 (lane % 4) + e)
+__device__ __forceinline__ int frag_col(int j, int e, int lane) { return 8 * j + 2 * (lane & 3) + e; }
+
 __global__ void __launch_bounds__(TC_THREADS, 1) k_pair_rows_tc(TcArgs a, int tile0) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int H = a.H, Hp = a.Hp, W = a.W;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int quad = warp & 3, half = warp >> 2;      // TMEM lane quadrant (hardware: warp % 4), column part 0..TC_PARTS-1
-  const int row = quad * 32 + lane;                 // this thread's pair within the tile
+  const int wg = warp >> 2;                                   // warpgroup: pairs [64 wg, 64 wg + 64)
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // this thread's two pairs: r0 and r0 + 8
   if (a.sel) {
     const long long t = a.sel[1];
     tile0 = (int)a.tile_off[t];
@@ -124,44 +95,44 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_pair_rows_tc(TcArgs a, int ti
   // [64K, 208K)        phase A: 3 stages x 48K (3 limbs x 256 x KA bf16)
   // [64K, 128K)                                                 | phase B: D lo
   // [128K, 224K)                                                | phase B: 3 stages x 32K (4 tables x Hp x KB)
-  // tail               barriers, TMEM base, m0 / PB rows
+  // tail               barriers, m0 / PB rows
   unsigned char* opA = smem;
   unsigned char* stg = smem + 128 * 1024;
+  unsigned char* stgA = smem + 64 * 1024;
   unsigned char* tail = stg + 96 * 1024;
   uint64_t* fullA = reinterpret_cast<uint64_t*>(tail);        // [STAGES_A]
   uint64_t* emptyA = fullA + STAGES_A;                        // [STAGES_A]
   uint64_t* fullB = emptyA + STAGES_A;                        // [STAGES_B]
   uint64_t* emptyB = fullB + STAGES_B;                        // [STAGES_B]
-  uint64_t* doneA = emptyB + STAGES_B;
-  uint64_t* doneB = doneA + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(doneB + 1);
-  float* m0s = reinterpret_cast<float*>(tmem_slot + 2);       // [Hp]
+  float* m0s = reinterpret_cast<float*>(emptyB + STAGES_B + 2);   // [Hp]
   float* pbs = m0s + Hp;                                      // [Hp]
-  float* xsum = reinterpret_cast<float*>(stg);                // [TC_PARTS][128] row-sum parts  (stage region: idle in epilogue B)
-  float* xgain = xsum + TC_PARTS * TC_M;                      // [TC_PARTS][128] gain parts
-  unsigned char* stgA = smem + 64 * 1024;
+
+  const int nka = Hp / KA;                       // phase-A chunks
+  constexpr int nkb = TC_NODES / KB;             // phase-B chunks per pass
+  const int nblk = Hp / 32;                      // 32-model column blocks
+  const int npass = nblk > NBMAX ? 2 : 1;
+  const int nb0 = (nblk + npass - 1) / npass;    // blocks of pass 0 (pass 1 takes the rest)
+  const int nqb = npass * nkb;                   // phase-B chunks over all passes
+  const uint32_t bytesA = 3u * TC_NODES * KA * 2u;          // per stage
+  const uint32_t tabB = (uint32_t)Hp * KB * 2u;             // one table, one chunk
+  const uint32_t bytesB = 4u * tabB;
+  const unsigned char* srcA = reinterpret_cast<const unsigned char*>(a.dLb) + (size_t)c * nka * bytesA;
+  const unsigned char* srcB = reinterpret_cast<const unsigned char*>(a.Gb) + (size_t)c * nkb * bytesB;
 
   if (tid == 0) {
-    for (int i = 0; i < STAGES_A; ++i) { mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], 1); }
-    for (int i = 0; i < STAGES_B; ++i) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 1); }
-    mbar_init(doneA, 1);
-    mbar_init(doneB, 1);
+    for (int i = 0; i < STAGES_A; ++i) { mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], TC_THREADS / 32); }
+    for (int i = 0; i < STAGES_B; ++i) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], TC_THREADS / 32); }
     mbar_fence_init();
-  }
-  if (warp == 0) {   // TMEM: all 512 columns (one CTA per SM)
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   const bool want_gain = a.gain != nullptr;
   for (int h = tid; h < Hp; h += TC_THREADS) {
     m0s[h] = (want_gain && h < H) ? a.m0[h] : 0.f;
     pbs[h] = a.PB[(size_t)c * Hp + h];
   }
-  // ---- Z operand: row = this thread's pair, K = models, bf16 {0, 1} ----------------------------
+  // ---- Z operand: row = pair, K = models, bf16 {0, 1} ------------------------------------------
 #pragma unroll 1
-  for (int w = half; w < W; w += TC_PARTS) {       // rolled: one copy of the body instead of eight (instruction cache)
+  for (int i = tid; i < TC_M * W; i += TC_THREADS) {
+    const int row = i % TC_M, w = i / TC_M;
     const uint32_t z = row < cnt ? a.zmask[(size_t)(pid0 + row) * W + w] : 0u;
 #pragma unroll
     for (int q = 0; q < 4; ++q) {   // 8 models -> one 16-byte core row
@@ -174,211 +145,204 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_pair_rows_tc(TcArgs a, int ti
       *reinterpret_cast<uint4*>(opA + core_off(row, w * 32 + q * 8, TC_M)) = v;
     }
   }
-  fence_proxy_async();
-  tc_fence_before();
+  fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  if (tid == 0) {
+    for (int kc = 0; kc < STAGES_A && kc < nka; ++kc) {
+      mbar_expect_tx(&fullA[kc], bytesA);
+      tma_load_1d(stgA + (size_t)kc * 48 * 1024, srcA + (size_t)kc * bytesA, bytesA, &fullA[kc]);
+    }
+  }
   const uint32_t opA_s = smem_u32(opA), stg_s = smem_u32(stg), stgA_s = smem_u32(stgA);
-  const int nka = Hp / KA;                       // phase-A chunks
-  constexpr int nkb = TC_NODES / KB;             // phase-B chunks
-  const uint32_t bytesA = 3u * TC_NODES * KA * 2u;          // per stage
-  const uint32_t tabB = (uint32_t)Hp * KB * 2u;             // one table, one chunk
-  const uint32_t bytesB = 4u * tabB;
+  const uint32_t a_rows = (uint32_t)(wg * 8) * 128;          // this warpgroup's 8 row cores
+  constexpr uint32_t LBO_A = (TC_M / 8) * 128;
 
   // ---- phase A: logD = Z . dL (3 limbs) --------------------------------------------------------
-  // Two elected threads: tid 32 streams the operand chunks (it only ever waits for a stage to be released), tid 0 issues
-  // the MMAs (it only ever waits for a stage to be filled) -- so the tensor pipe is never held up by a TMA issue
-  // waiting for the previous chunk's MMAs to retire, and all STAGES_A stages are in flight.
-  if (tid == 32) {
-    const unsigned char* src = reinterpret_cast<const unsigned char*>(a.dLb) + (size_t)c * nka * bytesA;
-    for (int kc = 0; kc < nka; ++kc) {
-      const int s = kc % STAGES_A;
-      if (kc >= STAGES_A) mbar_wait(&emptyA[s], ((kc / STAGES_A) - 1) & 1);
-      mbar_expect_tx(&fullA[s], bytesA);
-      tma_load_1d(stgA + (size_t)s * 48 * 1024, src + (size_t)kc * bytesA, bytesA, &fullA[s]);
+  // Thread 0 refills the stage of chunk kc - 1 once both warpgroups have released it, STAGES_A - 1 chunks ahead.
+  float acc[2][NBMAX][16];        // phase A: acc[b / 4][b % 4] = node block b; phase B: acc[table][block]
+  for (int kc = 0; kc < nka; ++kc) {
+    const int s = kc % STAGES_A;
+    if (tid == 0 && kc >= 1 && kc - 1 + STAGES_A < nka) {
+      const int q = kc - 1 + STAGES_A, sq = q % STAGES_A;
+      mbar_wait(&emptyA[sq], ((kc - 1) / STAGES_A) & 1);
+      mbar_expect_tx(&fullA[sq], bytesA);
+      tma_load_1d(stgA + (size_t)sq * 48 * 1024, srcA + (size_t)q * bytesA, bytesA, &fullA[sq]);
     }
-    // prefetch the first phase-B stages while the epilogue below runs (their smem region is free once the
-    // phase-A MMAs have completed, which doneA certifies)
-    mbar_wait(doneA, 0);
-    const unsigned char* srcB = reinterpret_cast<const unsigned char*>(a.Gb) + (size_t)c * nkb * bytesB;
-    for (int kc = 0; kc < STAGES_B && kc < nkb; ++kc) {
-      mbar_expect_tx(&fullB[kc], bytesB);
-      tma_load_1d(stg + (size_t)kc * 32 * 1024, srcB + (size_t)kc * bytesB, bytesB, &fullB[kc]);
-    }
-  }
-  if (tid == 0) {
-    const uint32_t idesc = instr_desc_bf16(TC_NODES);
-    for (int kc = 0; kc < nka; ++kc) {
-      const int s = kc % STAGES_A;
-      mbar_wait(&fullA[s], (kc / STAGES_A) & 1);
-      tc_fence_after();
+    __syncwarp();
+    mbar_wait(&fullA[s], (kc / STAGES_A) & 1);
+    wg_fence();
 #pragma unroll
-      for (int limb = 0; limb < 3; ++limb) {
+    for (int limb = 0; limb < 3; ++limb) {
 #pragma unroll
-        for (int ks = 0; ks < KA / 16; ++ks) {
-          // A: Z tile [k_core][16 r_core]: LBO = 16 * 128, advance 2 k-cores per K=16 step
-          const uint64_t ad = smem_desc(opA_s + (uint32_t)(kc * (KA / 8) + ks * 2) * (TC_M / 8) * 128, (TC_M / 8) * 128, 128);
-          // B: limb tile [4 k_core][32 r_core]: LBO = 32 * 128
-          const uint64_t bd = smem_desc(stgA_s + (uint32_t)s * 48 * 1024 + (uint32_t)limb * (TC_NODES * KA * 2) +
-                                            (uint32_t)(ks * 2) * (TC_NODES / 8) * 128,
-                                        (TC_NODES / 8) * 128, 128);
-          mma_bf16(tmem, ad, bd, idesc, (kc | limb | ks) ? 1u : 0u);
-        }
+      for (int ks = 0; ks < KA / 16; ++ks) {
+        // A: Z tile [k_core][16 r_core], this warpgroup's rows; advance 2 k-cores per K = 16 step
+        const uint64_t ad = wg_desc(opA_s + (uint32_t)(kc * (KA / 8) + ks * 2) * LBO_A + a_rows, LBO_A, 128);
+        const uint32_t bb = stgA_s + (uint32_t)s * 48 * 1024 + (uint32_t)limb * (TC_NODES * KA * 2) +
+                            (uint32_t)(ks * 2) * (TC_NODES / 8) * 128;
+        const uint32_t first = (kc | limb | ks) ? 1u : 0u;
+#pragma unroll
+        for (int b = 0; b < TC_NODES / 32; ++b)   // B: limb tile [4 k_core][32 r_core], 32-node block b
+          mma_n32(acc[b >> 2][b & 3], ad, wg_desc(bb + (uint32_t)b * 4 * 128, (TC_NODES / 8) * 128, 128), first);
       }
-      mma_commit(&emptyA[s]);
     }
-    mma_commit(doneA);
+    wg_commit();
+    wg_wait0();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&emptyA[s]);
   }
-  __syncwarp();
-  mbar_wait(doneA, 0);
-  tc_fence_after();
+  __syncthreads();                               // every phase-A read is done: D lo and the phase-B stages may land
+
+  if (tid == 0) {
+    for (int q = 0; q < STAGES_B && q < nqb; ++q) {
+      mbar_expect_tx(&fullB[q], bytesB);
+      tma_load_1d(stg + (size_t)q * 32 * 1024, srcB + (size_t)(q % nkb) * bytesB, bytesB, &fullB[q]);
+    }
+  }
 
   // ---- epilogue A: D = exp(logD) -> bf16 hi / lo limbs in the A-operand layout ---------------------
   {
     unsigned char* dhi = opA;
     unsigned char* dlo = opA + 64 * 1024;
-    const uint32_t trow = tmem + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-    for (int cc = half * (TC_NODES / 32 / TC_PARTS); cc < (half + 1) * (TC_NODES / 32 / TC_PARTS); ++cc) {
-      float v[32];
-      tmem_ld32(trow + cc * 32, v);
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t hi[4], lo[4];
+    for (int b = 0; b < TC_NODES / 32; ++b) {
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float d0 = __expf(v[g * 8 + 2 * e]), d1 = __expf(v[g * 8 + 2 * e + 1]);   // ex2.approx: 2 ulp, far inside the 16-bit limb pair D is cut into
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float* v = &acc[b >> 2][b & 3][4 * j + 2 * i];
+          const float d0 = __expf(v[0]), d1 = __expf(v[1]);   // ex2.approx: 2 ulp, far inside the 16-bit limb pair D is cut into
           const __nv_bfloat16 h0 = __float2bfloat16_rn(d0), h1 = __float2bfloat16_rn(d1);
-          hi[e] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-          lo[e] = pack_bf16(d0 - __bfloat162float(h0), d1 - __bfloat162float(h1));
+          const uint32_t hi = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
+          const uint32_t lo = pack_bf16(d0 - __bfloat162float(h0), d1 - __bfloat162float(h1));
+          const uint32_t off = core_off(r0 + 8 * i, b * 32 + frag_col(j, 0, lane), TC_M);
+          *reinterpret_cast<uint32_t*>(dhi + off) = hi;
+          *reinterpret_cast<uint32_t*>(dlo + off) = lo;
         }
-        const uint32_t off = core_off(row, cc * 32 + g * 8, TC_M);
-        *reinterpret_cast<uint4*>(dhi + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(dlo + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
       }
     }
   }
-  fence_proxy_async();
-  tc_fence_before();
+  fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
 
-  // ---- phase B: prob_k = D . G_k -----------------------------------------------------------------
-  if (tid == 32) {                                // the chunks beyond the STAGES_B prefetched above
-    const unsigned char* srcB = reinterpret_cast<const unsigned char*>(a.Gb) + (size_t)c * nkb * bytesB;
-    for (int kc = STAGES_B; kc < nkb; ++kc) {
-      const int s = kc % STAGES_B;
-      mbar_wait(&emptyB[s], ((kc / STAGES_B) - 1) & 1);
-      mbar_expect_tx(&fullB[s], bytesB);
-      tma_load_1d(stg + (size_t)s * 32 * 1024, srcB + (size_t)kc * bytesB, bytesB, &fullB[s]);
-    }
-  }
-  if (tid == 0) {
-    const uint32_t idesc = instr_desc_bf16(Hp);
-    const uint32_t lboB = (uint32_t)(Hp / 8) * 128;
+  // ---- phase B: prob_k = D . G_k, one pass per column half --------------------------------------------
+  float keep[NBMAX][16];          // selected probabilities of pass 0 when there are two passes
+  float sum[2] = {0.f, 0.f};      // row sums of rows r0, r0 + 8 (this thread's columns)
+  const uint32_t lboB = (uint32_t)(Hp / 8) * 128;
+  for (int pass = 0; pass < npass; ++pass) {
+    const int blo = pass * nb0, nbp = min(nblk - blo, nb0);
     for (int kc = 0; kc < nkb; ++kc) {
-      const int s = kc % STAGES_B;
-      mbar_wait(&fullB[s], (kc / STAGES_B) & 1);
-      tc_fence_after();
-      const uint64_t ahi = smem_desc(opA_s + (uint32_t)(kc * 2) * (TC_M / 8) * 128, (TC_M / 8) * 128, 128);
-      const uint64_t alo = smem_desc(opA_s + 64 * 1024 + (uint32_t)(kc * 2) * (TC_M / 8) * 128, (TC_M / 8) * 128, 128);
-      const uint32_t sb = stg_s + (uint32_t)s * 32 * 1024;
+      const int q = pass * nkb + kc, s = q % STAGES_B;
+      if (tid == 0 && q >= 1 && q - 1 + STAGES_B < nqb) {
+        const int qn = q - 1 + STAGES_B, sn = qn % STAGES_B;
+        mbar_wait(&emptyB[sn], ((q - 1) / STAGES_B) & 1);
+        mbar_expect_tx(&fullB[sn], bytesB);
+        tma_load_1d(stg + (size_t)sn * 32 * 1024, srcB + (size_t)(qn % nkb) * bytesB, bytesB, &fullB[sn]);
+      }
+      __syncwarp();
+      mbar_wait(&fullB[s], (q / STAGES_B) & 1);
+      wg_fence();
+      const uint64_t ahi = wg_desc(opA_s + (uint32_t)(kc * 2) * LBO_A + a_rows, LBO_A, 128);
+      const uint64_t alo = wg_desc(opA_s + 64 * 1024 + (uint32_t)(kc * 2) * LBO_A + a_rows, LBO_A, 128);
+      const uint32_t sb = stg_s + (uint32_t)s * 32 * 1024 + (uint32_t)blo * 4 * 128;
+      const uint32_t first = kc ? 1u : 0u;
 #pragma unroll
       for (int k = 0; k < 2; ++k) {              // k = 0 miss table (G0), 1 hit table (G1)
-        const uint64_t ghi = smem_desc(sb + (uint32_t)(2 * k) * tabB, lboB, 128);
-        const uint64_t glo = smem_desc(sb + (uint32_t)(2 * k + 1) * tabB, lboB, 128);
-        const uint32_t acc = tmem + (uint32_t)k * 256;
-        mma_bf16(acc, ahi, ghi, idesc, kc ? 1u : 0u);
-        mma_bf16(acc, ahi, glo, idesc, 1u);
-        mma_bf16(acc, alo, ghi, idesc, 1u);
-      }
-      mma_commit(&emptyB[s]);
-    }
-    mma_commit(doneB);
-  }
-  __syncwarp();
-  mbar_wait(doneB, 0);
-  tc_fence_after();
-
-  // ---- epilogue B: (pair, column half) per thread ---------------------------------------------------
-  {
-    const uint32_t trow = tmem + ((uint32_t)(quad * 32) << 16);
-    const int nch = Hp / 32;
-    const int per_part = (nch + TC_PARTS - 1) / TC_PARTS;
-    const int ch_lo = min(nch, half * per_part), ch_hi = min(nch, (half + 1) * per_part);
-    // The chunk loops stay ROLLED: unrolled eight ways (one copy per possible chunk, each warp running two of them) the
-    // epilogue was 10 000 SASS lines = 160 KB, and ncu attributed 43 % of the kernel to it with instruction-fetch stalls
-    // (stall_no_inst) on top.  The mask words of this thread's (at most two) chunks are re-read (L1 hits).
-    uint32_t zsel[2] = {0u, 0u};
-    if (row < cnt) {
-      if (ch_lo < ch_hi) zsel[0] = a.zmask[(size_t)(pid0 + row) * W + ch_lo];
-      if (ch_lo + 1 < ch_hi) zsel[1] = a.zmask[(size_t)(pid0 + row) * W + ch_lo + 1];
-    }
-    float sum = 0.f;
-#pragma unroll 1
-    for (int ch = ch_lo; ch < ch_hi; ++ch) {
-      float p0[32], p1[32];
-      tmem_ld32(trow + ch * 32, p0);
-      tmem_ld32(trow + 256 + ch * 32, p1);
-      const uint32_t zb = (ch == ch_lo) ? zsel[0] : zsel[1];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) sum += ((zb >> i) & 1u) ? p1[i] : p0[i];
-    }
-    xsum[half * TC_M + row] = sum;
-    __syncthreads();
-    sum = 0.f;
-#pragma unroll
-    for (int q = 0; q < TC_PARTS; ++q) sum += xsum[q * TC_M + row];
-    uint32_t bad = 0;
-    if (row < cnt && half == 0 && !isfinite(sum)) bad = CODA_B200_FLAG_NONFINITE_EIG;
-    const float rden = 1.0f / fmaxf(sum, 1e-30f);                    // coda.py:114
-    const float pic = want_gain ? a.pi_hat[c] : 0.f;
-    float g = 0.f;
-    const int orow = row < cnt ? a.row_of[pid0 + row] : 0;
-    if (row < cnt && half == 0 && sum < 0.9999e-30f) bad |= CODA_B200_FLAG_ROWSUM_WARN;    // util.py:37-39
-    float* cache = (a.ph_cache && row < cnt) ? a.ph_cache + (size_t)orow * Hp : nullptr;
-#pragma unroll 1
-    for (int ch = ch_lo; ch < ch_hi; ++ch) {
-      float p0[32], p1[32];
-      tmem_ld32(trow + ch * 32, p0);
-      tmem_ld32(trow + 256 + ch * 32, p1);
-      const uint32_t zb = (ch == ch_lo) ? zsel[0] : zsel[1];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int h = ch * 32 + i;
-        float ph = (((zb >> i) & 1u) ? p1[i] : p0[i]) * rden;
-        if (h >= H) ph = 0.f;
-        if (ph < -1e-12f) bad |= CODA_B200_FLAG_NEGATIVE_PROB;          // util.py:33-35
-        p0[i] = ph;
-        if (want_gain && h < H) {
-          const float m = m0s[h];
-          g += ent_term(m) - ent_term(m + pic * (ph - pbs[h]));      // coda.py:254, 274-276
+        for (int b = 0; b < NBMAX; ++b) {
+          if (b < nbp) {                         // warp-uniform
+            const uint64_t ghi = wg_desc(sb + (uint32_t)(2 * k) * tabB + (uint32_t)b * 4 * 128, lboB, 128);
+            const uint64_t glo = wg_desc(sb + (uint32_t)(2 * k + 1) * tabB + (uint32_t)b * 4 * 128, lboB, 128);
+            mma_n32(acc[k][b], ahi, ghi, first);
+            mma_n32(acc[k][b], ahi, glo, 1u);
+            mma_n32(acc[k][b], alo, ghi, 1u);
+          }
         }
       }
-      if (cache) {
+      wg_commit();
+      wg_wait0();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&emptyB[s]);
+    }
+    // select hit / miss by the pair's mask bit; the selection lands in keep (pass 0 of two) or acc[0] (last pass)
 #pragma unroll
-        for (int i = 0; i < 32; i += 4)
-          *reinterpret_cast<float4*>(cache + ch * 32 + i) = make_float4(p0[i], p0[i + 1], p0[i + 2], p0[i + 3]);
+    for (int b = 0; b < NBMAX; ++b) {
+      if (b < nbp) {
+        uint32_t z[2];                           // mask words (32 models) of both rows for this block
+#pragma unroll
+        for (int i = 0; i < 2; ++i) z[i] = r0 + 8 * i < cnt ? a.zmask[(size_t)(pid0 + r0 + 8 * i) * W + blo + b] : 0u;
+#pragma unroll
+        for (int r = 0; r < 16; ++r) {
+          const int i = (r >> 1) & 1, col = frag_col(r >> 2, r & 1, lane);
+          const float v = ((z[i] >> col) & 1u) ? acc[1][b][r] : acc[0][b][r];
+          sum[i] += v;
+          if (pass + 1 < npass) keep[b][r] = v;
+          else acc[0][b][r] = v;
+        }
       }
     }
-    if (want_gain) {
-      xgain[half * TC_M + row] = g;
-      __syncthreads();
-      if (half == 0 && row < cnt) {
-        float gs = 0.f;
+  }
+
+  // ---- epilogue B: normalise, gain, cached rows --------------------------------------------------
 #pragma unroll
-        for (int q = 0; q < TC_PARTS; ++q) gs += xgain[q * TC_M + row];
-        a.gain[orow] = gs;
+  for (int i = 0; i < 2; ++i) {
+    sum[i] += __shfl_xor_sync(CODA_FULL, sum[i], 1);
+    sum[i] += __shfl_xor_sync(CODA_FULL, sum[i], 2);
+  }
+  const float pic = want_gain ? a.pi_hat[c] : 0.f;
+  uint32_t bad = 0;
+  float g[2] = {0.f, 0.f};
+  int orow[2];
+  float* cache[2];
+  float rden[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = r0 + 8 * i;
+    orow[i] = row < cnt ? a.row_of[pid0 + row] : 0;
+    cache[i] = (a.ph_cache && row < cnt) ? a.ph_cache + (size_t)orow[i] * Hp : nullptr;
+    rden[i] = 1.0f / fmaxf(sum[i], 1e-30f);                       // coda.py:114
+    if (row < cnt && (lane & 3) == 0) {
+      if (!isfinite(sum[i])) bad |= CODA_B200_FLAG_NONFINITE_EIG;
+      if (sum[i] < 0.9999e-30f) bad |= CODA_B200_FLAG_ROWSUM_WARN;   // util.py:37-39
+    }
+  }
+#pragma unroll
+  for (int pass = 0; pass < 2; ++pass) {
+    if (pass < npass) {
+      const int blo = pass * nb0, nbp = min(nblk - blo, nb0);
+#pragma unroll
+      for (int b = 0; b < NBMAX; ++b) {
+        if (b < nbp) {
+#pragma unroll
+          for (int r = 0; r < 16; r += 2) {
+            const int i = (r >> 1) & 1;
+            const int h0 = (blo + b) * 32 + frag_col(r >> 2, 0, lane);
+            float ph[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int h = h0 + e;
+              const float v = (pass + 1 < npass) ? keep[b][r + e] : acc[0][b][r + e];
+              ph[e] = h < H ? v * rden[i] : 0.f;
+              if (ph[e] < -1e-12f) bad |= CODA_B200_FLAG_NEGATIVE_PROB;          // util.py:33-35
+              if (want_gain && h < H) {
+                const float m = m0s[h];
+                g[i] += ent_term(m) - ent_term(m + pic * (ph[e] - pbs[h]));      // coda.py:254, 274-276
+              }
+            }
+            if (cache[i]) *reinterpret_cast<float2*>(cache[i] + h0) = make_float2(ph[0], ph[1]);
+          }
+        }
       }
     }
-    if (bad) atomicOr(a.flags, bad);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+  if (want_gain) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      g[i] += __shfl_xor_sync(CODA_FULL, g[i], 1);
+      g[i] += __shfl_xor_sync(CODA_FULL, g[i], 2);
+      if ((lane & 3) == 0 && r0 + 8 * i < cnt) a.gain[orow[i]] = g[i];
+    }
   }
+  if (bad) atomicOr(a.flags, bad);
 }
 
 }  // namespace

@@ -1,8 +1,9 @@
-// pi_full on the 5th-generation tensor cores:  U[n][c] = sum_h sum_s preds[h][n][s] * D[h][c][s]   (coda.py:227-229)
+// pi_full on the Hopper tensor cores (wgmma):  U[n][c] = sum_h sum_s preds[h][n][s] * D[h][c][s]   (coda.py:227-229)
 //
-// A skinny GEMM: M = N items, N = C classes, K = H*C.  One CTA owns a tile of 128 items and walks the H models; per model
-// the 128 x C block of the slab is ONE contiguous blob (51 KB at C = 100), fetched by four 1-D bulk TMA copies.  fp32 does
-// not go through tcgen05, so both operands are cut into two fp16 limbs, x = hi + 2^-12 lo  (11 + 11 significant bits: 2^-22
+// A skinny GEMM: M = N items, N = C classes, K = H*C.  One CTA owns a tile of 128 items (64 when C is too large for two
+// such stages in shared memory) and walks the H models; per model the tile's block of the slab is ONE contiguous blob
+// (51 KB at C = 100), fetched by one 1-D bulk TMA copy together with the model's D limbs.  fp32 does not go through the
+// tensor cores, so both operands are cut into two fp16 limbs, x = hi + 2^-12 lo  (11 + 11 significant bits: 2^-22
 // relative at worst, a quarter of an fp32 ulp on average; lo is stored scaled so that it stays a normal fp16 number),
 // and three products are formed per K = 16 chunk:
 //
@@ -11,20 +12,15 @@
 //
 // preds lie in [0, 1]; D (Dirichlet parameters) is multiplied by a power of two chosen from max |D| so that it stays
 // inside the fp16 range, and U is scaled back at the end (exact).  The tensor core accumulates in fp32 with truncation,
-// which biases a long chain of positive terms; so the two TMEM accumulators are drained every G (= 4) models into fp32
-// registers (round-to-nearest adds) by dedicated warps, double-buffered so the drain of one group overlaps the MMAs of
-// the next.  Against an fp64 contraction the result is closer than the 25 600-term fp32 FMA chain of the SIMT kernel
-// (slab.cu: k_pi_full), see tests/test_gpu_parity.py::test_tensor_core_marginals_match_fp64.
+// which biases a long chain of positive terms; so the two accumulators are folded every G (= 4) models into fp32
+// registers (round-to-nearest adds) and restarted.  Against an fp64 contraction the result is closer than the
+// 25 600-term fp32 FMA chain of the SIMT kernel (slab.cu: k_pi_full), see
+// tests/test_gpu_parity.py::test_tensor_core_marginals_match_fp64.
 //
-// Roles (1024 threads x 64 registers, one CTA per SM):
-//   warp 0 lane 0     slab producer     bulk TMA of (model, 32-item quarter) fp32 blocks into a staging ring
-//   warp 1 lane 0     D producer        bulk TMA of the D limbs (pre-packed by k_pi_w_limbs), one K chunk per ring slot
-//   warp 2            MMA issuer        per chunk A_hi . [D_hi | D_lo] (N = 2 Np: main | corr) and A_lo . D_hi (N = Np, into corr),
-//                                       one tcgen05.commit per chunk frees its A and D slots
-//   warps 4..19       drain             tcgen05.ld of both accumulators every G models, final store of U
-//   warps 20..31      converters        fp32 staging -> fp16 hi / lo limbs in the UMMA K-major core-matrix order
-// The kernel lives on bytes in flight: every (tile, model) pulls 51 KB of slab from HBM and 50 KB of D limbs from L2, so
-// shared memory is split between the fp32 staging ring and a deep D ring; the converted A chunks only need a short ring.
+// Each warpgroup owns 64 items.  The A limbs never touch shared memory: every thread converts the fp32 slab values of
+// its own wgmma A fragment (2 items x 4 classes of the chunk) to fp16 limbs in registers.  B (the D limbs, pre-packed by
+// k_pi_w_limbs in the K-major core-matrix order) is read by wgmma straight from the staged blob, in 16-class blocks.
+// Thread 0 refills the stage of model h - 1 with model h - 1 + S once both warpgroups have released it.
 // Every wait is bounded: a pipeline that stops sets CODA_B200_FLAG_PIPELINE_TIMEOUT and the kernel drains out.
 #include "common.cuh"
 
@@ -33,20 +29,13 @@
 
 namespace {
 
-constexpr int PT_M = 128;                 // items per tile
-constexpr int PT_THREADS = 1024;          // 32 warps x 64 registers: the whole register file
-constexpr int PT_DRAIN_WARP0 = 4, PT_DRAIN_WARPS = 16;   // 4 lane quadrants x 4 column parts (<= 32 accumulator registers each)
-constexpr int PT_DRAIN_PARTS = PT_DRAIN_WARPS / 4;
-constexpr int PT_CONV_WARP0 = 20, PT_CONV_WARPS = 12;
-constexpr int PT_WARPS_PER_CHUNK = 4;     // converter warps that share one K chunk (32 items each)
-constexpr int PT_CONV_GROUPS = PT_CONV_WARPS / PT_WARPS_PER_CHUNK;
-constexpr int PT_HALF = PT_M / PT_WARPS_PER_CHUNK;   // items per staging unit: one converter warp's share of a chunk
-constexpr int PT_MAX_STAGES = 12;         // staging units
-constexpr int PT_MAX_DSLOTS = 16;         // D chunks in flight (<= PT_CHUNK_BARS)
-constexpr int PT_CHUNK_BARS = 16;         // per-chunk barriers, indexed by chunk number & 15 (power of two)
-constexpr int PT_NBAR = 2 * PT_MAX_STAGES + 2 * PT_CHUNK_BARS + 4;
+constexpr int PT_WG = 64;                 // items per warpgroup
+constexpr int PT_MAXB = 8;                // 16-class blocks (Np <= 128)
+constexpr int PT_MAX_STAGES = 6;
 constexpr float PT_LO_SCALE = 4096.f;     // lo limbs are stored times 2^12
 constexpr long long PT_TIMEOUT_CYCLES = 4000000000LL;   // ~2 s
+constexpr size_t PT_SMEM_BUDGET = 227 * 1024;
+constexpr size_t PT_TAIL = 256;           // barriers + abort flag
 
 struct PiTcArgs {
   const float* preds;
@@ -57,8 +46,11 @@ struct PiTcArgs {
   uint32_t* flags;
   long long N;
   int H, C, Np, KC;
-  int NST, SA, SD;            // ring depths: staging units, converted A chunks, D chunks
-  int G;                      // models per accumulator drain
+  int rows;                   // items per CTA: 64 x warpgroups
+  int S;                      // stages (one model each)
+  uint32_t xbytes;            // stage offset of the D limbs (the items block rounded up to 128 bytes)
+  uint32_t sbytes;            // bytes per stage
+  int G;                      // models per accumulator fold
 };
 
 // power of two that brings max |D| below 2^15 (fp16 overflows at 65504); 0 when no scaling is needed
@@ -67,29 +59,7 @@ __device__ __forceinline__ int pt_down_shift(uint32_t maxbits) {
   return max(0, e - 14);
 }
 
-__device__ __forceinline__ void pt_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void pt_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void pt_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void pt_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// one lane of a converged warp
-__device__ __forceinline__ bool pt_elect() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xFFFFFFFF;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t"
-      "}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // try_wait with a suspend-time hint: the warp is parked by the hardware until the phase completes (or ~the hint elapses)
-// instead of burning the issue slots the converter warps need
 __device__ __forceinline__ bool pt_try(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -104,7 +74,7 @@ __device__ __forceinline__ bool pt_try(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 
-// false = the pipeline was aborted (here or by another role)
+// false = the pipeline was aborted (here or by another thread)
 __device__ __forceinline__ bool pt_wait(uint64_t* bar, uint32_t parity, volatile int* abort_s) {
   if (pt_try(bar, parity)) return true;
   const long long t0 = clock64();
@@ -118,50 +88,34 @@ __device__ __forceinline__ bool pt_wait(uint64_t* bar, uint32_t parity, volatile
   }
 }
 
-// a position in a ring of `n` slots walked one or several steps at a time; `ph` = parity of the number of wraps
-struct Ring {
-  int slot, ph, wrapped;
-  __device__ __forceinline__ void step(int by, int n) {
-    slot += by;
-    while (slot >= n) { slot -= n; ph ^= 1; wrapped = 1; }
-  }
-};
+// AND of `ok` over the 128 threads of warpgroup `wg` (named barrier 1 + wg; 0 is __syncthreads): the wgmma instructions
+// are warpgroup-wide, so a pipeline abort has to be agreed by the whole warpgroup before any of its warps leaves the loop
+__device__ __forceinline__ bool wg_all(bool ok, int wg) {
+  uint32_t r;
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.and.pred q, %2, 128, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t"
+      "}"
+      : "=r"(r)
+      : "r"((uint32_t)ok), "r"(1 + wg)
+      : "memory");
+  return r != 0;
+}
 
-// cute::UMMA::SmemDescriptor words (SWIZZLE_NONE, K-major, see pairs_tc.cu) are assembled in the MMA warp
-__device__ __forceinline__ uint64_t pt_pack(uint32_t lo, uint32_t hi) {
-  uint64_t d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
-  return d;
-}
-// cute::UMMA::InstrDescriptor: c = F32 (1) [4,6), a = b = F16 (0) [7,10) [10,13), K-major both, N >> 3 [17,23), M >> 4 [24,29)
-__device__ __forceinline__ uint32_t pt_idesc(int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(PT_M >> 4) << 24);
-}
-__device__ __forceinline__ void pt_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// D[64 x 16] (+)= A[64 x 16] . B[16 x 16]^T: A fp16 from registers (wgmma A fragment), B fp16 in shared memory (K-major)
+__device__ __forceinline__ void mma_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accum) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void pt_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void pt_tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+      "setp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accum));
 }
 
 // two floats -> packed fp16 hi limbs and packed fp16 lo limbs:  x = hi + lo / 4096 (+ 2^-22 x at worst)
@@ -185,7 +139,6 @@ __global__ void __launch_bounds__(256) k_pi_w_max(const float* __restrict__ D, l
 
 // ---- D -> fp16 limbs in the B-operand order: one blob per (model, K chunk) -----------------------------------------
 // blob = [k_core 2][n_core 2 Np/8: hi limbs, then lo limbs][8 classes][8 s] fp16;  class = n_core*8 + r,  s = chunk*16 + k_core*8 + e
-// (hi and lo side by side along N, so that A_hi . [D_hi | D_lo] is ONE tcgen05.mma of N = 2 Np)
 __global__ void __launch_bounds__(256) k_pi_w_limbs(const float* __restrict__ D, int H, int C, int Np, int KC,
                                                     const uint32_t* __restrict__ dmax, __half* __restrict__ wb) {
   const long long per_limb = (long long)2 * Np * 8;           // elements of one limb of one chunk (= Np x 16)
@@ -211,279 +164,136 @@ __global__ void __launch_bounds__(256) k_pi_w_limbs(const float* __restrict__ D,
   }
 }
 
-__global__ void __launch_bounds__(PT_THREADS, 1) k_pi_full_tc(PiTcArgs a) {
+__global__ void __launch_bounds__(2 * 128, 1) k_pi_full_tc(PiTcArgs a) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int H = a.H, C = a.C, Np = a.Np, KC = a.KC, NST = a.NST, SA = a.SA, SD = a.SD, G = a.G;
-  const long long n0 = (long long)blockIdx.x * PT_M;
-  const int cnt = (int)min((long long)PT_M, a.N - n0);
+  const int H = a.H, C = a.C, Np = a.Np, KC = a.KC, S = a.S, G = a.G;
+  const int nb = Np / 16;                                     // 16-class blocks
+  const long long n0 = (long long)blockIdx.x * a.rows;
+  const int cnt = (int)min((long long)a.rows, a.N - n0);
+  const int r0 = (warp >> 2) * PT_WG + (warp & 3) * 16 + (lane >> 2);   // this thread's items: r0 and r0 + 8
+  const int nwarps = blockDim.x >> 5;
 
-  // ---- shared memory carve-up ----------------------------------------------------------------------
-  const uint32_t stage_bytes = (uint32_t)PT_HALF * C * 4u;                    // fp32 block of one (model, 32-item quarter)
-  const uint32_t stage_stride = (stage_bytes + 127u) & ~127u;
-  const uint32_t a_limb = (uint32_t)PT_M * 16u * 2u;                          // 4 KB: one limb of one A chunk
-  const uint32_t b_limb = (uint32_t)Np * 16u * 2u;                            // one limb of one D chunk
-  unsigned char* stage0 = smem;
-  unsigned char* aslots = smem + (uint32_t)NST * stage_stride;                // [SA][2 limbs]
-  unsigned char* dslots = aslots + (uint32_t)SA * 2u * a_limb;                // [SD][2 limbs]
-  unsigned char* tail = dslots + (uint32_t)SD * 2u * b_limb;
-  uint64_t* fullS = reinterpret_cast<uint64_t*>(tail);        // staging unit filled (TMA)
-  uint64_t* emptyS = fullS + PT_MAX_STAGES;                   // staging unit consumed (its converter warps)
-  uint64_t* fullK = emptyS + PT_MAX_STAGES;                   // chunk q ready (index q & 15): 2 converter warps + the D TMA
-  uint64_t* doneK = fullK + PT_CHUNK_BARS;                    // chunk q consumed (index q & 15): tcgen05.commit
-  uint64_t* accFull = doneK + PT_CHUNK_BARS;                  // [2] accumulator group complete (tcgen05.commit)
-  uint64_t* accEmpty = accFull + 2;                           // [2] accumulator drained (drain warps)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accEmpty + 2);
-  volatile int* abort_s = reinterpret_cast<volatile int*>(tmem_slot + 1);
-
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)S * a.sbytes);
+  uint64_t* empty = full + PT_MAX_STAGES;
+  volatile int* abort_s = reinterpret_cast<volatile int*>(empty + PT_MAX_STAGES);
   if (tid == 0) {
-    for (int i = 0; i < PT_MAX_STAGES; ++i) {
-      mbar_init(&fullS[i], 1);
-      mbar_init(&emptyS[i], PT_CONV_GROUPS);
-    }
-    for (int i = 0; i < PT_CHUNK_BARS; ++i) {
-      mbar_init(&fullK[i], PT_WARPS_PER_CHUNK + 1);
-      mbar_init(&doneK[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&accFull[i], 1);
-      mbar_init(&accEmpty[i], PT_DRAIN_WARPS);
+    for (int i = 0; i < S; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], nwarps);
     }
     *abort_s = (*a.flags & CODA_B200_FLAG_PIPELINE_TIMEOUT) ? 1 : 0;          // an earlier CTA already gave up
     mbar_fence_init();
   }
-  if (warp == 3) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  pt_fence_before();
   __syncthreads();
-  pt_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const int total_chunks = H * KC;
-  const int ngroups = (H + G - 1) / G;
+  const uint32_t xbytes = (uint32_t)cnt * C * 4u, dbytes = (uint32_t)KC * Np * 64u;
+  auto load = [&](int h) {
+    unsigned char* st = smem + (size_t)(h % S) * a.sbytes;
+    uint64_t* bar = &full[h % S];
+    mbar_expect_tx(bar, xbytes + dbytes);
+    tma_load_1d(st, a.preds + (size_t)h * a.ldh + (size_t)n0 * C, xbytes, bar);
+    tma_load_1d(st + a.xbytes, a.wb + (size_t)h * dbytes, dbytes, bar);
+  };
+  if (tid == 0)
+    for (int h = 0; h < S && h < H; ++h) load(h);
 
-  if (warp == 0) {
-    // ---- slab producer: unit j = (model j / 4, 32-item quarter j % 4) ----------------------------------------
-    if (lane == 0) {
-      Ring r{0, 0, 0};
-      for (int j = 0; j < PT_WARPS_PER_CHUNK * H; ++j, r.step(1, NST)) {
-        const int hf = j % PT_WARPS_PER_CHUNK;
-        if (r.wrapped && !pt_wait(&emptyS[r.slot], r.ph ^ 1, abort_s)) break;
-        const int items = min(PT_HALF, max(0, cnt - hf * PT_HALF));
-        if (items == 0) {                                     // ragged last tile: nothing in this half
-          pt_arrive(&fullS[r.slot]);
-          continue;
-        }
-        const uint32_t bytes = (uint32_t)items * C * 4u;
-        mbar_expect_tx(&fullS[r.slot], bytes);
-        tma_load_1d(stage0 + (size_t)r.slot * stage_stride,
-                    a.preds + (size_t)(j / PT_WARPS_PER_CHUNK) * a.ldh + (size_t)(n0 + hf * PT_HALF) * C, bytes, &fullS[r.slot]);
-      }
+  float mainv[PT_MAXB][8], corr[PT_MAXB][8], tot[PT_MAXB][8];
+#pragma unroll
+  for (int b = 0; b < PT_MAXB; ++b)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) tot[b][i] = 0.f;
+  const uint32_t lbo = (uint32_t)(2 * Np / 8) * 128, lo_off = (uint32_t)(Np / 8) * 128, chunk_bytes = (uint32_t)Np * 64u;
+  const bool in0 = r0 < cnt, in1 = r0 + 8 < cnt;
+  bool ok = true;
+  for (int h = 0; h < H && ok; ++h) {
+    const int s = h % S;
+    if (tid == 0 && h >= 1 && h - 1 + S < H) {
+      if (pt_wait(&empty[(h - 1) % S], ((h - 1) / S) & 1, abort_s)) load(h - 1 + S);
     }
-  } else if (warp == 1) {
-    // ---- D producer ---------------------------------------------------------------------------------
-    if (lane == 0) {
-      const uint32_t bytes = 2u * b_limb;
-      Ring r{0, 0, 0};
-      for (int q = 0; q < total_chunks; ++q, r.step(1, SD)) {
-        const int w = q - SD;                                 // the chunk that held this slot
-        if (w >= 0 && !pt_wait(&doneK[w & (PT_CHUNK_BARS - 1)], (w / PT_CHUNK_BARS) & 1, abort_s)) break;
-        uint64_t* full = &fullK[q & (PT_CHUNK_BARS - 1)];
-        mbar_expect_tx(full, bytes);
-        tma_load_1d(dslots + (size_t)r.slot * bytes, a.wb + (size_t)q * bytes, bytes, full);
+    __syncwarp();
+    ok = wg_all(pt_wait(&full[s], (h / S) & 1, abort_s), warp >> 2);
+    if (!ok) break;
+    const unsigned char* st = smem + (size_t)s * a.sbytes;
+    const float* x0 = reinterpret_cast<const float*>(st) + (size_t)r0 * C;
+    const float* x1 = x0 + (size_t)8 * C;
+    const uint32_t dst = smem_u32(st + a.xbytes);
+    const bool restart = h % G == 0;
+    for (int kc = 0; kc < KC; ++kc) {
+      // this thread's A fragment: items r0, r0 + 8 x classes c0, c0 + 1, c0 + 8, c0 + 9 of the chunk (C % 4 == 0)
+      const int c0 = kc * 16 + 2 * (lane & 3);
+      const float2 z = make_float2(0.f, 0.f);
+      const float2 v00 = (in0 && c0 < C) ? *reinterpret_cast<const float2*>(x0 + c0) : z;
+      const float2 v10 = (in1 && c0 < C) ? *reinterpret_cast<const float2*>(x1 + c0) : z;
+      const float2 v01 = (in0 && c0 + 8 < C) ? *reinterpret_cast<const float2*>(x0 + c0 + 8) : z;
+      const float2 v11 = (in1 && c0 + 8 < C) ? *reinterpret_cast<const float2*>(x1 + c0 + 8) : z;
+      uint32_t ahi[4], alo[4];
+      pt_split2(v00.x, v00.y, ahi[0], alo[0]);
+      pt_split2(v10.x, v10.y, ahi[1], alo[1]);
+      pt_split2(v01.x, v01.y, ahi[2], alo[2]);
+      pt_split2(v11.x, v11.y, ahi[3], alo[3]);
+      const uint32_t bc = dst + (uint32_t)kc * chunk_bytes;
+      const uint32_t acc = (restart && kc == 0) ? 0u : 1u;
+      wg_fence();
+#pragma unroll
+      for (int b = 0; b < PT_MAXB; ++b) {
+        if (b < nb) {                                         // warp-uniform
+          const uint64_t bhi = wg_desc(bc + (uint32_t)b * 256u, lbo, 128);
+          const uint64_t blo = wg_desc(bc + lo_off + (uint32_t)b * 256u, lbo, 128);
+          mma_n16(mainv[b], ahi, bhi, acc);                   // main (+)= A_hi . D_hi
+          mma_n16(corr[b], ahi, blo, acc);                    // corr (+)= A_hi . D_lo
+          mma_n16(corr[b], alo, bhi, 1u);                     // corr  += A_lo . D_hi
+        }
       }
+      wg_commit();
+      wg_wait0();
     }
-  } else if (warp == 2) {
-    // ---- MMA issuer: the whole warp walks the loop (so everything stays in uniform registers), one elected lane issues.
-    // The issue rate of this one warp bounds the tensor pipe (an MMA of N = 112 is 56 cycles), so ring positions and
-    // descriptors are stepped incrementally: no division, no descriptor rebuild per chunk.
-    {
-      const uint32_t tmem_u = __shfl_sync(CODA_FULL, tmem, 0);
-      const uint32_t idesc2 = pt_idesc(2 * Np), idesc1 = pt_idesc(Np);
-      // descriptor words (SWIZZLE_NONE, K-major): lo = start >> 4 | LBO >> 4 << 16, hi = SBO >> 4 | version 1 << 14
-      const uint32_t a_lo0 = ((smem_u32(aslots) & 0x3FFFFu) >> 4) | ((uint32_t)((PT_M / 8) * 128 >> 4) << 16);
-      const uint32_t d_lo0 = ((smem_u32(dslots) & 0x3FFFFu) >> 4) | ((uint32_t)((2 * Np / 8) * 128 >> 4) << 16);
-      const uint32_t desc_hi = (128u >> 4) | (1u << 14);
-      const uint32_t a_step = (2u * a_limb) >> 4, a_limb16 = a_limb >> 4, d_step = (2u * b_limb) >> 4;
-      uint32_t a_off = 0, d_off = 0, kph = 0;
-      int a_slot = 0, d_slot = 0, bi = 0;
-      bool ok = true;
-      for (int g = 0; g < ngroups && ok; ++g) {
-        const int buf = g & 1;
-        if (g >= 2) {
-          ok = pt_wait(&accEmpty[buf], ((g >> 1) - 1) & 1, abort_s);
-          ok = __all_sync(CODA_FULL, ok);
-          if (!ok) break;
-          pt_fence_after();
-        }
-        const uint32_t t_main = tmem_u + (uint32_t)buf * 256u, t_corr = t_main + (uint32_t)Np;
-        const int nchunks = (min(H, (g + 1) * G) - g * G) * KC;
-        for (int k = 0; k < nchunks; ++k) {
-          ok = pt_wait(&fullK[bi], kph, abort_s);
-          ok = __all_sync(CODA_FULL, ok);
-          if (!ok) break;
-          pt_fence_after();
-          if (pt_elect()) {
-            const uint64_t d_all = pt_pack(d_lo0 + d_off, desc_hi);
-            pt_mma(t_main, pt_pack(a_lo0 + a_off, desc_hi), d_all, idesc2, k ? 1u : 0u);     // [main | corr] (+)= A_hi . [D_hi | D_lo]
-            pt_mma(t_corr, pt_pack(a_lo0 + a_off + a_limb16, desc_hi), d_all, idesc1, 1u);    // corr += A_lo . D_hi
-            pt_commit(&doneK[bi]);
-          }
-          __syncwarp();
-          a_off += a_step;
-          if (++a_slot == SA) { a_slot = 0; a_off = 0; }
-          d_off += d_step;
-          if (++d_slot == SD) { d_slot = 0; d_off = 0; }
-          if (++bi == PT_CHUNK_BARS) { bi = 0; kph ^= 1u; }
-        }
-        if (ok && pt_elect()) pt_commit(&accFull[buf]);
-        __syncwarp();
-      }
-    }
-  } else if (warp >= PT_DRAIN_WARP0 && warp < PT_DRAIN_WARP0 + PT_DRAIN_WARPS) {
-    // ---- drain: (item, column part) per thread: lane quadrant = warp % 4 (hardware rule), 16-column units u_lo..u_hi -----
-    const int quad = warp & 3, part = (warp - PT_DRAIN_WARP0) >> 2;
-    const int row = quad * 32 + lane;
-    const int nu = Np / 16;                                   // 16-column units (<= 8)
-    const int per = (nu + PT_DRAIN_PARTS - 1) / PT_DRAIN_PARTS;               // <= 2 units per thread
-    const int u_lo = min(nu, part * per), u_hi = min(nu, u_lo + per);
-    float acc[2][16];
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
+    if ((h + 1) % G == 0 || h + 1 == H) {
 #pragma unroll
-    for (int u = 0; u < 2; ++u)
+      for (int b = 0; b < PT_MAXB; ++b)
 #pragma unroll
-      for (int i = 0; i < 16; ++i) acc[u][i] = 0.f;
-    bool ok = true;
-    for (int g = 0; g < ngroups; ++g) {
-      const int buf = g & 1;
-      ok = pt_wait(&accFull[buf], (g >> 1) & 1, abort_s);
-      ok = __all_sync(CODA_FULL, ok);
-      if (!ok) break;
-      pt_fence_after();
-      const uint32_t trow = tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)buf * 256u;
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        if (u_lo + u < u_hi) {                                // warp-uniform
-          float m[16];
-          pt_tmem_ld16(trow + (uint32_t)(u_lo + u) * 16u, m);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) acc[u][i] += m[i];
-          pt_tmem_ld16(trow + (uint32_t)Np + (uint32_t)(u_lo + u) * 16u, m);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) acc[u][i] = fmaf(m[i], 1.0f / PT_LO_SCALE, acc[u][i]);
-        }
-      }
-      pt_fence_before();
-      __syncwarp();
-      if (lane == 0) pt_arrive(&accEmpty[buf]);
-    }
-    if (ok && row < cnt) {
-      const float up = __uint_as_float((uint32_t)(127 + pt_down_shift(*a.dmax)) << 23);      // undo the D range scaling
-      float* urow = a.U + (size_t)(n0 + row) * C;
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        if (u_lo + u < u_hi) {
-          const int c0 = (u_lo + u) * 16;
-#pragma unroll
-          for (int i = 0; i < 16; i += 4)
-            if (c0 + i < C)                                   // C % 4 == 0: whole float4 in range
-              *reinterpret_cast<float4*>(urow + c0 + i) =
-                  make_float4(acc[u][i] * up, acc[u][i + 1] * up, acc[u][i + 2] * up, acc[u][i + 3] * up);
-        }
-      }
-    }
-  } else if (warp >= PT_CONV_WARP0) {
-    // ---- converters: warp pair `grp` takes chunks q = grp, grp + PT_CONV_GROUPS, ...; `sub` picks the 32-item quarter ------
-    const int cw = warp - PT_CONV_WARP0;
-    const int grp = cw / PT_WARPS_PER_CHUNK, sub = cw % PT_WARPS_PER_CHUNK;
-    bool ok = true;
-    int q = grp;                                              // this warp's next chunk (global chunk index)
-    Ring rs{0, 0, 0}, ra{0, 0, 0};
-    rs.step(sub, NST);                                        // staging unit PT_WARPS_PER_CHUNK * h + sub
-    ra.step(grp, SA);
-    for (int h = 0; h < H && ok; ++h, rs.step(PT_WARPS_PER_CHUNK, NST)) {
-      ok = pt_wait(&fullS[rs.slot], rs.ph, abort_s);
-      ok = __all_sync(CODA_FULL, ok);
-      if (!ok) break;
-      const float* src = reinterpret_cast<const float*>(stage0 + (size_t)rs.slot * stage_stride);
-      for (; q < (h + 1) * KC; q += PT_CONV_GROUPS, ra.step(PT_CONV_GROUPS, SA)) {
-        const int kc = q - h * KC;
-        const int w = q - SA;                                 // the chunk that held this A slot
-        if (w >= 0) {
-          ok = pt_wait(&doneK[w & (PT_CHUNK_BARS - 1)], (w / PT_CHUNK_BARS) & 1, abort_s);
-          ok = __all_sync(CODA_FULL, ok);
-          if (!ok) break;
-        }
-        unsigned char* dst = aslots + (size_t)ra.slot * 2u * a_limb;
-        // all loads first: the limb stores below go to shared memory too, so the compiler would not hoist loads over them
-        float4 v[PT_HALF / 32][2][2];
-#pragma unroll
-        for (int it = 0; it < PT_HALF / 32; ++it) {
-          const float* rowp = src + (size_t)(it * 32 + lane) * C + kc * 16;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)                         // 4 x float4 = the 16 columns of this chunk
-            v[it][j >> 1][j & 1] = (kc * 16 + j * 4 < C) ? *reinterpret_cast<const float4*>(rowp + j * 4)
-                                                          : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int it = 0; it < PT_HALF / 32; ++it) {
-          const int item = sub * PT_HALF + it * 32 + lane;
-#pragma unroll
-          for (int kcore = 0; kcore < 2; ++kcore) {
-            const float4 x = v[it][kcore][0], y = v[it][kcore][1];
-            uint4 hi, lo;
-            pt_split2(x.x, x.y, hi.x, lo.x);
-            pt_split2(x.z, x.w, hi.y, lo.y);
-            pt_split2(y.x, y.y, hi.z, lo.z);
-            pt_split2(y.z, y.w, hi.w, lo.w);
-            const uint32_t off = (uint32_t)((kcore * (PT_M / 8) + (item >> 3)) * 128 + (item & 7) * 16);
-            *reinterpret_cast<uint4*>(dst + off) = hi;
-            *reinterpret_cast<uint4*>(dst + a_limb + off) = lo;
-          }
-        }
-        pt_fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) pt_arrive(&fullK[q & (PT_CHUNK_BARS - 1)]);
-      }
-      __syncwarp();
-      if (lane == 0) pt_arrive(&emptyS[rs.slot]);
+        for (int i = 0; i < 8; ++i) tot[b][i] = fmaf(corr[b][i], 1.0f / PT_LO_SCALE, tot[b][i] + mainv[b][i]);
     }
   }
-
-  pt_fence_before();
   __syncthreads();
   if (tid == 0 && *abort_s) atomicOr(a.flags, CODA_B200_FLAG_PIPELINE_TIMEOUT);
-  if (warp == 3) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+  if (*abort_s) return;
+  // accumulator fragment: register 4 j + 2 i + e of block b = item r0 + 8 i, class 16 b + 8 j + 2 (lane % 4) + e
+  const float up = __uint_as_float((uint32_t)(127 + pt_down_shift(*a.dmax)) << 23);      // undo the D range scaling
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    if (r0 + 8 * i >= cnt) continue;
+    float* urow = a.U + (size_t)(n0 + r0 + 8 * i) * C;
+#pragma unroll
+    for (int b = 0; b < PT_MAXB; ++b) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int col = 16 * b + 8 * j + 2 * (lane & 3);
+        if (b < nb && col < C)                                // C % 4 == 0: both classes in range
+          *reinterpret_cast<float2*>(urow + col) = make_float2(tot[b][4 * j + 2 * i] * up, tot[b][4 * j + 2 * i + 1] * up);
+      }
+    }
   }
 }
 
 struct PiTcPlan {
-  int stages, aslots, dslots;
+  int rows, stages;
+  uint32_t xbytes, sbytes;
   size_t smem;
 };
 
-// shared-memory split: a short ring of converted A chunks, the rest shared between slab staging and D chunks in flight
-PiTcPlan pi_tc_plan(int C, int Np) {
-  const size_t budget = 227 * 1024;
-  const size_t stage = ((size_t)PT_HALF * C * 4 + 127) & ~(size_t)127;
-  const size_t aslot = 2 * (size_t)PT_M * 32, dslot = 2 * (size_t)Np * 32;
-  const size_t fixed = (size_t)PT_NBAR * 8 + 64;
+// two warpgroups (128 items per CTA) when two stages fit shared memory, else one; then as many stages as fit
+PiTcPlan pi_tc_plan(int C, int Np, int KC) {
   PiTcPlan p;
-  p.aslots = PT_CONV_GROUPS + 1;
-  p.stages = PT_WARPS_PER_CHUNK + 1;
-  p.dslots = 2;
-  for (;;) {      // grow the two rings in turn, balancing the BYTES IN FLIGHT (units not being converted, D chunks not being read)
-    const size_t used = fixed + p.aslots * aslot + p.stages * stage + p.dslots * dslot;
-    const bool more_stage = p.stages < PT_MAX_STAGES && used + stage <= budget;
-    const bool more_d = p.dslots < PT_MAX_DSLOTS && used + dslot <= budget;
-    if (more_d && ((p.dslots - 1) * dslot <= (p.stages - PT_WARPS_PER_CHUNK) * stage || !more_stage)) ++p.dslots;
-    else if (more_stage) ++p.stages;
-    else break;
+  const size_t dbytes = (size_t)KC * Np * 64;
+  for (p.rows = 2 * PT_WG; ; p.rows -= PT_WG) {
+    p.xbytes = (uint32_t)(((size_t)p.rows * C * 4 + 127) & ~(size_t)127);
+    p.sbytes = (uint32_t)(p.xbytes + dbytes);
+    if (2 * (size_t)p.sbytes + PT_TAIL <= PT_SMEM_BUDGET || p.rows == PT_WG) break;
   }
-  p.smem = fixed + p.aslots * aslot + p.stages * stage + p.dslots * dslot;
+  p.stages = (int)min((size_t)PT_MAX_STAGES, (PT_SMEM_BUDGET - PT_TAIL) / p.sbytes);
+  p.smem = (size_t)p.stages * p.sbytes + PT_TAIL;
   return p;
 }
 
@@ -513,18 +323,18 @@ extern "C" int coda_b200_pi_full_tc(const float* preds, int64_t model_stride, co
   CODA_LAUNCH_OK("k_pi_w_max");
   k_pi_w_limbs<<<coda_sm_count() * 4, 256, 0, as_stream(stream)>>>(D, H, C, Np, KC, dmax, reinterpret_cast<__half*>(wb));
   CODA_LAUNCH_OK("k_pi_w_limbs");
-  const PiTcPlan plan = pi_tc_plan(C, Np);
-  CODA_CHECK_ARG(plan.smem <= 227 * 1024, "pi_full_tc: C=%d does not fit shared memory", C);
+  const PiTcPlan plan = pi_tc_plan(C, Np, KC);
+  CODA_CHECK_ARG(plan.stages >= 2, "pi_full_tc: C=%d does not fit shared memory", C);
   PiTcArgs a;
   a.preds = preds; a.ldh = model_stride; a.wb = wb; a.dmax = dmax; a.U = U; a.flags = flags;
   a.N = N; a.H = H; a.C = C; a.Np = Np; a.KC = KC;
-  a.NST = plan.stages; a.SA = plan.aslots; a.SD = plan.dslots;
-  // models per drain: the truncating fp32 accumulate of the tensor core loses up to 2^-24 per K = 8 sub-step of the chain
+  a.rows = plan.rows; a.S = plan.stages; a.xbytes = plan.xbytes; a.sbytes = plan.sbytes;
+  // models per fold: the truncating fp32 accumulate of the tensor core loses up to 2^-24 per K = 8 sub-step of the chain
   const char* genv = getenv("CODA_B200_PI_DRAIN");
   a.G = genv ? max(1, min(16, atoi(genv))) : 4;
   CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_full_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
-  const long long grid = (N + PT_M - 1) / PT_M;
-  k_pi_full_tc<<<(unsigned)grid, PT_THREADS, plan.smem, as_stream(stream)>>>(a);
+  const long long grid = (N + plan.rows - 1) / plan.rows;
+  k_pi_full_tc<<<(unsigned)grid, 2 * plan.rows, plan.smem, as_stream(stream)>>>(a);
   CODA_LAUNCH_OK("k_pi_full_tc");
   return CODA_B200_OK;
 }

@@ -834,10 +834,6 @@ __global__ void __launch_bounds__(256, 3) k_pi_rank1_v4(const float* __restrict_
 #define R1X_ST 4
 #define R1X_TB 16
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
 template <int KC>
 __global__ void __launch_bounds__(R1X_THREADS, 1) k_pi_rank1_tma(const float* __restrict__ preds,
                                                                  const float* __restrict__ E, long long N, int C, int TR,

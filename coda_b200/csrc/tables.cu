@@ -159,7 +159,7 @@ __global__ void __launch_bounds__(TP_ * NP) k_beta_combine(const double* __restr
       G0T[((size_t)c * TP_ + x) * Hp + h] = g0f;
       G1T[((size_t)c * TP_ + x) * Hp + h] = g1f;
       if (dLb) {
-        // tensor-core operand tables (pairs_tc.cu): bf16 limbs in the UMMA no-swizzle K-major core-matrix order
+        // tensor-core operand tables (pairs_tc.cu): bf16 limbs in the wgmma no-swizzle K-major core-matrix order
         // [k_core][r_core][8 rows][8 elements].  dLb tile: rows = nodes, K = 32 models; Gb tile: rows = models, K = 16 nodes.
         const __nv_bfloat16 d0 = __float2bfloat16_rn(dlf);
         const float r1 = dlf - __bfloat162float(d0);

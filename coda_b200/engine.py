@@ -71,7 +71,7 @@ class Engine:
             raise ValueError(f"mode must be one of {MODES}")
         self.compact = preds if isinstance(preds, CompactSlab) else None
         if not ((isinstance(preds, torch.Tensor) or self.compact is not None) and preds.is_cuda):
-            raise RuntimeError("coda_b200: dataset.preds must live on a CUDA (sm_100a) device; "
+            raise RuntimeError("coda_b200: dataset.preds must live on a CUDA (sm_90a) device; "
                                "there is no CPU path in this package")
         H, N, Cc = (int(s) for s in preds.shape)
         if N < 1:
@@ -365,7 +365,7 @@ class Engine:
                    _ptr(self.flags), s)
 
     def _pi_full(self):
-        """coda.py:227-229 over the dense slab: the tcgen05 kernel when the shape allows it (pi_tc.cu), else fp32 SIMT.
+        """coda.py:227-229 over the dense slab: the wgmma kernel when the shape allows it (pi_tc.cu), else fp32 SIMT.
         ``CODA_B200_PI_FULL=simt`` forces the SIMT kernel."""
         H, N, C, s = self.H, self.N, self.C, self._s()
         if self._pi_tc is None:
@@ -404,7 +404,7 @@ class Engine:
         del ent_cnt, heavy_cnt
         self.cls_base_host = cls_base
         self.cls_base = torch.from_numpy(cls_base).to(self.dev)
-        # tiles of <= 32 (SIMT) or <= 128 (tcgen05) same-class work-list positions
+        # tiles of <= 32 (SIMT) or <= 128 (wgmma) same-class work-list positions
         def make_tiles(width):
             nt = (per_cls + width - 1) // width
             tile_off = np.zeros(C + 1, dtype=np.int64)

@@ -1,4 +1,4 @@
-"""``CODA`` -- host-side mirror of the reference selector (coda/coda.py:171-346) over the sm_100a kernels.
+"""``CODA`` -- host-side mirror of the reference selector (coda/coda.py:171-346) over the sm_90a kernels.
 
 Same constructor, same three ``ModelSelector`` calls, same attributes callers read
 (``stochastic``, ``unlabeled_idxs``, ``pi_hat``, ``pi_hat_xi``, ``dirichlets``, ``labeled_idxs``,

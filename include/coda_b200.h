@@ -1,4 +1,4 @@
-/* coda_b200 -- C ABI of the B200-native CODA acquisition hot path.
+/* coda_b200 -- C ABI of the CUDA-native CODA acquisition hot path (H100, sm_90a).
  *
  * Drop-in boundary (SURVEY.md 8b).  The reference (justinkay/coda) is pure Python/PyTorch
  * and has no FFI of its own; these entry points are what a ctypes binding inside
@@ -20,7 +20,7 @@
  *     (class-major: c*(1+H) + 0 = no model predicts c, + 1 + h = only model h predicts c); rows [T, T + n_heavy) are
  *     the heavy rows (two or more models predict the class), ITEM-major: the heavy rows of item n are
  *     T + heavy_off[n] .. T + heavy_off[n+1] - 1 in ascending class order;
- *   - built for sm_100a only.
+ *   - built for sm_90a only.
  */
 #ifndef CODA_B200_H
 #define CODA_B200_H
@@ -60,7 +60,7 @@ typedef void* coda_stream_t;
 const char* coda_b200_last_error(void);
 int coda_b200_version(void);
 int coda_b200_sm_count(void);
-int coda_b200_device_check(void); /* fails loudly when no sm_100 device is present */
+int coda_b200_device_check(void); /* fails loudly when no sm_90 device is present */
 /* cudaLimitMaxL2FetchGranularity hint (32/64/128 B) for the sector-gather kernels (per device). */
 int coda_b200_set_l2_fetch_granularity(int bytes);
 
@@ -117,8 +117,8 @@ int coda_b200_init_dirichlets(const int64_t* conf_fx, const int64_t* conf_rest, 
 int coda_b200_pi_full(const float* preds, int64_t model_stride, const float* D, int H, int64_t N, int C, float* U,
                       coda_stream_t stream);
 
-/* The same contraction on the tensor cores (tcgen05, TMEM accumulators, bulk-TMA slab stream): both operands are cut
- * into two bf16 limbs, 4 MMAs per K = 16 chunk, accumulators drained to fp32 registers every 4 models (pi_tc.cu).
+/* The same contraction on the tensor cores (wgmma, register accumulators, bulk-TMA slab stream): both operands are cut
+ * into two fp16 limbs, 3 MMAs per K = 16 chunk, accumulators folded into fp32 registers every 4 models (pi_tc.cu).
  * Usable when pi_full_tc_ok(...) != 0 (16 <= C <= 128, C % 4 == 0, model_stride % 4 == 0); `scratch` =
  * pi_full_tc_scratch_bytes(H, C) bytes (the D limbs).  A stopped pipeline sets CODA_B200_FLAG_PIPELINE_TIMEOUT. */
 int coda_b200_pi_full_tc_ok(int H, int64_t N, int C, int64_t model_stride);
@@ -222,7 +222,7 @@ int coda_b200_pair_rows(const int32_t* tiles, int tile_lo, int tile_hi, const ui
                         const float* dL, const float* G0T, const float* G1T, const float* PB, const float* m0,
                         const float* pi_hat, int H, float* ph_cache, float* gain, const int64_t* sel /*optional*/,
                         const int64_t* tile_off /*[C+1], with sel*/, uint32_t* flags, coda_stream_t stream);
-/* The same computation on the tcgen05 tensor cores (Hp <= 256): tiles128 are tiles of <= 128 same-class positions,
+/* The same computation on the wgmma tensor cores (Hp <= 256): tiles128 are tiles of <= 128 same-class positions,
  * operands come from the bf16 limb tables of coda_b200_beta_tables. */
 int coda_b200_pair_rows_tc(const int32_t* tiles128, int tile_lo, int tile_hi, const uint32_t* zmask,
                            const int32_t* row_of, const void* dLb, const void* Gb, const float* PB, const float* m0,

@@ -8,11 +8,11 @@ reference`` legs have something to check and time the CUDA path against.  The
 product (``coda_b200``) never imports it; nothing here is a fallback.
 
 Parity status: the reference ships no tests or golden vectors (SURVEY.md 8c), so
-the oracle is pinned against *outputs of the reference itself*, run on CPU in the
-build container by ``tests/golden/make_golden.py`` and committed under
+the oracle is pinned against *outputs of the reference itself*, run on CPU by
+``tests/golden/make_golden.py`` and committed under
 ``tests/golden/``.  ``tests/test_oracle_golden.py`` replays them.
 
-Every function cites the reference lines (``/root/reference/coda/coda.py`` unless
+Every function cites the reference lines (the reference's ``coda/coda.py`` unless
 another file is named) whose arithmetic it restates.  Arithmetic order follows the
 reference where fp32 rounding is order-sensitive (the cumulative trapezoid, the
 clamped leave-one-out product), so the oracle agrees with the reference to a few

@@ -1,7 +1,7 @@
-"""BASELINE.json configs[0]: run the reference's REAL driver (`/root/reference/main.py`, unmodified, with the
+"""BASELINE.json configs[0]: run the reference's REAL driver (its `main.py`, unmodified, with the
 reference's own `coda` package) on the cifar10_5592 stand-in on CPU and keep what it logged.
 
-    python tests/golden/make_cfg1_golden.py [iters]     # needs /root/reference; ~70 s per iteration on 8 cores
+    CODA_REFERENCE_PATH=<reference checkout> python tests/golden/make_cfg1_golden.py [iters]   # ~70 s per iteration on 8 cores
 
 The paper's tensors are not in the reference checkout (README.md:31, a 3.25 GB download), so the task file is the
 synthetic stand-in SURVEY.md 8(d) names: synth(80, 10000, 10, seed 0) saved as cifar10_5592.pt / _labels.pt.
@@ -20,7 +20,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("CODA_REFERENCE_PATH", "/root/reference")
+REF = os.environ.get("CODA_REFERENCE_PATH", "")
 TASK = dict(H=80, N=10000, C=10, seed=0)
 
 

@@ -1,12 +1,11 @@
-"""Generate golden fixtures by RUNNING THE REFERENCE (CPU, fp32) in the build container.
+"""Generate golden fixtures by RUNNING THE REFERENCE (CPU, fp32).
 
-    python tests/golden/make_golden.py            # needs /root/reference; writes tests/golden/*.npz
+    CODA_REFERENCE_PATH=<reference checkout> python tests/golden/make_golden.py [cases]   # writes tests/golden/*
 
 The reference has no tests or golden vectors of its own (SURVEY.md 8c), so the pins are
-outputs of the unmodified ``/root/reference/coda/coda.py`` on seeded synthetic slabs
-(``coda_b200.synth``).  ``/root/reference`` does not exist on the GPU box; only the small
-``.npz`` files travel.  ``matplotlib`` is not installed here and ``coda/util.py:2`` imports
-it, so an empty stub module is put on ``sys.modules`` first (nothing on the path uses it).
+outputs of the unmodified reference ``coda/coda.py`` on seeded synthetic slabs
+(``coda_b200.synth``).  The tests read only the stored files, never the reference.  ``coda/util.py:2``
+imports matplotlib, so an empty stub module is put on ``sys.modules`` first (nothing on the path uses it).
 
 Each fixture stores the synthetic-task parameters (the slab is regenerated from them), the
 reference's initial state, and a free-running K-step trajectory: per step the candidate
@@ -24,10 +23,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 
-REF = os.environ.get("CODA_REFERENCE_PATH", "/root/reference")
+REF = os.environ.get("CODA_REFERENCE_PATH", "")
 
 
 def import_reference():
+    torch.set_num_threads(8)     # tests/test_oracle_golden.py replays with the same CPU reduction split
     for name in ("matplotlib", "matplotlib.pyplot"):
         sys.modules.setdefault(name, types.ModuleType(name))
     sys.path.insert(0, REF)
@@ -110,13 +110,51 @@ def run_case(ref_coda, name, H, N, C, data_seed, steps, dense=False, ctor=None, 
                final_dirichlets=sel.dirichlets.numpy().copy(), stochastic=int(sel.stochastic))
     if save_eig:
         out["eig"] = np.stack(eigs)
+    out.pop("final_dirichlets")   # init_dirichlets with the dir_row slices written back (tests/helpers.py: load_golden)
+    if N > 5000:                  # only the GPU trajectory test replays this golden, and it never reads the xi slab
+        out.pop("init_pi_hat_xi")
+        out["labels"] = out["labels"].astype(np.int8 if C < 128 else np.int16)
     if slim:     # H*C*C-sized arrays make a multi-megabyte fixture: keep the per-step rows only
-        for k in ("init_dirichlets", "final_dirichlets", "init_pi_hat_xi"):
-            out.pop(k)
+        for k in ("init_dirichlets", "init_pi_hat_xi"):
+            out.pop(k, None)
         out["xi_head"] = out["xi_head"][:, :8]
     path = os.path.join(HERE, name + ".npz")
     np.savez_compressed(path, **out)
     print(name, "idx", idxs, "ties", ntie, "->", path, os.path.getsize(path) // 1024, "KiB")
+
+
+def rng_digest():
+    """Fingerprint of Python's RNG state: equal digests = the same draws were consumed."""
+    import hashlib
+    return hashlib.sha256(repr(random.getstate()).encode()).hexdigest()[:16]
+
+
+def acquisition_vectors(ref_coda):
+    """The ablation acquisitions (coda.py:287-295) and the --prefilter-n subsample (coda.py:221-223): picks, scores,
+    best model and the RNG state after every pick, for the oracle's RNG-consumption tests."""
+    import json
+    from coda_b200.synth import synth
+    out = {}
+    for q in ("iid", "uncertainty"):
+        preds, labels = synth(12, 500, 6, seed=17)
+        random.seed(4)
+        r = ref_coda.CODA(_DS(preds, labels), q=q)
+        steps = []
+        for _ in range(4):
+            i, qq = r.get_next_item_to_label()
+            rng = rng_digest()
+            r.add_label(i, int(labels[i]), qq)
+            steps.append(dict(idx=int(i), q=float(qq), rng=rng, best=int(r.get_best_model_prediction())))
+        out[q] = dict(H=12, N=500, C=6, data_seed=17, seed=4, steps=steps)
+    preds, labels = synth(10, 600, 6, seed=8)
+    random.seed(5)
+    r = ref_coda.CODA(_DS(preds, labels), prefilter_n=50)
+    i, qq = r.get_next_item_to_label()
+    out["prefilter"] = dict(H=10, N=600, C=6, data_seed=8, seed=5, prefilter_n=50,
+                            steps=[dict(idx=int(i), q=float(qq), rng=rng_digest())], stochastic=bool(r.stochastic))
+    with open(os.path.join(HERE, "acquisitions.json"), "w") as f:
+        json.dump(out, f, indent=1)
+    print("acquisitions", out)
 
 
 def unit_vectors(ref_coda):
@@ -133,9 +171,14 @@ def unit_vectors(ref_coda):
 
 
 if __name__ == "__main__":
+    if not os.path.isdir(os.path.join(REF, "coda")):
+        raise SystemExit("set CODA_REFERENCE_PATH to a checkout of the reference")
     ref = import_reference()
-    unit_vectors(ref)
-    which = sys.argv[1:] or ["tiny", "small", "c100", "dense", "nodiag"]
+    which = sys.argv[1:] or ["kat", "acq", "tiny", "small", "c100", "dense", "nodiag"]
+    if "kat" in which:
+        unit_vectors(ref)
+    if "acq" in which:
+        acquisition_vectors(ref)
     if "tiny" in which:
         run_case(ref, "traj_tiny_h8_n300_c5", 8, 300, 5, 1, steps=6)
     if "small" in which:

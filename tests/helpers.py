@@ -25,6 +25,13 @@ def load_golden(name):
     g["ctor"] = {}
     for k, v in zip(g["ctor_keys"].tolist(), g["ctor_vals"].tolist()):
         g["ctor"][k] = bool(v) if k == "disable_diag_prior" else (int(v) if k == "prefilter_n" else float(v))
+    if "final_dirichlets" not in g and "init_dirichlets" in g:
+        # a step rewrites only the labeled class's slice D[:, t], which every golden stores as dir_row: the final
+        # posterior is the initial one with those slices in step order (exact; kept out of the files for size)
+        fin = g["init_dirichlets"].copy()
+        for k, i in enumerate(g["idx"]):
+            fin[:, int(g["labels"][int(i)])] = g["dir_row"][k]
+        g["final_dirichlets"] = fin
     return g
 
 

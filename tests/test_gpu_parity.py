@@ -1,5 +1,5 @@
 """Parity of the CUDA path (through the C ABI / coda_b200.CODA) with the reference goldens and the CPU oracle.
-Run on the B200 box:  python -m pytest tests -m gpu -x -q
+Run on an H100:  python -m pytest tests -m gpu -x -q
 
 Tolerances (SURVEY.md 8c; the reference is fp32 with a measured EIG noise floor of ~1.2e-6):
   EIG vector            abs 5e-6          P(best) / pi_hat      abs 1e-5 (north_star: 1e-4)
@@ -350,7 +350,7 @@ def test_prefilter_n_subsample_path():
 
 
 def test_tensor_core_rows_match_simt_rows(monkeypatch):
-    """pairs_tc.cu (tcgen05, bf16 limbs) against pairs.cu (fp32 SIMT) on the same tables: per-item EIG and P(best)."""
+    """pairs_tc.cu (wgmma, bf16 limbs) against pairs.cu (fp32 SIMT) on the same tables: per-item EIG and P(best)."""
     from coda_b200.synth import synth
     for (H, N, C, seed) in [(256, 6000, 20, 3), (40, 3000, 12, 2), (100, 2000, 7, 6)]:
         preds, labels = synth(H, N, C, seed=seed)
@@ -551,7 +551,7 @@ def test_device_loop_follows_the_reference_trajectory(name, mode):
 
 
 def test_full_width_tensor_core_tile_against_the_reference():
-    """H = 256, C = 100 (Hp = 256: 8 K-chunks, all 512 TMEM columns of k_pair_rows_tc) pinned to the reference's
+    """H = 256, C = 100 (Hp = 256: 8 K-chunks, two column passes of k_pair_rows_tc) pinned to the reference's
     compute_pbest_beta_batched (coda.py:77-119) through a golden generated by the reference itself -- not to the
     SIMT twin.  Teacher-forced; EIG vector, pick, P(best), posterior rows."""
     names = [n for n in golden_names() if "h256" in n]
@@ -658,7 +658,7 @@ def test_marginal_refresh_variants_carry_identical_bits(shape, monkeypatch):
 @pytest.mark.parametrize("shape", [(256, 1000, 100, 1.0), (5, 128, 16, 1.0), (9, 700, 128, 1.0), (30, 257, 20, 3e5),
                                    (64, 4100, 52, 1e-3), (3, 40, 24, 1.0)])
 def test_tensor_core_marginals_match_fp64(shape):
-    """coda.py:227-229 on tcgen05 (k_pi_full_tc: two fp16 limbs per operand, TMEM accumulators drained every 4 models)
+    """coda.py:227-229 on wgmma (k_pi_full_tc: two fp16 limbs per operand, accumulators folded every 4 models)
     against an fp64 contraction and against the fp32 SIMT kernel, through the raw C ABI: ragged last tile, class counts
     that are not a multiple of 16, a model count that is not a multiple of the drain group, Dirichlet parameters far
     outside the fp16 range (rescaled by a power of two inside), a slab VIEW (model stride larger than the shard), and

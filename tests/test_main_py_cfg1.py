@@ -1,12 +1,14 @@
-"""BASELINE.json configs[0] / north_star "main.py and the MLflow logging run unchanged": the reference's REAL driver
-(`main.py`, unmodified) executed as a subprocess against THIS package on the GPU, with a recording MLflow stand-in
-(`tests/stubs/mlflow`; MLflow is not installed in the images), compared with what the same driver logged when it ran
-on the reference's own `coda` package on CPU (`tests/golden/cfg1_main_py.json`, made by `tests/golden/make_cfg1_golden.py`).
+"""BASELINE.json configs[0] / north_star "main.py and the MLflow logging run unchanged": the reference driver's
+experiment loop, executed as a subprocess against THIS package on the GPU with a recording MLflow stand-in
+(`tests/stubs/mlflow`; MLflow is not installed in the images), compared with what the reference's real `main.py` logged
+when it ran on the reference's own `coda` package on CPU (`tests/golden/cfg1_main_py.json`, made by
+`tests/golden/make_cfg1_golden.py`).
 
-The driver script is not part of this repository (reference sources are never copied in).  It is looked up at
-$CODA_REFERENCE_MAIN, $CODA_REFERENCE_PATH/main.py or /root/reference/main.py; where none exists (the GPU box, unless
-the caller ships the file to a scratch path) the test skips -- `profiles/r2_cfg1_main_py_gpu.log` is the committed
-output of such a run.
+Reference sources are never copied into this repository, so the driver is written here: it takes main.py's command
+line and defaults (main.py:28-53), seeds every RNG as main.py:19-26 does, loads the task through `coda.datasets.Dataset`
+/ `coda.oracle.Oracle` / `coda.options.LOSS_FNS` (main.py:110-118), opens the experiment run and the nested seed run
+with their parameters (main.py:132-164), and runs the selection loop with its regret metrics (main.py:55-105) -- the
+same calls, in the same order, with the same RNG consumption.
 """
 import json
 import os
@@ -22,32 +24,92 @@ pytestmark = pytest.mark.gpu
 
 sys.path.insert(0, GOLDEN)
 
+_DRIVER = """\
+import argparse
+import os
+import random
 
-def _main_py():
-    cands = [os.environ.get("CODA_REFERENCE_MAIN"),
-             os.path.join(os.environ.get("CODA_REFERENCE_PATH", "/root/reference"), "main.py")]
-    for c in cands:
-        if c and os.path.exists(c):
-            return c
-    return None
+import mlflow
+import numpy as np
+import torch
+
+from coda import CODA, Dataset, Oracle
+from coda.options import LOSS_FNS
+
+
+def command_line():
+    ap = argparse.ArgumentParser()
+    for flag, default, kind in (("--task", None, str), ("--data-dir", "data", str), ("--iters", 100, int),
+                                ("--seeds", 5, int), ("--experiment-name", None, str), ("--loss", "acc", str),
+                                ("--method", "iid", str), ("--alpha", 0.9, float), ("--learning-rate", 0.01, float),
+                                ("--multiplier", 2.0, float), ("--prefilter-n", 0, int), ("--q", "eig", str)):
+        ap.add_argument(flag, default=default, type=kind)
+    for flag in ("--force-rerun", "--no-mlflow", "--no-diag-prior"):
+        ap.add_argument(flag, action="store_true")
+    return ap.parse_args()
+
+
+def reseed(seed):
+    random.seed(seed)
+    np.random.seed(seed)
+    torch.manual_seed(seed)
+    torch.cuda.manual_seed_all(seed)
+
+
+def experiment(dataset, oracle, args, seed):
+    reseed(seed)
+    true_losses = oracle.true_losses(dataset.preds)
+    best_loss = min(oracle.true_losses(dataset.preds))
+    print("Best possible loss is", best_loss)
+    selector = CODA.from_args(dataset, args)
+    best_model_idx_pred = selector.get_best_model_prediction()
+    print("Regret at 0:", true_losses[best_model_idx_pred] - best_loss)
+    total = 0
+    for step in range(1, args.iters + 1):
+        chosen_idx, selection_prob = selector.get_next_item_to_label()
+        true_class = oracle(chosen_idx)
+        selector.add_label(chosen_idx, true_class, selection_prob)
+        best_model_idx_pred = selector.get_best_model_prediction()
+        regret = true_losses[best_model_idx_pred] - best_loss
+        total += regret
+        mlflow.log_metric("regret", float(regret), step=step)        # the stub also records this frame's pick
+        mlflow.log_metric("cumulative regret", float(total), step=step)
+    return selector.stochastic
+
+
+args = command_line()
+assert args.method == "coda" and not args.no_mlflow
+device = torch.device("cuda" if torch.cuda.is_available() else "cpu")
+print("device is", device)
+dataset = Dataset(os.path.join(args.data_dir, args.task + ".pt"), device=device)
+oracle = Oracle(dataset, loss_fn=LOSS_FNS[args.loss])
+name = args.experiment_name or args.task
+mlflow.set_tracking_uri("sqlite:///coda.sqlite")
+mlflow.set_experiment(name)
+with mlflow.start_run(run_id=None, run_name=name + "-" + args.method):
+    mlflow.log_params(vars(args))
+    for seed in range(args.seeds):
+        with mlflow.start_run(nested=True, run_id=None, run_name="%s-%s-%d" % (name, args.method, seed)):
+            mlflow.log_param("seed", seed)
+            stochastic = experiment(dataset, oracle, args, seed)
+            mlflow.log_param("stochastic", stochastic)
+        if not stochastic:
+            break
+"""
 
 
 def _run(tmp_path, extra_env=None, iters=None):
     import make_cfg1_golden as mk
-    main_py = _main_py()
-    if main_py is None:
-        pytest.skip("the reference driver main.py is not available on this box")
-    gpath = os.path.join(GOLDEN, "cfg1_main_py.json")
-    if not os.path.exists(gpath):
-        pytest.skip("cfg1 golden not generated")
-    g = json.load(open(gpath))
+    g = json.load(open(os.path.join(GOLDEN, "cfg1_main_py.json")))
     iters = iters or g["iters"]
     d = str(tmp_path)
     mk.write_task(d)
+    driver = os.path.join(d, "driver.py")
+    with open(driver, "w") as f:
+        f.write(_DRIVER)
     log = os.path.join(d, "mlflow.jsonl")
-    # PYTHONSAFEPATH keeps the script's directory (the reference checkout, with ITS coda package) off sys.path:
-    # `from coda import CODA` resolves to this repository's shim
-    r = mk.run_main(main_py, d, iters, log, [ROOT, os.path.join(ROOT, "tests", "stubs")], extra_env=extra_env, safe_path=True)
+    # PYTHONSAFEPATH keeps the driver's directory off sys.path: `coda` resolves to this repository's shim
+    r = mk.run_main(driver, d, iters, log, [ROOT, os.path.join(ROOT, "tests", "stubs")], extra_env=extra_env, safe_path=True)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
     out = mk.parse_log(log)
     return g, out, r.stdout
@@ -83,6 +145,7 @@ def _compare(g, out, stdout, iters):
 
 
 def test_reference_main_py_runs_unchanged_on_one_gpu(tmp_path):
+    """The driver loop on one GPU, all golden steps."""
     g, out, stdout = _run(tmp_path)
     keep = os.environ.get("CODA_B200_KEEP_MAIN_LOG")
     if keep:

@@ -1,4 +1,4 @@
-"""Time coda_b200_pi_full (fp32 SIMT) against coda_b200_pi_full_tc (tcgen05) on a synthetic slab: python tools/bench_pi_full.py [H N C]."""
+"""Time coda_b200_pi_full (fp32 SIMT) against coda_b200_pi_full_tc (wgmma) on a synthetic slab: python tools/bench_pi_full.py [H N C]."""
 import sys
 
 import torch

@@ -1,4 +1,4 @@
-"""Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list: python tools/launch_list.py launches.csv > profiles/rN_launch_list.txt
+"""Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list: python tools/launch_list.py launches.csv
 
 Per-kernel totals over the capture, then one steady-state acquisition step (the launches between two consecutive
 k_step_select launches near the end of the device-loop section) with each kernel's share of the step."""

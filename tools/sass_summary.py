@@ -1,5 +1,5 @@
-"""Per-kernel counts of the SASS mnemonics that prove tcgen05 / TMEM / bulk-TMA use (B200_PROFILING.md):
-    python tools/sass_summary.py > profiles/sass_summary.txt
+"""Per-kernel counts of the SASS mnemonics that prove wgmma / bulk-TMA use:
+    python tools/sass_summary.py
 """
 import collections
 import os
@@ -9,7 +9,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "coda_b200", "lib", "libcoda_b200.so")
-PAT = ["UTCHMMA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "UBLKCP", "UTMALDG", "SYNCS", "LDGSTS", "MUFU.LG2", "MUFU.EX2", "HMMA", "REDUX", "ATOMG", "RED."]
+PAT = ["HGMMA", "WARPGROUP", "UBLKCP", "UTMALDG", "SYNCS", "LDGSTS", "MUFU.LG2", "MUFU.EX2", "HMMA", "REDUX", "ATOMG", "RED."]
 
 
 def main():
@@ -32,8 +32,8 @@ def main():
             for p in PAT:
                 if p in line:
                     counts[cur][p] += 1
-    print(f"# cuobjdump -sass {os.path.relpath(LIB, ROOT)} (sm_100a): instruction counts per kernel")
-    print("# UTCHMMA = tcgen05.mma (bf16), LDTM = tcgen05.ld (TMEM -> registers), UTCBAR = tcgen05.commit, UBLKCP = cp.async.bulk (1-D TMA),")
+    print(f"# cuobjdump -sass {os.path.relpath(LIB, ROOT)} (sm_90a): instruction counts per kernel")
+    print("# HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / arrive, UBLKCP = cp.async.bulk (1-D TMA),")
     print("# SYNCS = mbarrier ops, MUFU.LG2/EX2 = the entropy / exp terms")
     print(f"{'kernel':70s} {'instr':>7s}  " + "  ".join(f"{p:>8s}" for p in PAT))
     for k, c in counts.items():

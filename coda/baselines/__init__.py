@@ -1,23 +1,17 @@
-"""The competing selectors (IID, Uncertainty, ActiveTesting, VMA, ModelPicker) are outside the scope of
-this package (SURVEY.md section 2, rows 7).  ``main.py`` imports their names unconditionally
-(main.py:10), so they resolve here: to the reference's own classes when a reference checkout is
-reachable through ``CODA_REFERENCE_PATH``, else to placeholders that raise on construction."""
+"""The competing selectors (IID, Uncertainty, ActiveTesting, VMA, ModelPicker) that ``main.py --method ...`` runs next
+to CODA (main.py:10, 67-80).  Resolution order:
+
+1. ``CODA_REFERENCE_PATH`` names a reference checkout whose ``coda/baselines/<name>.py`` modules load: the reference's
+   own classes, unchanged (they also take ``coda.baselines.<name>`` in ``sys.modules``, so
+   ``from coda.baselines.modelpicker import TASK_EPS`` then gets the reference's table);
+2. otherwise the GPU classes of ``coda_b200.baselines`` (one sm_90a device, dense slab; a CPU ``dataset.preds`` raises
+   ``NotImplementedError``)."""
 import importlib.util
 import os
 import sys
 
 _NAMES = {"IID": "iid", "ActiveTesting": "activetesting", "VMA": "vma", "ModelPicker": "modelpicker",
           "Uncertainty": "uncertainty"}
-
-
-def _placeholder(name):
-    class _Missing:
-        def __init__(self, *a, **k):
-            raise NotImplementedError(
-                f"coda.baselines.{name} is not part of coda_b200; set CODA_REFERENCE_PATH to a checkout of "
-                "justinkay/coda to use the reference implementation")
-    _Missing.__name__ = name
-    return _Missing
 
 
 def _load_reference(path):
@@ -42,5 +36,8 @@ if _ref and os.path.isdir(_ref):
         _loaded = _load_reference(_ref)
     except Exception:  # pragma: no cover - the reference needs matplotlib etc.
         _loaded = None
+if _loaded is None:
+    from coda_b200 import baselines as _ours
+    _loaded = {cls: getattr(_ours, cls) for cls in _NAMES}
 for _cls in _NAMES:
-    globals()[_cls] = _loaded[_cls] if _loaded else _placeholder(_cls)
+    globals()[_cls] = _loaded[_cls]

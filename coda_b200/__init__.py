@@ -11,6 +11,8 @@ from .datasets import (CompactDataset, CompactSlab, Dataset, ShardedFileDataset,
                        SyntheticDataset, TensorDataset)
 from .oracle import Oracle
 from .selector import CODA
+from .baselines import IID, VMA, ActiveTesting, ModelPicker, Uncertainty
 
 __all__ = ["CODA", "Dataset", "Oracle", "ModelSelector", "TensorDataset", "SyntheticDataset", "ShardedFileDataset",
-           "CompactSlab", "CompactDataset", "SyntheticCompactDataset"]
+           "CompactSlab", "CompactDataset", "SyntheticCompactDataset", "IID", "Uncertainty", "ActiveTesting", "VMA",
+           "ModelPicker"]

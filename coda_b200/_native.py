@@ -108,6 +108,13 @@ SIGNATURES = {
     "coda_b200_step_mixture": (i32, [PS, PX, p]),
     "coda_b200_ties": (i32, [p, i64, p, p, i64, p, i32, p, p, p, p]),
     "coda_b200_report_gather": (i32, [p, i32, p, PX, p, p]),
+    "coda_b200_mp_entropy": (i32, [p, p, i32, i64, i32, f64, p, p, i32, p, p]),
+    "coda_b200_static_scores": (i32, [p, p, i32, i64, i32, p, p, p]),
+    "coda_b200_select_blocks": (i32, [i64]),
+    "coda_b200_weighted_total": (i32, [p, p, i64, p, p, p]),
+    "coda_b200_weighted_draw": (i32, [p, p, i64, p, f64, p, p, p]),
+    "coda_b200_select_extreme": (i32, [p, p, i64, i32, p, p, p]),
+    "coda_b200_select_kth": (i32, [p, p, i64, p, p, i64, p, p]),
 }
 
 

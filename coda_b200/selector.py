@@ -238,8 +238,8 @@ class CODA(ModelSelector):
             if getattr(self, "_ens_entropy", None) is None:      # non-adaptive: computed once (uncertainty.py:6-11)
                 if self.engine.ens is None:
                     raise RuntimeError("q='uncertainty' needs the ensemble sums (CODA_B200_ENS=0 disables them)")
-                mean = self._cat("ens") / float(self.H)
-                self._ens_entropy = -(mean * torch.log(mean + 1e-8)).sum(-1)
+                from .baselines import ensemble_entropy
+                self._ens_entropy = ensemble_entropy(self._cat("ens"), self.H)
             qv = self._ens_entropy
         best = qv[mask].max()
         ties = torch.isclose(qv, best, rtol=1e-8) & mask        # coda.py:307

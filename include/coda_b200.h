@@ -316,6 +316,45 @@ int coda_b200_ties(const float* eig, int64_t N, const uint8_t* labeled, const ui
 int coda_b200_report_gather(const int64_t* rep, int rep_words, int64_t* rep_all, const coda_xchg_t* x,
                             uint32_t* flags, coda_stream_t stream);
 
+/* ---- competing selectors (coda/baselines/<name>.py), over the products of coda_b200_scan_slab ----------------------
+ * One shard, dense slab.  Per-item vectors are [N] over all items; `labeled` [N] u8 marks the items already labeled. */
+
+/* ModelPicker acquisition, modelpicker.py:58-86 (the C-class loop at 74-86 with (N, H) temporaries per class).
+ * For item n let Z_c be the models predicting class c, A_c = sum_{h in Z_c} p_h, Q_c = sum_{h in Z_c} p_h log2 p_h,
+ * S = sum p, B = sum p log2 p (0 log 0 = 0), g = gamma:  H_c = log2(S + (g-1) A_c) - (B + (g-1) Q_c + g log2(g) A_c) /
+ * (S + (g-1) A_c); a class no model predicts gives log2 S - B / S; ent[n] = mean over the C classes, accumulated in
+ * fp64 per item with the groups taken in the order of their lowest model index, rounded once.  The 1e-12 clamp of
+ * modelpicker.py:83 is not applied (its effect is below H * 4e-11).  ent[n] = +inf for labeled items and, when
+ * mask_agreeing != 0, for items every model agrees on (modelpicker.py:64-66). */
+int coda_b200_mp_entropy(const uint16_t* hard, const float* posterior /*[H]*/, int H, int64_t N, int C, double gamma,
+                         const uint8_t* labeled, const uint8_t* disagree, int mask_agreeing, float* ent,
+                         coda_stream_t stream);
+/* Static acquisition scores from l_h = 1 - ens[n][hard[n][h]] / H (the mean-ensemble surrogate, activetesting.py:18, 33):
+ * at_score[n] = sum_h l_h (activetesting.py:33-44), vma_score[n] = sum_{h < h'} |l_h - l_h'| (vma.py:18-41, the
+ * H x H x |D_U| tensor of vma.py:31), both over the item's distinct predicted classes with multiplicities.
+ * Either output may be NULL. */
+int coda_b200_static_scores(const uint16_t* hard, const float* ens, int H, int64_t N, int C, float* at_score,
+                            float* vma_score, coda_stream_t stream);
+/* number of partial records of the selection calls below (per-block chunks of the item axis) */
+int coda_b200_select_blocks(int64_t N);
+/* random.choices(d_u_idxs, weights) (activetesting.py:45-48, vma.py:44-60).  weighted_total: total[0] = fp64 sum of w
+ * over the unlabeled items, total[1] = their count.  weighted_draw: the weights w / (float)total[0] (fp32 division,
+ * the normalisation of activetesting.py:44), their running fp64 sum cum in index order, and the first unlabeled item
+ * with cum > u * cum_total (bisect_right, the last one if none) -> out = {position among the unlabeled items, item,
+ * float bits of its normalised weight}.  u = random.random() drawn by the caller.  partials: 2 * select_blocks doubles. */
+int coda_b200_weighted_total(const float* w, const uint8_t* labeled, int64_t N, double* partials, double* total /*[2]*/,
+                             coda_stream_t stream);
+int coda_b200_weighted_draw(const float* w, const uint8_t* labeled, int64_t N, const double* total, double u,
+                            double* partials, int64_t* out /*[3]*/, coda_stream_t stream);
+/* Minimum (want_max = 0, modelpicker.py:68-69) or maximum (uncertainty.py:37-38) of v over the unlabeled items and the
+ * number of items exactly equal to it: out = {float bits, count}; partials: 2 * select_blocks int64.  select_kth: the
+ * k-th (ascending index, from 0) unlabeled item equal to best[0] (modelpicker.py:70, uncertainty.py:39-43), from the
+ * partials of the select_extreme call that produced `best`; -1 if there is none. */
+int coda_b200_select_extreme(const float* v, const uint8_t* labeled, int64_t N, int want_max, int64_t* partials,
+                             int64_t* out /*[2]*/, coda_stream_t stream);
+int coda_b200_select_kth(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
+                         const int64_t* best, int64_t k, int64_t* out_idx /*[1]*/, coda_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

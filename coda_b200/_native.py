@@ -49,7 +49,7 @@ class StepStruct(C.Structure):
         ("H", i32), ("C", i32), ("N", i64), ("n_offset", i64), ("fx_shift", i32), ("lr", f32),
         ("hard", p), ("labeled", p), ("D", p), ("jvec", p), ("sel", p),
         ("terms", p), ("slot_of_model", p), ("shadow_off", i64), ("shadow_col_stride", i64), ("model_stride", i64),
-        ("have_ens", i32), ("compact_k", i32),
+        ("ens_off", i64), ("ens_col_stride", i64), ("have_ens", i32), ("compact_k", i32),
         ("pisum_fx", p), ("PB", p), ("pi_hat", p), ("m0", p), ("h_before", p), ("best_model", p),
         ("partials", p), ("nblocks", i32), ("eig", p), ("bestrec", p),
         ("labels_global", p), ("hist_idx", p), ("hist_q", p), ("hist_tie", p), ("hist_cap", i64), ("step_ctr", p),

@@ -660,8 +660,7 @@ __constant__ R1Term c_terms_bank[R1_CONST_TERMS];
 // GU: gathers in flight per lane, NR: U rows in flight per warp (more of both = more bytes in flight per SM at
 // the price of registers / resident warps)
 template <int KC, int GU = 16, int NR = 4, bool CONST_TERMS = false>
-__global__ void __launch_bounds__(256, (GU > 16 ? 3 : 4)) k_pi_rank1(const float* __restrict__ preds, const float* __restrict__ E,
-                                                  long long N, int C, const long long* __restrict__ sel,
+__global__ void __launch_bounds__(256, (GU > 16 ? 3 : 4)) k_pi_rank1(const float* __restrict__ preds, long long N, int C, const long long* __restrict__ sel,
                                                   const int32_t* __restrict__ hdr, const R1Term* __restrict__ gterms,
                                                   int const_base, float lr, float fxs,
                                                   float* __restrict__ U, unsigned long long* __restrict__ pisum_fx,
@@ -671,7 +670,7 @@ __global__ void __launch_bounds__(256, (GU > 16 ? 3 : 4)) k_pi_rank1(const float
   R1Term* s_terms = reinterpret_cast<R1Term*>(wacc_all + (size_t)8 * C);        // [nt] gather list (broadcast reads)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t = (int)sel[1];
-  const int nt = hdr[0], tp = hdr[1];
+  const int nt = hdr[0];
   if (!CONST_TERMS)
     for (int k = threadIdx.x; k < nt; k += blockDim.x) s_terms[k] = gterms[k];
   const R1Term* c_terms = CONST_TERMS ? (c_terms_bank + const_base) : s_terms;
@@ -689,7 +688,6 @@ __global__ void __launch_bounds__(256, (GU > 16 ? 3 : 4)) k_pi_rank1(const float
     const long long n = n0 + lane;
     float d = 0.f;
     if (n < N) {
-      if (tp >= 0) d = __ldg(E + (size_t)n * C + tp);
       int k = 0;
       for (; k + GU <= nt; k += GU) {
         float v[GU];
@@ -737,8 +735,7 @@ __global__ void __launch_bounds__(256, (GU > 16 ? 3 : 4)) k_pi_rank1(const float
 // four times fewer DRAM page switches for the same bytes.  Same arithmetic, same order as k_pi_rank1.
 #define R1V_WI 128     // items per warp
 template <int KC>
-__global__ void __launch_bounds__(256, 3) k_pi_rank1_v4(const float* __restrict__ preds, const float* __restrict__ E,
-                                                     long long N, int C, const long long* __restrict__ sel,
+__global__ void __launch_bounds__(256, 3) k_pi_rank1_v4(const float* __restrict__ preds, long long N, int C, const long long* __restrict__ sel,
                                                      const int32_t* __restrict__ hdr, const R1Term* __restrict__ gterms,
                                                      float lr, float fxs, float* __restrict__ U,
                                                      unsigned long long* __restrict__ pisum_fx,
@@ -748,7 +745,7 @@ __global__ void __launch_bounds__(256, 3) k_pi_rank1_v4(const float* __restrict_
   R1Term* c_terms = reinterpret_cast<R1Term*>(wacc_all + (size_t)8 * C);        // [nt]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t = (int)sel[1];
-  const int nt = hdr[0], tp = hdr[1];
+  const int nt = hdr[0];
   for (int k = threadIdx.x; k < nt; k += blockDim.x) c_terms[k] = gterms[k];
   long long racc[KC];
 #pragma unroll
@@ -760,11 +757,6 @@ __global__ void __launch_bounds__(256, 3) k_pi_rank1_v4(const float* __restrict_
     const long long nl = n0 + 4 * lane;
     const bool full4 = nl + 3 < N;
     float d[4] = {0.f, 0.f, 0.f, 0.f};
-    if (tp >= 0) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        if (nl + i < N) d[i] = __ldg(E + (size_t)(nl + i) * C + tp);
-    }
     int k = 0;
     for (; k + 8 <= nt; k += 8) {
       float v[8][4];
@@ -836,7 +828,7 @@ __global__ void __launch_bounds__(256, 3) k_pi_rank1_v4(const float* __restrict_
 
 template <int KC>
 __global__ void __launch_bounds__(R1X_THREADS, 1) k_pi_rank1_tma(const float* __restrict__ preds,
-                                                                 const float* __restrict__ E, long long N, int C, int TR,
+                                                                 long long N, int C, int TR,
                                                                  const long long* __restrict__ sel,
                                                                  const int32_t* __restrict__ hdr,
                                                                  const R1Term* __restrict__ gterms, float lr, float fxs,
@@ -845,7 +837,7 @@ __global__ void __launch_bounds__(R1X_THREADS, 1) k_pi_rank1_tma(const float* __
                                                                  uint32_t* __restrict__ flags) {
   extern __shared__ __align__(128) unsigned char smem_r1x[];
   unsigned char* smem_raw = smem_r1x;
-  const int nt = hdr[0], tp = hdr[1];
+  const int nt = hdr[0];
   const int t = (int)sel[1];
   const size_t u_bytes = ((size_t)TR * C * 4 + 127) & ~(size_t)127;
   float* Ut = reinterpret_cast<float*>(smem_raw);                                        // [TR][C]
@@ -925,7 +917,6 @@ __global__ void __launch_bounds__(R1X_THREADS, 1) k_pi_rank1_tma(const float* __
     const long long n = n0 + li;
     const bool valid = li < rows;
     float d = 0.f;
-    if (valid && tp >= 0) d = __ldg(E + (size_t)n * C + tp);
     int shi = 0;                                     // shadow terms consumed in this tile
     const float* slot = ring;
     for (int k = 0; k < nt; ++k) {
@@ -1024,9 +1015,11 @@ extern "C" int coda_b200_pi_rank1(const float* preds, const float* ens, int H, i
   const R1Term* tlist = reinterpret_cast<const R1Term*>(terms + 2);            // <= 2H x 16 bytes
   cudaStream_t st = as_stream(stream);
   // bulk-TMA pipeline: C <= 128, 16-byte aligned U / preds / E, item counts that keep every bulk copy aligned
-  // variants (identical bits): "v1" one item per lane (default; measured fastest: 0.40 ms at cfg3), "v4" four items
-  // per lane / 512-byte runs per term (0.51 ms), "tma" the bulk-TMA pipeline (1.2 ms: 8 consumer warps per SM in
-  // lock-step phases).  CODA_B200_R1 selects one for A/B runs.
+  // variants (identical bits): "v1" one item per lane (default), "v4" four items per lane / 512-byte runs per term,
+  // "tma" the bulk-TMA pipeline (8 consumer warps per SM in lock-step phases).  On an H100 (400 W) at cfg3 with 140
+  // shadow models, whole-step rates of the graph loop: v1 580-620 steps/s, v1d 583-598, v4 548-563, tma 486-497; v1 at
+  // 8 CTAs per SM or one CTA per 256 items instead of 4 per SM, and a grid that leaves an eighth of the SMs to the side
+  // stream (527-530), were not better.  CODA_B200_R1 selects one for A/B runs.
   const char* r1env = getenv("CODA_B200_R1");
   const bool want_tma = r1env && r1env[0] == 't';
   const bool want_v1 = !(r1env && r1env[0] == 'v' && r1env[1] == '4');
@@ -1045,7 +1038,7 @@ extern "C" int coda_b200_pi_rank1(const float* preds, const float* ens, int H, i
 #define LAUNCH_R1X(KC)                                                                                              \
   do {                                                                                                              \
     CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1_tma<KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_x)); \
-    k_pi_rank1_tma<KC><<<gridx, R1X_THREADS, smem_x, st>>>(preds, ens, N, C, TR, reinterpret_cast<const long long*>(sel), \
+    k_pi_rank1_tma<KC><<<gridx, R1X_THREADS, smem_x, st>>>(preds, N, C, TR, reinterpret_cast<const long long*>(sel), \
                                                           hdr, tlist, (float)lr, exp2f((float)fx_shift), U,        \
                                                           reinterpret_cast<unsigned long long*>(pisum_fx), flags); \
   } while (0)
@@ -1066,7 +1059,7 @@ extern "C" int coda_b200_pi_rank1(const float* preds, const float* ens, int H, i
 #define LAUNCH_R1V(KC)                                                                                            \
   do {                                                                                                            \
     CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1_v4<KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    k_pi_rank1_v4<KC><<<grid4, 256, smem, st>>>(preds, ens, N, C, reinterpret_cast<const long long*>(sel), hdr,   \
+    k_pi_rank1_v4<KC><<<grid4, 256, smem, st>>>(preds, N, C, reinterpret_cast<const long long*>(sel), hdr,   \
                                                tlist, (float)lr, exp2f((float)fx_shift), U,                       \
                                                reinterpret_cast<unsigned long long*>(pisum_fx), flags);           \
   } while (0)
@@ -1091,19 +1084,19 @@ extern "C" int coda_b200_pi_rank1(const float* preds, const float* ens, int H, i
   do {                                                                                                         \
     if (use_const) {                                                                                           \
       CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1<KC, 16, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-      k_pi_rank1<KC, 16, 4, true><<<grid, 256, smem, st>>>(preds, ens, N, C, reinterpret_cast<const long long*>(sel), hdr, \
+      k_pi_rank1<KC, 16, 4, true><<<grid, 256, smem, st>>>(preds, N, C, reinterpret_cast<const long long*>(sel), hdr, \
                                             tlist, const_base, (float)lr, exp2f((float)fx_shift), U,           \
                                             reinterpret_cast<unsigned long long*>(pisum_fx), flags);           \
       break;                                                                                                   \
     }                                                                                                          \
     CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1<KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    k_pi_rank1<KC><<<grid, 256, smem, st>>>(preds, ens, N, C, reinterpret_cast<const long long*>(sel), hdr,    \
+    k_pi_rank1<KC><<<grid, 256, smem, st>>>(preds, N, C, reinterpret_cast<const long long*>(sel), hdr,    \
                                             tlist, 0, (float)lr, exp2f((float)fx_shift), U,                    \
                                             reinterpret_cast<unsigned long long*>(pisum_fx), flags);           \
   } while (0)
   if (want_deep && C > 64 && C <= 128) {
     CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1<4, 32, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_pi_rank1<4, 32, 8><<<grid, 256, smem, st>>>(preds, ens, N, C, reinterpret_cast<const long long*>(sel), hdr, tlist, 0,
+    k_pi_rank1<4, 32, 8><<<grid, 256, smem, st>>>(preds, N, C, reinterpret_cast<const long long*>(sel), hdr, tlist, 0,
                                                   (float)lr, exp2f((float)fx_shift), U,
                                                   reinterpret_cast<unsigned long long*>(pisum_fx), flags);
     CODA_LAUNCH_OK("k_pi_rank1<deep>");

@@ -47,8 +47,15 @@ __device__ void apply_label(const coda_step_t& a, int t, const int* jv, int* cnt
   __syncthreads();
   const int tp = s_tp, M = s_m;
   const bool ens = a.have_ens && 2 * M < H;
+  // dense slab: the shortcut's base E[n][t'] is the first term of the list, read like any other term (coalesced from
+  // the class-major ensemble slot when there is one); the compact kernels load it themselves from hdr[1]
+  const bool ens_term = ens && a.compact_k == 0;
+  if (ens_term && tid == 0) {
+    const bool cm = a.ens_col_stride > 0;
+    terms[0] = R1Term{a.ens_off + (long long)tp * (cm ? a.ens_col_stride : 1), 1.f, cm ? 1 : C};
+  }
   // every model contributes 1 (direct), or 0 / 2 (ensemble shortcut) terms: exclusive scan over models, in order
-  int carry = 0;
+  int carry = ens_term ? 1 : 0;
   const int lane = tid & 31, warp = tid >> 5;
   for (int h0 = 0; h0 < H; h0 += ST_THREADS) {
     const int h = h0 + tid;

@@ -60,6 +60,16 @@ def _ptr(t):
     return t.data_ptr() if t is not None else None
 
 
+def shadow_slots(free: int, reserve: int, slot_bytes: int, want: int, ens: bool, left: int = 1, total: int = 1):
+    """-> (model slots, ensemble slots) of one shard's shadow.  ``free``: device bytes free now; ``total`` shards on
+    the device keep ``reserve`` bytes each, and the ``left`` shards still to be sized (this one included) split the rest
+    equally.  The ensemble slot (one per step, in every list with the majority shortcut) comes first, then up to
+    ``want`` models."""
+    n = max(0, (free - total * reserve) // max(1, left) // slot_bytes)
+    ne = 1 if ens and n >= 1 else 0
+    return int(max(0, min(want, n - ne))), ne
+
+
 class Engine:
     rep_words = REP_WORDS
 
@@ -256,6 +266,12 @@ class Engine:
         st.shadow_off = ((self.shadow.data_ptr() - self._slab_ptr()) // 4) if self.shadow is not None else 0
         st.shadow_col_stride = self.shadow_cs
         st.model_stride = self.model_stride
+        if self.shadow is not None and self.shadow.shape[0] > self.n_shadow:     # class-major ensemble slot
+            st.ens_off = (self.shadow[self.n_shadow].data_ptr() - self._slab_ptr()) // 4
+            st.ens_col_stride = self.shadow_cs
+        else:
+            st.ens_off = ((self.ens.data_ptr() - self._slab_ptr()) // 4) if self.ens is not None else 0
+            st.ens_col_stride = 0
         st.have_ens = 1 if self.ens is not None else 0
         st.compact_k = self.K if self.compact is not None else 0
         st.pisum_fx, st.PB, st.pi_hat, st.m0 = _ptr(self.pisum), _ptr(self.PB), _ptr(self.pi_hat), _ptr(self.m0)
@@ -305,9 +321,14 @@ class Engine:
             self.conf_fx = self.conf_rest = self.conf_buf = None    # H*C*C int64, only needed once
             self._marginals_full()
             self._build_rows()
-            self._build_shadow()
+
+    def construct_tables(self, left: int = 1, total: int = 1):
+        """Shadow slab, step struct and class tables.  Runs after every shard of the device has its row cache;
+        ``left`` / ``total``: shards on this device that have still to build a shadow (this one included) / in all."""
+        with self._on():
+            self._build_shadow(left, total)
             self._make_step_struct()
-            self._tables(0, C)
+            self._tables(0, self.C)
             self.cache_valid = False     # incremental mode: P(best | hypothetical) rows are cached once scored
             self.pending = False         # a side-stream refresh the next scoring pass has to join
             self.scored = False          # block records (`partials`) are current
@@ -454,36 +475,54 @@ class Engine:
             else:
                 self.ph_cache = self._e((self.npairs, self.Hp), torch.float32)
 
-    def _build_shadow(self):
-        """Class-major shadow copy of as many models as spare HBM allows (least accurate first)."""
+    def shadow_reserve(self) -> int:
+        """Device bytes this shard leaves free when it sizes its shadow: what it still allocates after construction
+        (the largest is a U-sized ``pi_hat_xi`` read-out; graph instantiation, lazily loaded kernels, the report and
+        history read-outs are small) plus a 1 GiB margin for the caller.  ``CODA_B200_SHADOW_RESERVE_GB`` overrides."""
+        env = os.environ.get("CODA_B200_SHADOW_RESERVE_GB")
+        if env is not None:
+            return int(float(env) * 2 ** 30)
+        return 4 * self.N * self.C + (1 << 30)
+
+    def _build_shadow(self, left: int = 1, total: int = 1):
+        """Class-major shadow copy of the ensemble sums and of as many models as spare HBM allows (least accurate
+        first): slots [0, n_shadow) hold models, slot n_shadow (when present) holds E.  ``left`` / ``total``: shards on
+        this device that have still to build a shadow (this one included) / in all -- each takes an equal share of
+        what is free once every shard's reserve is set aside."""
         self.shadow, self.slot_of_model, self.n_shadow, self.shadow_cs = None, None, 0, 0
         if self.mode == "recompute_all" or os.environ.get("CODA_B200_SHADOW", "1") == "0" or self.compact is not None:
             return
         H, N, C = self.H, self.N, self.C
         cs = (N + 3) // 4 * 4                                   # every (slot, class) column starts 16-byte aligned
-        torch.cuda.synchronize(self.dev)
-        torch.cuda.empty_cache()
-        free, _total = torch.cuda.mem_get_info(self.dev)
-        reserve = int(float(os.environ.get("CODA_B200_SHADOW_RESERVE_GB", "8")) * 2 ** 30)
-        per_model = cs * C * 4
-        S = int(min(H, max(0, (free - reserve) // per_model)))
         cap = os.environ.get("CODA_B200_SHADOW_MODELS")
-        if cap is not None:
-            S = min(S, int(cap))
-        if S <= 0:
+        want = H if cap is None else max(0, min(H, int(cap)))
+        order = None
+        if want > 0:
+            # disagreement of every model with the ensemble pseudo-label: the models that will need gathers most often
+            dis = torch.zeros(H, dtype=torch.int64, device=self.dev)
+            step = max(1, (64 << 20) // max(1, H))
+            for n0 in range(0, N, step):
+                blk = self.hard[n0:n0 + step].to(torch.int32) & 0xFFFF
+                dis += (blk != self.pseudo[n0:n0 + step, None]).sum(0)
+            order = torch.argsort(dis, descending=True, stable=True).to(torch.int32)
+            del dis, blk
+        torch.cuda.synchronize(self.dev)
+        torch.cuda.empty_cache()                                # the temporaries above are not spare memory
+        free, _total = torch.cuda.mem_get_info(self.dev)
+        S, ne = shadow_slots(free, self.shadow_reserve(), cs * C * 4, want, self.ens is not None, left, total)
+        if S + ne == 0:
             return
-        # disagreement of every model with the ensemble pseudo-label: the models that will need gathers most often
-        dis = torch.zeros(H, dtype=torch.int64, device=self.dev)
-        step = max(1, (64 << 20) // max(1, H))
-        for n0 in range(0, N, step):
-            blk = self.hard[n0:n0 + step].to(torch.int32) & 0xFFFF
-            dis += (blk != self.pseudo[n0:n0 + step, None]).sum(0)
-        order = torch.argsort(dis, descending=True, stable=True)[:S].to(torch.int32)
         slot = torch.full((H,), -1, dtype=torch.int32, device=self.dev)
-        slot[order.long()] = torch.arange(S, dtype=torch.int32, device=self.dev)
-        self.shadow = self._e((S, C, cs), torch.float32)
-        self._call("coda_b200_shadow_build", _ptr(self.preds), self.model_stride, H, N, C, _ptr(order), S, cs,
-                   _ptr(self.shadow), self._s())
+        self.shadow = self._e((S + ne, C, cs), torch.float32)
+        if S > 0:
+            order = order[:S].contiguous()
+            slot[order.long()] = torch.arange(S, dtype=torch.int32, device=self.dev)
+            self._call("coda_b200_shadow_build", _ptr(self.preds), self.model_stride, H, N, C, _ptr(order), S, cs,
+                       _ptr(self.shadow), self._s())
+        if ne:                                                  # E [N][C] is a one-model slab
+            first = torch.zeros(1, dtype=torch.int32, device=self.dev)
+            self._call("coda_b200_shadow_build", _ptr(self.ens), N * C, 1, N, C, _ptr(first), 1, cs,
+                       _ptr(self.shadow[S]), self._s())
         self.slot_of_model, self.n_shadow, self.shadow_cs = slot, S, cs
 
     # ------------------------------------------------------------------------ step pieces (enqueue only)
@@ -881,6 +920,15 @@ def build_engines(shards, group, **kw):
     group.allreduce_sum_([e.conf_buf for e in engines])         # coda.py:42 sums over ALL items
     for e in engines:
         e.construct_posterior()
+    # shadows last: every row cache of a device is in place before any shadow takes what is left, and shards that
+    # share a device split what is left between them
+    total = {}
+    for e in engines:
+        total[e.dev] = total.get(e.dev, 0) + 1
+    left = dict(total)
+    for e in engines:
+        e.construct_tables(left[e.dev], total[e.dev])
+        left[e.dev] -= 1
     for e in engines:
         e.construct_mixture()
     for e in engines:

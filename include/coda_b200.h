@@ -141,7 +141,9 @@ int coda_b200_shadow_build(const float* preds, int64_t model_stride, int H, int6
  * then the same normalise + column sums as pi_reduce.  The gather list (`terms`, written by the step kernels
  * below) is {nterms, majority class t' or -1} followed by nterms x {element offset, sign, item stride}: with the
  * ensemble sums E the sum over models is taken as E[n][t'] + corrections for the models that disagree with the
- * majority class t' of jvec (exact algebra, fewer gathers); models with a shadow slot are read from the shadow.
+ * majority class t' of jvec (exact algebra, fewer gathers); E[n][t'] is the first term of the list (from the
+ * shadow's class-major ensemble slot, else from the item-major ens), models with a shadow slot are read from the
+ * shadow.  `ens` is not read here: the list addresses the ensemble sums itself.
  * pisum_fx was zeroed by the step kernel and is accumulated into (this shard's sums).  ctas_per_sm (1..8)
  * bounds the grid so a concurrent stream keeps SM resources.  U must be 16-byte aligned and followed by 16
  * readable bytes (C <= 128 takes a bulk-TMA pipeline that rounds the last tile's copy up). */
@@ -271,6 +273,9 @@ typedef struct coda_step { /* host struct: this shard's device state */
   int32_t* terms; /* [2 + 8H] */
   const int32_t* slot_of_model;
   int64_t shadow_off, shadow_col_stride, model_stride;
+  /* ensemble sums E (the majority shortcut's first term): element offset of E[item 0][class 0] relative to preds and
+   * the class stride of a class-major copy (item stride 1), or 0 for the item-major [N][C] ens (item stride C) */
+  int64_t ens_off, ens_col_stride;
   int have_ens;
   int compact_k; /* > 0: the slab is in the compact top-K form, the gather list names (model, class) pairs */
   /* marginals / mixture */

@@ -29,6 +29,18 @@ FLAG_XCHG_TIMEOUT = 0x80
 FLAG_NEGATIVE_PROB = 0x100
 FLAG_ROWSUM_WARN = 0x200
 FLAG_PIPELINE_TIMEOUT = 0x400
+SLAB_F32, SLAB_F16, SLAB_BF16 = 0, 1, 2
+
+
+def slab_format(dtype) -> int:
+    """CODA_B200_SLAB_* code of a prediction-slab dtype (fp32, fp16, bf16); TypeError for any other."""
+    import torch
+    fmt = {torch.float32: SLAB_F32, torch.float16: SLAB_F16, torch.bfloat16: SLAB_BF16}.get(dtype)
+    if fmt is None:
+        raise TypeError(f"coda_b200: preds must be a float32, float16 or bfloat16 (H, N, C) tensor, got {dtype}")
+    return fmt
+
+
 FLAG_NAMES = {
     FLAG_NONFINITE_INPUT: "preds", FLAG_RANGE_INPUT: "preds range", FLAG_NONFINITE_TABLE: "pdf/cdf/integrand",
     FLAG_NONFINITE_PI: "pi_hat_xi", FLAG_NONFINITE_PBEST: "Pbest", FLAG_NONFINITE_EIG: "Pbest(beta) normalized",
@@ -91,6 +103,14 @@ SIGNATURES = {
     "coda_b200_pi_reduce": (i32, [p, i64, i32, i32, p, p, p, p]),
     "coda_b200_shadow_build": (i32, [p, i64, i32, i64, i32, p, i32, i64, p, p]),
     "coda_b200_pi_rank1": (i32, [p, p, i32, i64, i32, p, f64, i32, p, p, p, p, i32, i32, p]),
+    "coda_b200_scan_slab_x": (i32, [p, i32, i64, i32, i64, i32, p, p, p, p, p, p]),
+    "coda_b200_confusion_accum_x": (i32, [p, i32, i64, p, i32, i64, i32, i32, p, p]),
+    "coda_b200_confusion_sorted_x": (i32, [p, i32, i64, p, p, i32, i64, i32, i32, p, p]),
+    "coda_b200_pi_full_x": (i32, [p, i32, i64, p, i32, i64, i32, p, p]),
+    "coda_b200_pi_full_tc_ok_x": (i32, [i32, i32, i64, i32, i64]),
+    "coda_b200_pi_full_tc_x": (i32, [p, i32, i64, p, i32, i64, i32, p, p, p, p]),
+    "coda_b200_shadow_build_x": (i32, [p, i32, i64, i32, i64, i32, p, i32, i64, p, p]),
+    "coda_b200_pi_rank1_x": (i32, [p, i32, p, i32, i64, i32, p, f64, i32, p, p, p, p, i32, i32, p]),
     "coda_b200_tables_scratch_bytes": (sz, [i32, i32]),
     "coda_b200_beta_tables": (i32, [p, p, i32, i32, i32, f64, i32, i32, p, p, p, p, p, p, p, p, p, p]),
     "coda_b200_pair_count": (i32, [p, i32, i64, i32, p, p, p, p]),

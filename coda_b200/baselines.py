@@ -80,8 +80,9 @@ class _DeviceState:
         if default_comm().world > 1:
             raise NotImplementedError("coda_b200.baselines: one process per GPU (a torch.distributed group of world > 1) "
                                       "is not supported; the baselines run on one GPU")
-        if preds.dtype != torch.float32 or preds.dim() != 3:
-            raise TypeError("coda_b200: preds must be a float32 (H, N, C) tensor (coda/datasets.py:14)")
+        self.fmt = nat.slab_format(preds.dtype)      # float32, float16 or bfloat16 (read at its stored width)
+        if preds.dim() != 3:
+            raise TypeError("coda_b200: preds must be an (H, N, C) tensor (coda/datasets.py:14)")
         H, N, C = (int(s) for s in preds.shape)
         if int(getattr(dataset, "n_global", N)) != N:
             raise NotImplementedError("coda_b200.baselines: an N-range shard of a task is not supported; the baselines "
@@ -119,8 +120,12 @@ class _DeviceState:
             pseudo = torch.empty(N, dtype=torch.int32, device=self.dev)
             disagree = torch.empty(N, dtype=torch.uint8, device=self.dev)
             e = torch.empty((N, C), dtype=torch.float32, device=self.dev) if ens else None
-            self._call("coda_b200_scan_slab", _ptr(self.preds), self.model_stride, H, N, C, _ptr(hard), _ptr(pseudo),
-                       _ptr(disagree), _ptr(e), _ptr(self.flags), self._s())
+            if self.fmt == nat.SLAB_F32:
+                self._call("coda_b200_scan_slab", _ptr(self.preds), self.model_stride, H, N, C, _ptr(hard), _ptr(pseudo),
+                           _ptr(disagree), _ptr(e), _ptr(self.flags), self._s())
+            else:
+                self._call("coda_b200_scan_slab_x", _ptr(self.preds), self.fmt, self.model_stride, H, N, C, _ptr(hard),
+                           _ptr(pseudo), _ptr(disagree), _ptr(e), _ptr(self.flags), self._s())
             flags = int(self.flags.item())
         if flags & nat.FLAG_NONFINITE_INPUT:
             raise RuntimeError("[NUMERIC ERROR] preds has bad values (NaN/Inf)")
@@ -232,7 +237,8 @@ class IID(_Baseline):
     def add_label(self, chosen_idx, true_class, selection_prob=None):
         self._record(chosen_idx, true_class)
         # the per-label losses added in label order: the sum iid.py:37-43 recomputes from scratch
-        self._risk_sum += self.loss_fn(self.dataset.preds[:, chosen_idx, :],
+        # (a 16-bit slab's scores are widened first: the loss sees the fp32 values the reference loader would produce)
+        self._risk_sum += self.loss_fn(self.dataset.preds[:, chosen_idx, :].float(),
                                        torch.tensor([true_class], device=self.device).expand(self.H))
 
     def get_risk_estimates(self):
@@ -305,7 +311,7 @@ class ActiveTesting(IID):
 
     def add_label(self, chosen_idx, true_class, selection_prob=None):
         self._record(chosen_idx, true_class)
-        self.losses.append(self.loss_fn(self.dataset.preds[:, chosen_idx, :],
+        self.losses.append(self.loss_fn(self.dataset.preds[:, chosen_idx, :].float(),
                                         torch.tensor([true_class], device=self.device).repeat(self.H), reduction="none"))
         self.qs.append(selection_prob)
         self.M += 1

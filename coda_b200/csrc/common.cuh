@@ -1,6 +1,8 @@
 // Shared device/host helpers for the coda_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_fp16.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -42,6 +44,27 @@ void coda_set_error(const char* fmt, ...);
   } while (0)
 
 static inline cudaStream_t as_stream(coda_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
+
+// ---- slab element types ----------------------------------------------------------------
+// The prediction slab may be stored as fp32, fp16 or bf16 (CODA_B200_SLAB_*).  Every kernel that reads it widens the
+// value to fp32 at the load and does the rest in fp32, so a 16-bit slab gives the bits of its exact fp32 widening.
+__device__ __forceinline__ float slab_f(float v) { return v; }
+__device__ __forceinline__ float slab_f(__half v) { return __half2float(v); }
+__device__ __forceinline__ float slab_f(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <typename T>
+__device__ __forceinline__ float ldg_f(const T* p) { return slab_f(__ldg(p)); }
+
+// fn((const T*)preds) for the element type named by `fmt`
+template <typename Fn>
+static inline int slab_dispatch(int fmt, const void* preds, Fn&& fn) {
+  switch (fmt) {
+    case CODA_B200_SLAB_F32: return fn(static_cast<const float*>(preds));
+    case CODA_B200_SLAB_F16: return fn(static_cast<const __half*>(preds));
+    case CODA_B200_SLAB_BF16: return fn(static_cast<const __nv_bfloat16*>(preds));
+  }
+  coda_set_error("unknown slab format %d (CODA_B200_SLAB_F32 / F16 / BF16)", fmt);
+  return CODA_B200_EINVAL;
+}
 
 int coda_sm_count();   // cached multiprocessor count of the current device
 

@@ -22,10 +22,15 @@
 // k_pi_w_limbs in the K-major core-matrix order) is read by wgmma straight from the staged blob, in 16-class blocks.
 // Thread 0 refills the stage of model h - 1 with model h - 1 + S once both warpgroups have released it.
 // Every wait is bounded: a pipeline that stops sets CODA_B200_FLAG_PIPELINE_TIMEOUT and the kernel drains out.
+//
+// A 16-bit slab (fp16 / bf16) is widened to fp32 as the A fragment is loaded, then split into the same two limbs, so it
+// gives the bits of its fp32 widening.  Its tile of 128 items is 25 600 bytes at C = 100, but a tile (or a model) need not
+// start on a 16-byte boundary: the bulk copy takes the tile's 16-byte aligned interior and thread 0 copies the few
+// elements before and after it, so every shape the fp32 slab takes here is taken by the 16-bit slab too.
 #include "common.cuh"
 
-#include <cuda_fp16.h>
 #include <stdlib.h>
+#include <type_traits>
 
 namespace {
 
@@ -38,8 +43,8 @@ constexpr size_t PT_SMEM_BUDGET = 227 * 1024;
 constexpr size_t PT_TAIL = 256;           // barriers + abort flag
 
 struct PiTcArgs {
-  const float* preds;
-  long long ldh;              // floats between models
+  const void* preds;          // float, __half or __nv_bfloat16 (the kernel's T)
+  long long ldh;              // elements between models
   const unsigned char* wb;    // [H][KC][2 k_cores][2 Np/8 (hi | lo)][8][8] fp16, then the 16-byte header (max |D| bits)
   const uint32_t* dmax;       // header: bits of max |D|
   float* U;
@@ -48,7 +53,8 @@ struct PiTcArgs {
   int H, C, Np, KC;
   int rows;                   // items per CTA: 64 x warpgroups
   int S;                      // stages (one model each)
-  uint32_t xbytes;            // stage offset of the D limbs (the items block rounded up to 128 bytes)
+  uint32_t xbytes;            // stage offset of the D limbs (the items block, + 16 bytes of alignment slack for 16-bit
+                              // slabs, rounded up to 128 bytes)
   uint32_t sbytes;            // bytes per stage
   int G;                      // models per accumulator fold
 };
@@ -164,7 +170,15 @@ __global__ void __launch_bounds__(256) k_pi_w_limbs(const float* __restrict__ D,
   }
 }
 
+// two consecutive classes of one item -> fp32 (the fp32 slab keeps its 8-byte load)
+__device__ __forceinline__ float2 pt_ld2(const float* p) { return *reinterpret_cast<const float2*>(p); }
+template <typename T>
+__device__ __forceinline__ float2 pt_ld2(const T* p) { return make_float2(slab_f(p[0]), slab_f(p[1])); }
+
+template <typename T>
 __global__ void __launch_bounds__(2 * 128, 1) k_pi_full_tc(PiTcArgs a) {
+  constexpr bool WIDE = std::is_same<T, float>::value;
+  const T* preds = static_cast<const T*>(a.preds);
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int H = a.H, C = a.C, Np = a.Np, KC = a.KC, S = a.S, G = a.G;
@@ -186,12 +200,31 @@ __global__ void __launch_bounds__(2 * 128, 1) k_pi_full_tc(PiTcArgs a) {
     mbar_fence_init();
   }
   __syncthreads();
-  const uint32_t xbytes = (uint32_t)cnt * C * 4u, dbytes = (uint32_t)KC * Np * 64u;
+  const uint32_t xbytes = (uint32_t)cnt * C * (uint32_t)sizeof(T), dbytes = (uint32_t)KC * Np * 64u;
+  // byte offset of this CTA's tile of model h inside its stage: 0 for fp32; for a 16-bit slab the stage holds the
+  // tile's bytes from the 16-byte boundary at or below its first element
+  auto tile_pad = [&](int h) -> uint32_t {
+    return WIDE ? 0u : (uint32_t)(reinterpret_cast<uintptr_t>(preds + (size_t)h * a.ldh + (size_t)n0 * C) & 15);
+  };
   auto load = [&](int h) {
     unsigned char* st = smem + (size_t)(h % S) * a.sbytes;
     uint64_t* bar = &full[h % S];
-    mbar_expect_tx(bar, xbytes + dbytes);
-    tma_load_1d(st, a.preds + (size_t)h * a.ldh + (size_t)n0 * C, xbytes, bar);
+    const T* src = preds + (size_t)h * a.ldh + (size_t)n0 * C;
+    if (WIDE) {
+      mbar_expect_tx(bar, xbytes + dbytes);
+      tma_load_1d(st, src, xbytes, bar);
+    } else {
+      // [lo, hi): whole 16-byte units of the tile by bulk copy; the elements before lo and from hi on by this thread
+      const uintptr_t b = reinterpret_cast<uintptr_t>(src), e = b + xbytes, b0 = b & ~(uintptr_t)15;
+      uintptr_t lo = (b + 15) & ~(uintptr_t)15, hi = e & ~(uintptr_t)15;
+      if (hi <= lo) lo = hi = e;
+      for (uintptr_t x = b; x < lo; x += sizeof(T))
+        *reinterpret_cast<T*>(st + (x - b0)) = __ldg(reinterpret_cast<const T*>(x));
+      for (uintptr_t x = hi; x < e; x += sizeof(T))
+        *reinterpret_cast<T*>(st + (x - b0)) = __ldg(reinterpret_cast<const T*>(x));
+      mbar_expect_tx(bar, (uint32_t)(hi - lo) + dbytes);        // arrive (release): the stores above are visible
+      if (hi > lo) tma_load_1d(st + (lo - b0), reinterpret_cast<const void*>(lo), (uint32_t)(hi - lo), bar);
+    }
     tma_load_1d(st + a.xbytes, a.wb + (size_t)h * dbytes, dbytes, bar);
   };
   if (tid == 0)
@@ -214,18 +247,18 @@ __global__ void __launch_bounds__(2 * 128, 1) k_pi_full_tc(PiTcArgs a) {
     ok = wg_all(pt_wait(&full[s], (h / S) & 1, abort_s), warp >> 2);
     if (!ok) break;
     const unsigned char* st = smem + (size_t)s * a.sbytes;
-    const float* x0 = reinterpret_cast<const float*>(st) + (size_t)r0 * C;
-    const float* x1 = x0 + (size_t)8 * C;
+    const T* x0 = reinterpret_cast<const T*>(st + tile_pad(h)) + (size_t)r0 * C;
+    const T* x1 = x0 + (size_t)8 * C;
     const uint32_t dst = smem_u32(st + a.xbytes);
     const bool restart = h % G == 0;
     for (int kc = 0; kc < KC; ++kc) {
       // this thread's A fragment: items r0, r0 + 8 x classes c0, c0 + 1, c0 + 8, c0 + 9 of the chunk (C % 4 == 0)
       const int c0 = kc * 16 + 2 * (lane & 3);
       const float2 z = make_float2(0.f, 0.f);
-      const float2 v00 = (in0 && c0 < C) ? *reinterpret_cast<const float2*>(x0 + c0) : z;
-      const float2 v10 = (in1 && c0 < C) ? *reinterpret_cast<const float2*>(x1 + c0) : z;
-      const float2 v01 = (in0 && c0 + 8 < C) ? *reinterpret_cast<const float2*>(x0 + c0 + 8) : z;
-      const float2 v11 = (in1 && c0 + 8 < C) ? *reinterpret_cast<const float2*>(x1 + c0 + 8) : z;
+      const float2 v00 = (in0 && c0 < C) ? pt_ld2(x0 + c0) : z;
+      const float2 v10 = (in1 && c0 < C) ? pt_ld2(x1 + c0) : z;
+      const float2 v01 = (in0 && c0 + 8 < C) ? pt_ld2(x0 + c0 + 8) : z;
+      const float2 v11 = (in1 && c0 + 8 < C) ? pt_ld2(x1 + c0 + 8) : z;
       uint32_t ahi[4], alo[4];
       pt_split2(v00.x, v00.y, ahi[0], alo[0]);
       pt_split2(v10.x, v10.y, ahi[1], alo[1]);
@@ -284,11 +317,12 @@ struct PiTcPlan {
 };
 
 // two warpgroups (128 items per CTA) when two stages fit shared memory, else one; then as many stages as fit
-PiTcPlan pi_tc_plan(int C, int Np, int KC) {
+PiTcPlan pi_tc_plan(int C, int Np, int KC, size_t esz) {
   PiTcPlan p;
   const size_t dbytes = (size_t)KC * Np * 64;
+  const size_t slack = esz == 4 ? 0 : 16;                       // 16-bit tiles may start mid 16-byte unit
   for (p.rows = 2 * PT_WG; ; p.rows -= PT_WG) {
-    p.xbytes = (uint32_t)(((size_t)p.rows * C * 4 + 127) & ~(size_t)127);
+    p.xbytes = (uint32_t)(((size_t)p.rows * C * esz + slack + 127) & ~(size_t)127);
     p.sbytes = (uint32_t)(p.xbytes + dbytes);
     if (2 * (size_t)p.sbytes + PT_TAIL <= PT_SMEM_BUDGET || p.rows == PT_WG) break;
   }
@@ -303,18 +337,27 @@ extern "C" int coda_b200_pi_full_tc_ok(int H, int64_t N, int C, int64_t model_st
   return H >= 1 && N >= 1 && C >= 16 && C <= 128 && C % 4 == 0 && model_stride % 4 == 0;
 }
 
+// a 16-bit slab is staged at any element alignment (see the file comment): the model stride does not matter
+extern "C" int coda_b200_pi_full_tc_ok_x(int fmt, int H, int64_t N, int C, int64_t model_stride) {
+  if (fmt == CODA_B200_SLAB_F32) return coda_b200_pi_full_tc_ok(H, N, C, model_stride);
+  return (fmt == CODA_B200_SLAB_F16 || fmt == CODA_B200_SLAB_BF16) && H >= 1 && N >= 1 && C >= 16 && C <= 128 &&
+         C % 4 == 0;
+}
+
 extern "C" size_t coda_b200_pi_full_tc_scratch_bytes(int H, int C) {
   const int Np = (C + 15) / 16 * 16, KC = (C + 15) / 16;
   return (size_t)H * KC * 2 * Np * 16 * 2 + 16;
 }
 
-extern "C" int coda_b200_pi_full_tc(const float* preds, int64_t model_stride, const float* D, int H, int64_t N, int C,
-                                    float* U, void* scratch, uint32_t* flags, coda_stream_t stream) {
+template <typename T>
+static int pi_full_tc(const T* preds, int fmt, int64_t model_stride, const float* D, int H, int64_t N, int C, float* U,
+                      void* scratch, uint32_t* flags, coda_stream_t stream) {
   CODA_CHECK_ARG(preds && D && U && scratch && flags, "pi_full_tc: null pointer");
-  CODA_CHECK_ARG(coda_b200_pi_full_tc_ok(H, N, C, model_stride),
-                 "pi_full_tc: needs 16 <= C <= 128, C %% 4 == 0 and a 16-byte aligned model stride (C=%d)", C);
-  CODA_CHECK_ARG(((uintptr_t)preds & 15) == 0 && ((uintptr_t)U & 15) == 0 && ((uintptr_t)scratch & 15) == 0,
-                 "pi_full_tc: preds, U and scratch must be 16-byte aligned");
+  CODA_CHECK_ARG(coda_b200_pi_full_tc_ok_x(fmt, H, N, C, model_stride),
+                 "pi_full_tc: needs 16 <= C <= 128, C %% 4 == 0 and (fp32) a 16-byte aligned model stride (C=%d)", C);
+  CODA_CHECK_ARG((sizeof(T) != 4 || ((uintptr_t)preds & 15) == 0) && ((uintptr_t)U & 15) == 0 &&
+                     ((uintptr_t)scratch & 15) == 0,
+                 "pi_full_tc: preds (fp32), U and scratch must be 16-byte aligned");
   const int Np = (C + 15) / 16 * 16, KC = (C + 15) / 16;
   unsigned char* wb = reinterpret_cast<unsigned char*>(scratch);
   uint32_t* dmax = reinterpret_cast<uint32_t*>(wb + coda_b200_pi_full_tc_scratch_bytes(H, C) - 16);
@@ -323,7 +366,7 @@ extern "C" int coda_b200_pi_full_tc(const float* preds, int64_t model_stride, co
   CODA_LAUNCH_OK("k_pi_w_max");
   k_pi_w_limbs<<<coda_sm_count() * 4, 256, 0, as_stream(stream)>>>(D, H, C, Np, KC, dmax, reinterpret_cast<__half*>(wb));
   CODA_LAUNCH_OK("k_pi_w_limbs");
-  const PiTcPlan plan = pi_tc_plan(C, Np, KC);
+  const PiTcPlan plan = pi_tc_plan(C, Np, KC, sizeof(T));
   CODA_CHECK_ARG(plan.stages >= 2, "pi_full_tc: C=%d does not fit shared memory", C);
   PiTcArgs a;
   a.preds = preds; a.ldh = model_stride; a.wb = wb; a.dmax = dmax; a.U = U; a.flags = flags;
@@ -332,9 +375,21 @@ extern "C" int coda_b200_pi_full_tc(const float* preds, int64_t model_stride, co
   // models per fold: the truncating fp32 accumulate of the tensor core loses up to 2^-24 per K = 8 sub-step of the chain
   const char* genv = getenv("CODA_B200_PI_DRAIN");
   a.G = genv ? max(1, min(16, atoi(genv))) : 4;
-  CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_full_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
+  CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_full_tc<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
   const long long grid = (N + plan.rows - 1) / plan.rows;
-  k_pi_full_tc<<<(unsigned)grid, 2 * plan.rows, plan.smem, as_stream(stream)>>>(a);
+  k_pi_full_tc<T><<<(unsigned)grid, 2 * plan.rows, plan.smem, as_stream(stream)>>>(a);
   CODA_LAUNCH_OK("k_pi_full_tc");
   return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_pi_full_tc(const float* preds, int64_t model_stride, const float* D, int H, int64_t N, int C,
+                                    float* U, void* scratch, uint32_t* flags, coda_stream_t stream) {
+  return pi_full_tc(preds, CODA_B200_SLAB_F32, model_stride, D, H, N, C, U, scratch, flags, stream);
+}
+
+extern "C" int coda_b200_pi_full_tc_x(const void* preds, int fmt, int64_t model_stride, const float* D, int H, int64_t N,
+                                      int C, float* U, void* scratch, uint32_t* flags, coda_stream_t stream) {
+  return slab_dispatch(fmt, preds, [&](auto* p) {
+    return pi_full_tc(p, fmt, model_stride, D, H, N, C, U, scratch, flags, stream);
+  });
 }

@@ -8,13 +8,23 @@ import torch
 from .synth import shard_range, synth, synth_compact
 
 
+_KEPT_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def _slab_dtype(t: torch.Tensor, keep_dtype: bool) -> torch.dtype:
+    """fp32 (coda/datasets.py:14 widens on load), or with ``keep_dtype`` the stored width of an fp16 / bf16 / fp32 slab:
+    the kernels widen 16-bit values exactly, so the results are those of the fp32 slab at half the memory."""
+    return t.dtype if keep_dtype and t.dtype in _KEPT_DTYPES else torch.float32
+
+
 class Dataset:
     """(H, N, C) post-softmax scores from ``filepath`` (+ optional ``*_labels.pt``), forced to fp32
-    (coda/datasets.py:12-23)."""
+    (coda/datasets.py:12-23).  ``keep_dtype=True`` keeps a stored fp16 or bf16 slab at its width."""
 
-    def __init__(self, filepath, device):
+    def __init__(self, filepath, device, keep_dtype=False):
         self.device = device
-        self.preds = torch.load(filepath, map_location=device).float().contiguous()
+        preds = torch.load(filepath, map_location=device)
+        self.preds = preds.to(_slab_dtype(preds, keep_dtype)).contiguous()
         print("Loaded preds of shape", self.preds.shape)
         self.labels = None
         label_p = filepath.replace(".pt", "_labels.pt")
@@ -37,15 +47,18 @@ class TensorDataset:
 class ShardedFileDataset(TensorDataset):
     """This rank's contiguous N-range of an (H, N, C) ``.pt`` slab, read through ``torch.load(mmap=True)`` so that
     no rank ever materialises the whole tensor (the reference loader, coda/datasets.py:14, loads all of it onto
-    one device).  Labels (``*_labels.pt``, N int64) are small and replicated."""
+    one device).  Labels (``*_labels.pt``, N int64) are small and replicated.  ``keep_dtype``: see ``Dataset``."""
 
-    def __init__(self, filepath, device, rank=0, world=1):
+    def __init__(self, filepath, device, rank=0, world=1, keep_dtype=False):
         full = torch.load(filepath, map_location="cpu", mmap=True, weights_only=True)
         if full.dim() != 3:
             raise ValueError(f"{filepath}: expected an (H, N, C) tensor, got shape {tuple(full.shape)}")
         n = int(full.shape[1])
         lo, hi = shard_range(n, rank, world)
-        preds = full[:, lo:hi].float().contiguous().to(device)     # avoid fp16 precision errors (coda/datasets.py:14)
+        if keep_dtype:
+            preds = full[:, lo:hi].to(_slab_dtype(full, True)).contiguous().to(device)
+        else:
+            preds = full[:, lo:hi].float().contiguous().to(device)     # avoid fp16 precision errors (coda/datasets.py:14)
         labels = None
         label_p = filepath.replace(".pt", "_labels.pt")
         if os.path.exists(label_p):
@@ -57,10 +70,11 @@ class ShardedFileDataset(TensorDataset):
 class SyntheticDataset(TensorDataset):
     """This rank's shard of the synthetic task (SURVEY.md 8d); labels are replicated (N int64)."""
 
-    def __init__(self, H, N, C, seed=0, device="cuda", dense=False, rank=0, world=1, generator_device=None):
+    def __init__(self, H, N, C, seed=0, device="cuda", dense=False, rank=0, world=1, generator_device=None,
+                 dtype=torch.float32):
         lo, hi = shard_range(N, rank, world)
         gdev = generator_device or device
-        preds, _ = synth(H, N, C, seed, device=gdev, dense=dense, n_lo=lo, n_hi=hi)
+        preds, _ = synth(H, N, C, seed, device=gdev, dense=dense, n_lo=lo, n_hi=hi, dtype=dtype)
         _, labels = synth(H, N, C, seed, device=gdev, dense=dense, want_preds=False)
         super().__init__(preds.to(device), labels, n_offset=lo, n_global=N)
         self.labels_host = labels.cpu()

@@ -60,14 +60,17 @@ def _ptr(t):
     return t.data_ptr() if t is not None else None
 
 
-def shadow_slots(free: int, reserve: int, slot_bytes: int, want: int, ens: bool, left: int = 1, total: int = 1):
+def shadow_slots(free: int, reserve: int, slot_bytes: int, want: int, ens: bool, left: int = 1, total: int = 1,
+                 ens_slot_bytes: int | None = None):
     """-> (model slots, ensemble slots) of one shard's shadow.  ``free``: device bytes free now; ``total`` shards on
     the device keep ``reserve`` bytes each, and the ``left`` shards still to be sized (this one included) split the rest
     equally.  The ensemble slot (one per step, in every list with the majority shortcut) comes first, then up to
-    ``want`` models."""
-    n = max(0, (free - total * reserve) // max(1, left) // slot_bytes)
-    ne = 1 if ens and n >= 1 else 0
-    return int(max(0, min(want, n - ne))), ne
+    ``want`` models.  ``slot_bytes``: one model slot (the slab's element size); ``ens_slot_bytes``: the ensemble slot,
+    which is fp32 (default: ``slot_bytes``)."""
+    share = max(0, (free - total * reserve) // max(1, left))
+    eb = slot_bytes if ens_slot_bytes is None else ens_slot_bytes
+    ne = 1 if ens and share >= eb else 0
+    return int(max(0, min(want, (share - ne * eb) // slot_bytes))), ne
 
 
 class Engine:
@@ -91,13 +94,17 @@ class Engine:
                 raise NotImplementedError("coda_b200: mode='recompute_all' is not offered for a compact slab")
             self.K = self.compact.K
         else:
-            if preds.dtype != torch.float32 or preds.dim() != 3:
-                raise TypeError("coda_b200: preds must be a float32 (H, N, C) tensor (coda/datasets.py:14)")
+            nat.slab_format(preds.dtype)          # float32, float16 or bfloat16, else TypeError
+            if preds.dim() != 3:
+                raise TypeError("coda_b200: preds must be an (H, N, C) tensor (coda/datasets.py:14)")
             if not (preds.stride(2) == 1 and preds.stride(1) == Cc and (H == 1 or preds.stride(0) >= N * Cc)):
                 raise ValueError("coda_b200: preds must be (H, N, C) with contiguous items (an N-range view of a "
                                  "contiguous slab is fine)")
         self.lib = nat.load()
         self.preds = preds
+        # slab element type: a 16-bit slab is read at its stored width and widened to fp32 in every kernel
+        self.fmt = nat.slab_format(preds.dtype) if self.compact is None else nat.SLAB_F32
+        self.esz = int(preds.element_size()) if self.compact is None else 4
         self.dev = preds.device
         with torch.cuda.device(self.dev):
             nat.require_device()
@@ -168,13 +175,14 @@ class Engine:
 
     def _call(self, name, *args, n=1):
         prof = self.profile
-        if prof is not None and (self.profile_only is None or name in self.profile_only):
+        key = name[:-2] if name.endswith("_x") else name         # a slab entry point's 16-bit twin times under its name
+        if prof is not None and (self.profile_only is None or key in self.profile_only):
             st = self._cur()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(st)
             rc = getattr(self.lib, name)(*args)
             e1.record(st)
-            prof.setdefault(name, []).append((e0, e1))
+            prof.setdefault(key, []).append((e0, e1))
         else:
             rc = getattr(self.lib, name)(*args)
         nat.check(rc, name)
@@ -193,6 +201,13 @@ class Engine:
             out[k] = (len(ts), float(sum(ts)), float(max(ts)))
         self.profile = None
         return out
+
+    def _slab_call(self, name, *args, n=1):
+        """An entry point that reads the slab: the fp32 one, or its ``_x`` twin with the slab's element type."""
+        if self.fmt == nat.SLAB_F32:
+            self._call(name, _ptr(self.preds), *args, n=n)
+        else:
+            self._call(name + "_x", _ptr(self.preds), self.fmt, *args, n=n)
 
     def _z(self, shape, dtype):
         return torch.zeros(shape, dtype=dtype, device=self.dev)
@@ -263,14 +278,17 @@ class Engine:
         st.hard, st.labeled, st.D, st.jvec, st.sel = _ptr(self.hard), _ptr(self.labeled), _ptr(self.D), _ptr(self.jvec), _ptr(self.sel)
         st.terms = _ptr(self.terms)
         st.slot_of_model = _ptr(self.slot_of_model)
-        st.shadow_off = ((self.shadow.data_ptr() - self._slab_ptr()) // 4) if self.shadow is not None else 0
+        # gather-list offsets count slab elements from the slab; the ensemble term counts fp32 elements from the
+        # ensemble base (the slab itself for fp32, see ``_ens_base``)
+        st.shadow_off = ((self.shadow.data_ptr() - self._slab_ptr()) // self.esz) if self.shadow is not None else 0
         st.shadow_col_stride = self.shadow_cs
         st.model_stride = self.model_stride
-        if self.shadow is not None and self.shadow.shape[0] > self.n_shadow:     # class-major ensemble slot
-            st.ens_off = (self.shadow[self.n_shadow].data_ptr() - self._slab_ptr()) // 4
+        ens_base = self._ens_base()
+        if self.ens_shadow is not None:                                          # class-major ensemble slot
+            st.ens_off = (self.ens_shadow.data_ptr() - ens_base) // 4
             st.ens_col_stride = self.shadow_cs
         else:
-            st.ens_off = ((self.ens.data_ptr() - self._slab_ptr()) // 4) if self.ens is not None else 0
+            st.ens_off = ((self.ens.data_ptr() - ens_base) // 4) if self.ens is not None else 0
             st.ens_col_stride = 0
         st.have_ens = 1 if self.ens is not None else 0
         st.compact_k = self.K if self.compact is not None else 0
@@ -285,6 +303,13 @@ class Engine:
 
     def _slab_ptr(self):
         return self.preds.data_ptr() if self.compact is None else 0
+
+    def _ens_base(self):
+        """fp32 base address of the ensemble term of the gather list: the slab for an fp32 slab (one base for every
+        term, as the fp32 entry point reads it), the ensemble sums themselves for a 16-bit slab."""
+        if self.fmt == nat.SLAB_F32 or self.ens is None:
+            return self._slab_ptr()
+        return self.ens_shadow.data_ptr() if self.ens_shadow is not None else self.ens.data_ptr()
 
     def _x(self):
         return self.xchg if (self.xchg is not None and self.world > 1) else None
@@ -302,16 +327,16 @@ class Engine:
                            _ptr(self.pseudo), H, N, C, self.K, self.fx_shift, _ptr(self.conf_fx), _ptr(self.conf_rest), s)
                 self._build_compact_index()
                 return
-            self._call("coda_b200_scan_slab", _ptr(self.preds), self.model_stride, H, N, C, _ptr(self.hard),
-                       _ptr(self.pseudo), _ptr(self.disagree), _ptr(self.ens), _ptr(self.flags), s)
+            self._slab_call("coda_b200_scan_slab", self.model_stride, H, N, C, _ptr(self.hard),
+                            _ptr(self.pseudo), _ptr(self.disagree), _ptr(self.ens), _ptr(self.flags), s)
             if C <= 128:
                 order = torch.argsort(self.pseudo).to(torch.int32)      # init-time plumbing: any grouping by label will do
-                self._call("coda_b200_confusion_sorted", _ptr(self.preds), self.model_stride, _ptr(self.pseudo),
-                           _ptr(order), H, N, C, self.fx_shift, _ptr(self.conf_fx), s)
+                self._slab_call("coda_b200_confusion_sorted", self.model_stride, _ptr(self.pseudo),
+                                _ptr(order), H, N, C, self.fx_shift, _ptr(self.conf_fx), s)
                 del order
             else:
-                self._call("coda_b200_confusion_accum", _ptr(self.preds), self.model_stride, _ptr(self.pseudo), H, N, C,
-                           self.fx_shift, _ptr(self.conf_fx), s)
+                self._slab_call("coda_b200_confusion_accum", self.model_stride, _ptr(self.pseudo), H, N, C,
+                                self.fx_shift, _ptr(self.conf_fx), s)
 
     def construct_posterior(self):
         with self._on():
@@ -391,15 +416,25 @@ class Engine:
         H, N, C, s = self.H, self.N, self.C, self._s()
         if self._pi_tc is None:
             want = os.environ.get("CODA_B200_PI_FULL", "tc") != "simt"
-            self._pi_tc = bool(want and self.lib.coda_b200_pi_full_tc_ok(H, N, C, self.model_stride)
-                               and self.preds.data_ptr() % 16 == 0)
+            if self.fmt == nat.SLAB_F32:
+                self._pi_tc = bool(want and self.lib.coda_b200_pi_full_tc_ok(H, N, C, self.model_stride)
+                                   and self.preds.data_ptr() % 16 == 0)
+            else:
+                # the tensor-core and SIMT passes differ in the last bits: a 16-bit slab takes the pass its fp32
+                # widening (contiguous, aligned) would take, or stops
+                tc32 = bool(self.lib.coda_b200_pi_full_tc_ok(H, N, C, N * C))
+                ok = bool(self.lib.coda_b200_pi_full_tc_ok_x(self.fmt, H, N, C, self.model_stride))
+                if want and tc32 and not ok:
+                    raise NotImplementedError(f"coda_b200: the tensor-core marginal pass cannot read this "
+                                              f"{self.preds.dtype} slab (C={C}); its fp32 widening would take it")
+                self._pi_tc = bool(want and tc32)
             if self._pi_tc:
                 self._pi_scratch = self._e((int(self.lib.coda_b200_pi_full_tc_scratch_bytes(H, C)),), torch.uint8)
         if self._pi_tc:
-            self._call("coda_b200_pi_full_tc", _ptr(self.preds), self.model_stride, _ptr(self.D), H, N, C, _ptr(self.U),
-                       _ptr(self._pi_scratch), _ptr(self.flags), s, n=2)
+            self._slab_call("coda_b200_pi_full_tc", self.model_stride, _ptr(self.D), H, N, C, _ptr(self.U),
+                            _ptr(self._pi_scratch), _ptr(self.flags), s, n=2)
         else:
-            self._call("coda_b200_pi_full", _ptr(self.preds), self.model_stride, _ptr(self.D), H, N, C, _ptr(self.U), s)
+            self._slab_call("coda_b200_pi_full", self.model_stride, _ptr(self.D), H, N, C, _ptr(self.U), s)
 
     def _build_rows(self):
         H, N, C, W, T, s = self.H, self.N, self.C, self.W, self.T, self._s()
@@ -490,10 +525,11 @@ class Engine:
         this device that have still to build a shadow (this one included) / in all -- each takes an equal share of
         what is free once every shard's reserve is set aside."""
         self.shadow, self.slot_of_model, self.n_shadow, self.shadow_cs = None, None, 0, 0
+        self.ens_shadow = None
         if self.mode == "recompute_all" or os.environ.get("CODA_B200_SHADOW", "1") == "0" or self.compact is not None:
             return
         H, N, C = self.H, self.N, self.C
-        cs = (N + 3) // 4 * 4                                   # every (slot, class) column starts 16-byte aligned
+        cs = (N + 7) // 8 * 8 if self.esz == 2 else (N + 3) // 4 * 4    # every (slot, class) column starts 16-byte aligned
         cap = os.environ.get("CODA_B200_SHADOW_MODELS")
         want = H if cap is None else max(0, min(H, int(cap)))
         order = None
@@ -509,20 +545,27 @@ class Engine:
         torch.cuda.synchronize(self.dev)
         torch.cuda.empty_cache()                                # the temporaries above are not spare memory
         free, _total = torch.cuda.mem_get_info(self.dev)
-        S, ne = shadow_slots(free, self.shadow_reserve(), cs * C * 4, want, self.ens is not None, left, total)
+        # model slots hold the slab's own element type (exact); the ensemble slot is fp32
+        S, ne = shadow_slots(free, self.shadow_reserve(), cs * C * self.esz, want, self.ens is not None, left, total,
+                             ens_slot_bytes=cs * C * 4)
         if S + ne == 0:
             return
         slot = torch.full((H,), -1, dtype=torch.int32, device=self.dev)
-        self.shadow = self._e((S + ne, C, cs), torch.float32)
+        if self.esz == 4:
+            self.shadow = self._e((S + ne, C, cs), torch.float32)
+            self.ens_shadow = self.shadow[S] if ne else None
+        else:                                                   # a 16-bit slab: E in a buffer of its own
+            self.shadow = self._e((S, C, cs), self.preds.dtype) if S > 0 else None
+            self.ens_shadow = self._e((C, cs), torch.float32) if ne else None
         if S > 0:
             order = order[:S].contiguous()
             slot[order.long()] = torch.arange(S, dtype=torch.int32, device=self.dev)
-            self._call("coda_b200_shadow_build", _ptr(self.preds), self.model_stride, H, N, C, _ptr(order), S, cs,
-                       _ptr(self.shadow), self._s())
+            self._slab_call("coda_b200_shadow_build", self.model_stride, H, N, C, _ptr(order), S, cs,
+                            _ptr(self.shadow), self._s())
         if ne:                                                  # E [N][C] is a one-model slab
             first = torch.zeros(1, dtype=torch.int32, device=self.dev)
             self._call("coda_b200_shadow_build", _ptr(self.ens), N * C, 1, N, C, _ptr(first), 1, cs,
-                       _ptr(self.shadow[S]), self._s())
+                       _ptr(self.ens_shadow), self._s())
         self.slot_of_model, self.n_shadow, self.shadow_cs = slot, S, cs
 
     # ------------------------------------------------------------------------ step pieces (enqueue only)
@@ -624,9 +667,10 @@ class Engine:
                        C, self.K, _ptr(self.sel), self.lr, self.fx_shift, _ptr(self.terms), _ptr(self.U),
                        _ptr(self.pisum), _ptr(self.flags), s)
         else:
-            self._call("coda_b200_pi_rank1", _ptr(self.preds), _ptr(self.ens), H, N, C, _ptr(self.sel), self.lr,
-                       self.fx_shift, _ptr(self.terms), _ptr(self.U), _ptr(self.pisum), _ptr(self.flags),
-                       4 if fork else 8, self.const_slot, s)
+            ens = _ptr(self.ens) if self.fmt == nat.SLAB_F32 else self._ens_base()
+            self._slab_call("coda_b200_pi_rank1", ens, H, N, C, _ptr(self.sel), self.lr,
+                            self.fx_shift, _ptr(self.terms), _ptr(self.U), _ptr(self.pisum), _ptr(self.flags),
+                            4 if fork else 8, self.const_slot, s)
         if fork:
             main.wait_event(self.ev_tables)     # the mixture needs PB[t]; the rows are awaited by the scoring pass
             self.pending = True

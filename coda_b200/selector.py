@@ -60,7 +60,8 @@ def _auto_gpus(preds) -> int:
     env = os.environ.get("CODA_B200_GPUS")
     if env:
         return max(1, int(env))
-    if preds.numel() * 4 < (4 << 30):
+    nbytes = preds.numel() * (preds.element_size() if isinstance(preds, torch.Tensor) else 4)
+    if nbytes < (4 << 30):
         return 1
     return max(1, torch.cuda.device_count())
 

@@ -80,14 +80,15 @@ def _block(H, C, seed, block, device, dense, acc, out_preds, out_labels, lo, hi,
 
 
 def synth(H: int, N: int, C: int, seed: int = 0, device="cpu", dense: bool = False,
-          n_lo: int = 0, n_hi: int | None = None, want_preds: bool = True):
+          n_lo: int = 0, n_hi: int | None = None, want_preds: bool = True, dtype=torch.float32):
     """Return (preds[H, n_hi-n_lo, C] fp32, labels[n_hi-n_lo] int64) for the global
-    point range [n_lo, n_hi) of the synthetic task (H, N, C, seed)."""
+    point range [n_lo, n_hi) of the synthetic task (H, N, C, seed).  ``dtype`` (fp16 / bf16): the same bytes as
+    ``synth(...)[0].to(dtype)``, rounded model row by model row, so the fp32 slab never exists."""
     n_hi = N if n_hi is None else n_hi
     assert 0 <= n_lo <= n_hi <= N
     dev = torch.device(device)
     n = n_hi - n_lo
-    preds = torch.empty((H, n, C), dtype=torch.float32, device=dev) if want_preds else None
+    preds = torch.empty((H, n, C), dtype=dtype, device=dev) if want_preds else None
     labels = torch.empty((n,), dtype=torch.int64, device=dev)
     acc = model_accuracies(H, seed)
     b_lo, b_hi = n_lo // BLOCK, math.ceil(n_hi / BLOCK) if n_hi > 0 else 0

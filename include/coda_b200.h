@@ -154,6 +154,42 @@ int coda_b200_pi_rank1(const float* preds, const float* ens, int H, int64_t N, i
                        int fx_shift, const int32_t* terms, float* U, int64_t* pisum_fx, uint32_t* flags,
                        int ctas_per_sm, int const_slot, coda_stream_t stream);
 
+/* ---- 16-bit prediction slabs (the reference stores its task tensors in half precision and widens them on load,
+ *      coda/datasets.py:14) -----------------------------------------------------------------------------------------
+ * The _x entry points take `preds` as an untyped pointer plus its element type.  Every kernel widens the value to
+ * fp32 at the load and keeps the fp32 arithmetic in the same order, so a 16-bit slab gives exactly the bits of the
+ * fp32 entry points run on its fp32 widening; CODA_B200_SLAB_F32 runs the fp32 entry points' code.  Strides, offsets
+ * and the shadow column stride count slab ELEMENTS. */
+#define CODA_B200_SLAB_F32 0
+#define CODA_B200_SLAB_F16 1
+#define CODA_B200_SLAB_BF16 2
+/* coda.py:193-194, 215-219, 263, 316 (see coda_b200_scan_slab) */
+int coda_b200_scan_slab_x(const void* preds, int fmt, int64_t model_stride, int H, int64_t N, int C, uint16_t* hard,
+                          int32_t* pseudo, uint8_t* disagree, float* ens_out, uint32_t* flags, coda_stream_t stream);
+/* coda.py:42 (see coda_b200_confusion_accum / coda_b200_confusion_sorted) */
+int coda_b200_confusion_accum_x(const void* preds, int fmt, int64_t model_stride, const int32_t* pseudo, int H,
+                                int64_t N, int C, int fx_shift, int64_t* conf_fx, coda_stream_t stream);
+int coda_b200_confusion_sorted_x(const void* preds, int fmt, int64_t model_stride, const int32_t* pseudo,
+                                 const int32_t* order, int H, int64_t N, int C, int fx_shift, int64_t* conf_fx,
+                                 coda_stream_t stream);
+/* coda.py:227-229 (see coda_b200_pi_full / coda_b200_pi_full_tc).  For a 16-bit slab the tensor-core pass takes any
+ * model stride and any 2-byte aligned view (pi_full_tc_ok_x), so it serves every shape whose fp32 widening it serves. */
+int coda_b200_pi_full_x(const void* preds, int fmt, int64_t model_stride, const float* D, int H, int64_t N, int C,
+                        float* U, coda_stream_t stream);
+int coda_b200_pi_full_tc_ok_x(int fmt, int H, int64_t N, int C, int64_t model_stride);
+int coda_b200_pi_full_tc_x(const void* preds, int fmt, int64_t model_stride, const float* D, int H, int64_t N, int C,
+                           float* U, void* scratch, uint32_t* flags, coda_stream_t stream);
+/* Shadow copy in the slab's own element type (see coda_b200_shadow_build); col_stride a multiple of 8 elements. */
+int coda_b200_shadow_build_x(const void* preds, int fmt, int64_t model_stride, int H, int64_t N, int C,
+                             const int32_t* model_of_slot, int S, int64_t col_stride, void* T, coda_stream_t stream);
+/* coda.py:319 (see coda_b200_pi_rank1).  Model terms are slab elements relative to `preds`; the ensemble term (the
+ * first term of a list whose header names a majority class) is read as fp32 relative to `ens_base` instead, so the
+ * step struct's ens_off must be set relative to ens_base.  With CODA_B200_SLAB_F32 and ens_base == preds this is
+ * coda_b200_pi_rank1. */
+int coda_b200_pi_rank1_x(const void* preds, int fmt, const float* ens_base, int H, int64_t N, int C,
+                         const int64_t* sel, double lr, int fx_shift, const int32_t* terms, float* U,
+                         int64_t* pisum_fx, uint32_t* flags, int ctas_per_sm, int const_slot, coda_stream_t stream);
+
 /* ---- compact slab (BASELINE.json configs[4]: M=1024, N=4e6, C=1000 is 16.4 TB dense; no reference counterpart --
  *      the reference cannot run there, coda.py:227 materialises a second slab) ----------------------------------
  * For every (h, n) the K <= 8 highest-scoring classes: ids [H][N][K] u16 (descending score) and probs [H][N][K] f32;

@@ -135,6 +135,11 @@ SIGNATURES = {
     "coda_b200_weighted_draw": (i32, [p, p, i64, p, f64, p, p, p]),
     "coda_b200_select_extreme": (i32, [p, p, i64, i32, p, p, p]),
     "coda_b200_select_kth": (i32, [p, p, i64, p, p, i64, p, p]),
+    "coda_b200_select_extreme_xchg": (i32, [p, p, i64, i32, p, p, PX, p, p]),
+    "coda_b200_select_kth_xchg": (i32, [p, p, i64, p, p, i64, i64, p, PX, p, p]),
+    "coda_b200_weighted_total_xchg": (i32, [p, p, i64, p, p, PX, p, p]),
+    "coda_b200_weighted_draw_xchg": (i32, [p, p, i64, p, f64, i64, p, p, PX, p, p]),
+    "coda_b200_owner_share": (i32, [p, i32, i32, p, PX, p, p]),
 }
 
 

@@ -1,7 +1,8 @@
 // The competing selectors of the paper's comparison (reference coda/baselines/*.py): per-item scores and the
 // selection primitives they share.  Everything here reads the products of one slab scan (hard [N][H] u16,
-// disagree [N], ens [N][C]); nothing touches the slab itself.
-#include "common.cuh"
+// disagree [N], ens [N][C]); nothing touches the slab itself.  N-range shards exchange their selection records through
+// the mailboxes of xchg.cuh (record channel), so every shard ends a selection call with the same global answer.
+#include "xchg.cuh"
 
 #include <limits.h>
 
@@ -245,25 +246,22 @@ __global__ void k_wsum_final(const double* __restrict__ partials, int nblocks, d
   total[1] = c;
 }
 
-// One block: cum = running sum of the normalised weights in index order; the pick is the first unlabeled item with
-// cum > u * cum_total (bisect_right), the last one when rounding leaves none.  out = {position among the unlabeled
-// items, item, float bits of its normalised weight}.
-__global__ void __launch_bounds__(BL_THREADS) k_wdraw_pick(const float* __restrict__ w, const uint8_t* __restrict__ labeled,
-                                                          long long N, const double* __restrict__ total,
-                                                          const double* __restrict__ partials, int nblocks, double u,
-                                                          long long* __restrict__ out) {
+// Every thread of one block: cum = base0 + running sum of the normalised weights in index order over this vector's
+// chunks; the pick is the first unlabeled item with cum > target (bisect_right), the last one when rounding leaves
+// none.  base0, pos0 (the weight and the number of unlabeled items before this vector) and target are read from
+// thread 0.  res (thread 0) = {position among the unlabeled items, item, float bits of its normalised weight}, or
+// {-1, -1, 0} when no item is unlabeled.
+__device__ void wdraw_in_chunks(const float* __restrict__ w, const uint8_t* __restrict__ labeled, long long N, float tf,
+                                const double* __restrict__ partials, int nblocks, double base0, double pos0,
+                                double target, long long* res) {
   __shared__ double shs[BL_THREADS / 32];
   __shared__ int shc[BL_THREADS / 32];
   __shared__ double s_base, s_target;
   __shared__ long long s_pos0;
   __shared__ int s_blk;
   __shared__ unsigned long long s_first;
-  const float tf = (float)total[0];
   if (threadIdx.x == 0) {
-    double grand = 0.0;
-    for (int b = 0; b < nblocks; ++b) grand += partials[2 * b];
-    const double target = u * grand;
-    double base = 0.0, pos = 0.0;
+    double base = base0, pos = pos0;
     int blk = -1, last = -1;
     for (int b = 0; b < nblocks; ++b) {
       if (partials[2 * b + 1] == 0.0) continue;
@@ -286,7 +284,7 @@ __global__ void __launch_bounds__(BL_THREADS) k_wdraw_pick(const float* __restri
   __syncthreads();
   const int blk = s_blk;
   if (blk < 0) {
-    if (threadIdx.x == 0) { out[0] = -1; out[1] = -1; out[2] = 0; }
+    if (threadIdx.x == 0) { res[0] = -1; res[1] = -1; res[2] = 0; }
     return;
   }
   const long long lo = min(N, (long long)blk * BL_CHUNK + (long long)threadIdx.x * BL_IPT), hi = min(N, lo + BL_IPT);
@@ -320,10 +318,26 @@ __global__ void __launch_bounds__(BL_THREADS) k_wdraw_pick(const float* __restri
   __syncthreads();
   if (threadIdx.x == 0) {
     const long long i = (long long)blk * BL_CHUNK + (long long)(s_first & 0xffffull);
-    out[0] = (long long)(s_first >> 16);
-    out[1] = i;
-    out[2] = (long long)__float_as_uint(__fdiv_rn(w[i], tf));
+    res[0] = (long long)(s_first >> 16);
+    res[1] = i;
+    res[2] = (long long)__float_as_uint(__fdiv_rn(w[i], tf));
   }
+}
+
+// One block: the draw over the whole vector (target = u * the sum of the block partials in block order).
+__global__ void __launch_bounds__(BL_THREADS) k_wdraw_pick(const float* __restrict__ w, const uint8_t* __restrict__ labeled,
+                                                          long long N, const double* __restrict__ total,
+                                                          const double* __restrict__ partials, int nblocks, double u,
+                                                          long long* __restrict__ out) {
+  double target = 0.0;
+  if (threadIdx.x == 0) {
+    double grand = 0.0;
+    for (int b = 0; b < nblocks; ++b) grand += partials[2 * b];
+    target = u * grand;
+  }
+  long long res[3];
+  wdraw_in_chunks(w, labeled, N, (float)total[0], partials, nblocks, 0.0, 0.0, target, res);
+  if (threadIdx.x == 0) { out[0] = res[0]; out[1] = res[1]; out[2] = res[2]; }
 }
 
 extern "C" int coda_b200_select_blocks(int64_t N) { return (int)((N + BL_CHUNK - 1) / BL_CHUNK); }
@@ -398,15 +412,14 @@ __global__ void k_extreme_final(const long long* __restrict__ partials, int nblo
 
 // One block: the k-th (ascending index) unlabeled item whose value equals best[0].  Only blocks whose partial value is
 // the best hold such items, so the partials locate the chunk without another pass over the vector.
-__global__ void __launch_bounds__(BL_THREADS) k_select_kth(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
-                                                          long long N, const long long* __restrict__ partials, int nblocks,
-                                                          const long long* __restrict__ best, long long k,
-                                                          long long* __restrict__ out) {
+// Every thread of the block calls it; returns the item (to every thread), -1 if there is none.
+__device__ long long kth_in_chunks(const float* __restrict__ v, const uint8_t* __restrict__ labeled, long long N,
+                                   const long long* __restrict__ partials, int nblocks, float bv, long long k) {
   __shared__ long long shc[BL_THREADS / 32];
   __shared__ int s_blk;
-  __shared__ long long s_k;
-  const float bv = __uint_as_float((unsigned)best[0]);
+  __shared__ long long s_k, s_out;
   if (threadIdx.x == 0) {
+    s_out = -1;
     int blk = -1;
     long long kk = k;
     for (int b = 0; b < nblocks && blk < 0; ++b) {
@@ -420,19 +433,27 @@ __global__ void __launch_bounds__(BL_THREADS) k_select_kth(const float* __restri
   }
   __syncthreads();
   const int blk = s_blk;
-  if (blk < 0) {
-    if (threadIdx.x == 0) out[0] = -1;
-    return;
+  if (blk >= 0) {                                            // block-uniform
+    const long long lo = min(N, (long long)blk * BL_CHUNK + (long long)threadIdx.x * BL_IPT), hi = min(N, lo + BL_IPT);
+    long long cnt = 0;
+    for (long long i = lo; i < hi; ++i) cnt += (!labeled[i] && v[i] == bv);
+    long long tot;
+    long long r = s_k - block_excl_scan(cnt, shc, tot);
+    if (r >= 0 && r < cnt) {
+      for (long long i = lo; i < hi; ++i)
+        if (!labeled[i] && v[i] == bv && r-- == 0) { s_out = i; break; }
+    }
   }
-  const long long lo = min(N, (long long)blk * BL_CHUNK + (long long)threadIdx.x * BL_IPT), hi = min(N, lo + BL_IPT);
-  long long cnt = 0;
-  for (long long i = lo; i < hi; ++i) cnt += (!labeled[i] && v[i] == bv);
-  long long tot;
-  long long r = s_k - block_excl_scan(cnt, shc, tot);
-  if (r >= 0 && r < cnt) {
-    for (long long i = lo; i < hi; ++i)
-      if (!labeled[i] && v[i] == bv && r-- == 0) { out[0] = i; break; }
-  }
+  __syncthreads();
+  return s_out;
+}
+
+__global__ void __launch_bounds__(BL_THREADS) k_select_kth(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
+                                                          long long N, const long long* __restrict__ partials, int nblocks,
+                                                          const long long* __restrict__ best, long long k,
+                                                          long long* __restrict__ out) {
+  const long long i = kth_in_chunks(v, labeled, N, partials, nblocks, __uint_as_float((unsigned)best[0]), k);
+  if (threadIdx.x == 0) out[0] = i;
 }
 
 extern "C" int coda_b200_select_extreme(const float* v, const uint8_t* labeled, int64_t N, int want_max,
@@ -455,5 +476,300 @@ extern "C" int coda_b200_select_kth(const float* v, const uint8_t* labeled, int6
                                                         coda_b200_select_blocks(N), (const long long*)best, k,
                                                         (long long*)out_idx);
   CODA_LAUNCH_OK("k_select_kth");
+  return CODA_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// N-range shards.  Each call below runs the shard-local pass, then ONE single-CTA kernel that stores this shard's
+// record into every peer's mailbox (record channel of xchg.cuh), waits for every peer's record and merges them in rank
+// order, so every shard leaves with the same global answer.  Selection merges are exact integer / compare operations;
+// the weighted draw adds per-shard fp64 sums in rank order (DESIGN.md §6 (ix)).  With world 1 (x NULL) the kernels
+// touch no mailbox and merge their own record only, which gives the answers of the single-shard entry points.  A peer that never arrives sets CODA_B200_FLAG_XCHG_TIMEOUT in `flags`.
+// ---------------------------------------------------------------------------------------------------------------
+// the epoch of this kernel's (first) exchange; without peers there is no mailbox and no epoch counter to read (the
+// view's epoch pointer is NULL), and the epoch is never used
+__device__ __forceinline__ unsigned long long bl_epoch(const XchgView& x) {
+  return x.world > 1 ? xch_epoch(x, XCH_REC) : 0ull;
+}
+// src of rank s at epoch ep: its slot in the local mailbox, or this shard's own stage when there is no exchange
+__device__ __forceinline__ const void* bl_rec(const XchgView& x, unsigned long long ep, int s, const void* stage) {
+  return x.world > 1 ? (const void*)xch_data(x, XCH_REC, ep, s) : stage;
+}
+// all threads: stage (16-byte aligned, `bytes` a multiple of 16) to every peer, then wait for theirs -> epoch
+__device__ __forceinline__ unsigned long long bl_exchange(const XchgView& x, unsigned long long ep, const void* stage,
+                                                          uint32_t bytes, uint32_t* flags) {
+  if (x.world <= 1) return ep;
+  xch_push(x, XCH_REC, ep, stage, bytes);
+  const bool ok = xch_wait(x, XCH_REC, ep);
+  if (!ok && threadIdx.x == 0) atomicOr(flags, CODA_B200_FLAG_XCHG_TIMEOUT);
+  return ep;
+}
+// all threads, after every read of epoch ep's records
+__device__ __forceinline__ void bl_exchange_done(const XchgView& x, unsigned long long ep) {
+  __syncthreads();
+  if (x.world > 1) xch_done(x, XCH_REC, ep);
+}
+
+// out = {float bits of the global extreme, global count of items equal to it, such items on lower ranks, on this rank}
+__global__ void __launch_bounds__(BL_THREADS) k_extreme_xchg(const long long* __restrict__ partials, int nblocks,
+                                                            int want_max, XchgView x, long long* __restrict__ out,
+                                                            uint32_t* __restrict__ flags) {
+  __shared__ __align__(16) long long stage[2];
+  if (threadIdx.x == 0) {
+    ValCnt t{0.f, 0};
+    for (int b = 0; b < nblocks; ++b) vc_merge(t, ValCnt{__uint_as_float((unsigned)partials[2 * b]), partials[2 * b + 1]}, want_max);
+    stage[0] = (long long)__float_as_uint(t.v);
+    stage[1] = t.n;
+  }
+  __syncthreads();
+  const unsigned long long ep = bl_exchange(x, bl_epoch(x), stage, 16, flags);
+  if (threadIdx.x == 0) {
+    ValCnt g{0.f, 0};
+    for (int s = 0; s < x.world; ++s) {
+      const long long* r = reinterpret_cast<const long long*>(bl_rec(x, ep, s, stage));
+      vc_merge(g, ValCnt{__uint_as_float((unsigned)r[0]), r[1]}, want_max);
+    }
+    long long lower = 0, mine = 0;
+    for (int s = 0; s <= x.rank; ++s) {
+      const long long* r = reinterpret_cast<const long long*>(bl_rec(x, ep, s, stage));
+      const long long n = (g.n > 0 && r[1] > 0 && __uint_as_float((unsigned)r[0]) == g.v) ? r[1] : 0;
+      if (s < x.rank) lower += n;
+      else mine = n;
+    }
+    out[0] = (long long)__float_as_uint(g.v);
+    out[1] = g.n;
+    out[2] = lower;
+    out[3] = mine;
+  }
+  bl_exchange_done(x, ep);
+}
+
+// the k-th tied item over all shards: the shard whose ties cover k picks its local (k - lower)-th, all get n_offset + it
+__global__ void __launch_bounds__(BL_THREADS) k_select_kth_xchg(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
+                                                               long long N, const long long* __restrict__ partials,
+                                                               int nblocks, const long long* __restrict__ best, long long k,
+                                                               long long n_offset, XchgView x, long long* __restrict__ out,
+                                                               uint32_t* __restrict__ flags) {
+  __shared__ __align__(16) long long stage[2];
+  const long long kk = k - best[2];
+  long long i = -1;
+  if (kk >= 0 && kk < best[3])                                // block-uniform
+    i = kth_in_chunks(v, labeled, N, partials, nblocks, __uint_as_float((unsigned)best[0]), kk);
+  if (threadIdx.x == 0) {
+    stage[0] = i >= 0 ? n_offset + i : -1;
+    stage[1] = 0;
+  }
+  __syncthreads();
+  const unsigned long long ep = bl_exchange(x, bl_epoch(x), stage, 16, flags);
+  if (threadIdx.x == 0) {
+    long long g = -1;
+    for (int s = 0; s < x.world; ++s) {
+      const long long r = reinterpret_cast<const long long*>(bl_rec(x, ep, s, stage))[0];
+      if (r >= 0) g = r;
+    }
+    out[0] = g;
+  }
+  bl_exchange_done(x, ep);
+}
+
+// total = {fp64 sum over the shards (rank order) of each shard's block-ordered sum, number of unlabeled items}
+__global__ void __launch_bounds__(BL_THREADS) k_wsum_xchg(const double* __restrict__ partials, int nblocks, XchgView x,
+                                                         double* __restrict__ total, uint32_t* __restrict__ flags) {
+  __shared__ __align__(16) double stage[2];
+  if (threadIdx.x == 0) {
+    double s = 0.0, c = 0.0;
+    for (int b = 0; b < nblocks; ++b) { s += partials[2 * b]; c += partials[2 * b + 1]; }
+    stage[0] = s;
+    stage[1] = c;
+  }
+  __syncthreads();
+  const unsigned long long ep = bl_exchange(x, bl_epoch(x), stage, 16, flags);
+  if (threadIdx.x == 0) {
+    double s = 0.0, c = 0.0;
+    for (int r = 0; r < x.world; ++r) {
+      const double* d = reinterpret_cast<const double*>(bl_rec(x, ep, r, stage));
+      s += d[0];
+      c += d[1];
+    }
+    total[0] = s;
+    total[1] = c;
+  }
+  bl_exchange_done(x, ep);
+}
+
+// Exchange 1: every shard's {sum of its normalised weights (block order), unlabeled count}; every shard forms the grand
+// total in rank order, target = u * grand, and the owner shard (the first one whose running sum passes target, the
+// last non-empty one when rounding leaves none).  The owner draws inside its chunks from the lower ranks' running sum
+// and position.  Exchange 2: {owner?, position, global item, q bits} -> out on every shard.
+__global__ void __launch_bounds__(BL_THREADS) k_wdraw_xchg(const float* __restrict__ w, const uint8_t* __restrict__ labeled,
+                                                          long long N, const double* __restrict__ total,
+                                                          const double* __restrict__ partials, int nblocks, double u,
+                                                          long long n_offset, XchgView x, long long* __restrict__ out,
+                                                          uint32_t* __restrict__ flags) {
+  __shared__ __align__(16) double stage[2];
+  __shared__ __align__(16) long long pick[4];
+  __shared__ int s_own;
+  __shared__ double s_base, s_pos, s_target;
+  if (threadIdx.x == 0) {
+    double s = 0.0, c = 0.0;
+    for (int b = 0; b < nblocks; ++b) { s += partials[2 * b]; c += partials[2 * b + 1]; }
+    stage[0] = s;
+    stage[1] = c;
+  }
+  __syncthreads();
+  const unsigned long long ep = bl_exchange(x, bl_epoch(x), stage, 16, flags);
+  if (threadIdx.x == 0) {
+    double grand = 0.0;
+    for (int r = 0; r < x.world; ++r) grand += reinterpret_cast<const double*>(bl_rec(x, ep, r, stage))[0];
+    const double target = u * grand;
+    double base = 0.0, pos = 0.0;
+    int owner = -1, last = -1;
+    for (int r = 0; r < x.world; ++r) {
+      const double* d = reinterpret_cast<const double*>(bl_rec(x, ep, r, stage));
+      if (d[1] == 0.0) continue;
+      last = r;
+      if (base + d[0] > target) { owner = r; break; }
+      base += d[0];
+      pos += d[1];
+    }
+    if (owner < 0 && last >= 0) {                      // target at or beyond the total: the last unlabeled item
+      const double* d = reinterpret_cast<const double*>(bl_rec(x, ep, last, stage));
+      owner = last;
+      base -= d[0];
+      pos -= d[1];
+    }
+    s_own = owner == x.rank;
+    s_base = base;
+    s_pos = pos;
+    s_target = target;
+  }
+  bl_exchange_done(x, ep);
+  long long res[3] = {-1, -1, 0};
+  if (s_own) wdraw_in_chunks(w, labeled, N, (float)total[0], partials, nblocks, s_base, s_pos, s_target, res);
+  if (threadIdx.x == 0) {
+    const bool own = s_own && res[1] >= 0;
+    pick[0] = own ? 1 : 0;
+    pick[1] = own ? res[0] : -1;
+    pick[2] = own ? n_offset + res[1] : -1;
+    pick[3] = own ? res[2] : 0;
+  }
+  __syncthreads();
+  const unsigned long long ep2 = bl_exchange(x, ep + 1, pick, 32, flags);
+  if (threadIdx.x == 0) {
+    out[0] = -1; out[1] = -1; out[2] = 0;
+    for (int r = 0; r < x.world; ++r) {
+      const long long* p = reinterpret_cast<const long long*>(bl_rec(x, ep2, r, pick));
+      if (p[0] == 1) { out[0] = p[1]; out[1] = p[2]; out[2] = p[3]; }
+    }
+  }
+  bl_exchange_done(x, ep2);
+}
+
+// The owner's `bytes` from src -> dst on every shard (header {owner?, 0, 0, 0} + payload; the others send the header).
+__global__ void __launch_bounds__(BL_THREADS) k_owner_share(const unsigned char* __restrict__ src, int bytes, int own,
+                                                           unsigned char* __restrict__ dst, XchgView x,
+                                                           uint32_t* __restrict__ flags) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  int* hdr = reinterpret_cast<int*>(smem_raw);
+  unsigned char* pay = smem_raw + 16;
+  const int padded = (int)xch_align16((uint32_t)bytes);
+  __shared__ int s_src;
+  if (threadIdx.x < 4) hdr[threadIdx.x] = (threadIdx.x == 0 && own) ? 1 : 0;
+  for (int i = threadIdx.x; i < padded; i += blockDim.x) pay[i] = (own && i < bytes) ? src[i] : (unsigned char)0;
+  __syncthreads();
+  const unsigned long long ep = bl_exchange(x, bl_epoch(x), smem_raw, own ? 16u + (uint32_t)padded : 16u, flags);
+  if (threadIdx.x == 0) {
+    int from = -1;
+    for (int s = 0; s < x.world; ++s)
+      if (reinterpret_cast<const int*>(bl_rec(x, ep, s, smem_raw))[0] == 1) from = s;
+    s_src = from;
+  }
+  __syncthreads();
+  if (s_src >= 0) {
+    const unsigned char* p = reinterpret_cast<const unsigned char*>(bl_rec(x, ep, s_src, smem_raw)) + 16;
+    for (int i = threadIdx.x; i < bytes; i += blockDim.x) dst[i] = p[i];
+  }
+  bl_exchange_done(x, ep);
+}
+
+static int bl_view(const coda_xchg_t* x, XchgView* v, uint32_t need, const char* what) {
+  if (int rc = xchg_view_from(x, v)) return rc;
+  CODA_CHECK_ARG(v->world == 1 || need <= v->slot_bytes[XCH_REC], "%s: %u-byte record larger than the mailbox slot", what, need);
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_select_extreme_xchg(const float* v, const uint8_t* labeled, int64_t N, int want_max,
+                                             int64_t* partials, int64_t* out, const coda_xchg_t* x, uint32_t* flags,
+                                             coda_stream_t stream) {
+  CODA_CHECK_ARG(v && labeled && partials && out && flags, "select_extreme_xchg: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40), "select_extreme_xchg: bad N=%lld", (long long)N);
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 16, "select_extreme_xchg")) return rc;
+  const int nb = coda_b200_select_blocks(N);
+  k_extreme_blocks<<<nb, BL_THREADS, 0, as_stream(stream)>>>(v, labeled, N, want_max, (long long*)partials);
+  CODA_LAUNCH_OK("k_extreme_blocks");
+  k_extreme_xchg<<<1, BL_THREADS, 0, as_stream(stream)>>>((const long long*)partials, nb, want_max, xv, (long long*)out,
+                                                          flags);
+  CODA_LAUNCH_OK("k_extreme_xchg");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_select_kth_xchg(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
+                                         const int64_t* best, int64_t k, int64_t n_offset, int64_t* out_idx,
+                                         const coda_xchg_t* x, uint32_t* flags, coda_stream_t stream) {
+  CODA_CHECK_ARG(v && labeled && partials && best && out_idx && flags, "select_kth_xchg: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40) && k >= 0 && n_offset >= 0, "select_kth_xchg: bad N=%lld k=%lld",
+                 (long long)N, (long long)k);
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 16, "select_kth_xchg")) return rc;
+  k_select_kth_xchg<<<1, BL_THREADS, 0, as_stream(stream)>>>(v, labeled, N, (const long long*)partials,
+                                                             coda_b200_select_blocks(N), (const long long*)best, k,
+                                                             n_offset, xv, (long long*)out_idx, flags);
+  CODA_LAUNCH_OK("k_select_kth_xchg");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_weighted_total_xchg(const float* w, const uint8_t* labeled, int64_t N, double* partials,
+                                             double* total, const coda_xchg_t* x, uint32_t* flags,
+                                             coda_stream_t stream) {
+  CODA_CHECK_ARG(w && labeled && partials && total && flags, "weighted_total_xchg: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40), "weighted_total_xchg: bad N=%lld", (long long)N);
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 16, "weighted_total_xchg")) return rc;
+  const int nb = coda_b200_select_blocks(N);
+  k_wsum_blocks<false><<<nb, BL_THREADS, 0, as_stream(stream)>>>(w, labeled, N, nullptr, partials);
+  CODA_LAUNCH_OK("k_wsum_blocks");
+  k_wsum_xchg<<<1, BL_THREADS, 0, as_stream(stream)>>>(partials, nb, xv, total, flags);
+  CODA_LAUNCH_OK("k_wsum_xchg");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_weighted_draw_xchg(const float* w, const uint8_t* labeled, int64_t N, const double* total,
+                                            double u, int64_t n_offset, double* partials, int64_t* out,
+                                            const coda_xchg_t* x, uint32_t* flags, coda_stream_t stream) {
+  CODA_CHECK_ARG(w && labeled && total && partials && out && flags, "weighted_draw_xchg: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40) && n_offset >= 0, "weighted_draw_xchg: bad N=%lld", (long long)N);
+  CODA_CHECK_ARG(u >= 0.0 && u < 1.0, "weighted_draw_xchg: u must be in [0, 1)");
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 32, "weighted_draw_xchg")) return rc;
+  const int nb = coda_b200_select_blocks(N);
+  k_wsum_blocks<true><<<nb, BL_THREADS, 0, as_stream(stream)>>>(w, labeled, N, total, partials);
+  CODA_LAUNCH_OK("k_wsum_blocks");
+  k_wdraw_xchg<<<1, BL_THREADS, 0, as_stream(stream)>>>(w, labeled, N, total, partials, nb, u, n_offset, xv,
+                                                        (long long*)out, flags);
+  CODA_LAUNCH_OK("k_wdraw_xchg");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_owner_share(const void* src, int bytes, int own, void* dst, const coda_xchg_t* x,
+                                     uint32_t* flags, coda_stream_t stream) {
+  CODA_CHECK_ARG(dst && flags && (src || !own), "owner_share: null pointer");
+  CODA_CHECK_ARG(bytes >= 1 && bytes <= 8192, "owner_share: bad size %d", bytes);
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 16u + xch_align16((uint32_t)bytes), "owner_share")) return rc;
+  const size_t smem = 16 + xch_align16((uint32_t)bytes);
+  k_owner_share<<<1, BL_THREADS, smem, as_stream(stream)>>>((const unsigned char*)src, bytes, own, (unsigned char*)dst,
+                                                            xv, flags);
+  CODA_LAUNCH_OK("k_owner_share");
   return CODA_B200_OK;
 }

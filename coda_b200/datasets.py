@@ -120,6 +120,20 @@ class CompactSlab:
         dense.scatter_(2, (self.ids.to(torch.int64) & 0xFFFF), self.probs)
         return dense
 
+    def item_column(self, idx) -> torch.Tensor:
+        """The dense (H, C) float32 scores of item ``idx``: bit-identical to ``densify()[:, idx]`` (the same
+        element-wise fp32 operations), without densifying anything else."""
+        H, _, C = self.shape
+        p = self.probs[:, idx]
+        s = p[:, 0].clone()
+        for j in range(1, self.K):
+            s = s + p[:, j]
+        inv = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(float(C - self.K), dtype=torch.float32)
+        rest = (1.0 - s) * inv.to(s.device)
+        col = rest[:, None].expand(H, C).clone()
+        col.scatter_(1, (self.ids[:, idx].to(torch.int64) & 0xFFFF), p)
+        return col
+
 
 class CompactDataset:
     def __init__(self, slab: CompactSlab, labels=None, n_offset=0, n_global=None):

@@ -136,6 +136,34 @@ class Mailbox:
             pass
 
 
+def split_slab(preds, nshards, ngpus):
+    """N-range shards of a slab that lives on one device -> [(shard slab, n_offset)]: shards on the home device are
+    VIEWS of the caller's tensor (the kernels take the model stride), the others are contiguous copies on their device.
+    Consecutive shards share a device when there are more shards than GPUs.  Works for a dense tensor and a
+    ``CompactSlab``."""
+    from .synth import shard_range
+    n = preds.shape[1]
+    home = preds.device.index
+    devs = [home] + [d for d in range(torch.cuda.device_count()) if d != home]
+    devs = devs[:max(1, ngpus)]
+    out = []
+    for r in range(nshards):
+        lo, hi = shard_range(n, r, nshards)
+        d = devs[r * len(devs) // nshards]
+        if isinstance(preds, torch.Tensor):
+            view = preds[:, lo:hi]
+            if d != home:
+                view = view.to(torch.device("cuda", d)).contiguous()
+        else:                                           # CompactSlab
+            view = preds.narrow_items(lo, hi)
+            if d != home:
+                view = view.to(torch.device("cuda", d))
+        out.append((view, lo))
+    for d in devs:                                      # the peer copies ran on the current streams; the shards use their own
+        torch.cuda.synchronize(d)
+    return out
+
+
 class SoloGroup:
     """world == 1: no exchange."""
     world = 1
@@ -276,3 +304,53 @@ def choose_among_ties(tie_idx, rng):
     consumes exactly one ``_randbelow(len)``, so choosing a position is RNG-equivalent."""
     order = sorted(int(i) for i in tie_idx)
     return order[rng.choice(range(len(order)))]
+
+
+# host mirrors of the competing selectors' shard merges (csrc/baselines.cu, the *_xchg entry points)
+def merge_extreme(recs, want_max, rank):
+    """recs: per-shard (value, count) in rank order (count 0 = no unlabeled item on that shard).  -> (value, global count,
+    ties on ranks below ``rank``, ties on ``rank``): the rule of k_extreme_xchg."""
+    v, n = 0.0, 0
+    for (b, c) in recs:
+        if c == 0:
+            continue
+        if n == 0 or (b > v if want_max else b < v):
+            v, n = b, c
+        elif b == v:
+            n += c
+    tied = [c if (n > 0 and c > 0 and b == v) else 0 for (b, c) in recs]
+    return v, n, sum(tied[:rank]), tied[rank]
+
+
+def kth_owner(recs, want_max, k):
+    """The shard whose ties cover the k-th tied item (k_select_kth_xchg) and the item's rank among that shard's ties."""
+    for r in range(len(recs)):
+        _v, _n, lower, mine = merge_extreme(recs, want_max, r)
+        if lower <= k < lower + mine:
+            return r, k - lower
+    return -1, -1
+
+
+def draw_owner(sums, counts, u):
+    """k_wdraw_xchg's first merge: per-shard sums of the normalised weights and unlabeled counts in rank order ->
+    (owner shard, running sum and position before it, target = u * grand total), the last non-empty shard when rounding
+    leaves the target at or beyond the total; (-1, 0, 0, target) when no item is unlabeled."""
+    grand = 0.0
+    for s in sums:
+        grand += s
+    target = u * grand
+    base, pos, owner, last = 0.0, 0, -1, -1
+    for r, (s, c) in enumerate(zip(sums, counts)):
+        if c == 0:
+            continue
+        last = r
+        if base + s > target:
+            owner = r
+            break
+        base += s
+        pos += c
+    if owner < 0 and last >= 0:
+        owner = last
+        base -= sums[last]
+        pos -= counts[last]
+    return owner, base, pos, target

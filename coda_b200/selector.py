@@ -21,9 +21,8 @@ import numpy as np
 import torch
 
 from .base import ModelSelector
-from .dist import InProcessGroup, ProcessGroup, SoloGroup, choose_among_ties, default_comm
+from .dist import InProcessGroup, ProcessGroup, SoloGroup, choose_among_ties, default_comm, split_slab
 from .engine import TIE_CAP, build_engines
-from .synth import shard_range
 
 
 class _Unlabeled:
@@ -111,28 +110,7 @@ class CODA(ModelSelector):
 
     @staticmethod
     def _split(preds, nshards, ngpus):
-        """N-range shards of a slab that lives on one device: shards on the home device are VIEWS of the caller's
-        tensor (the kernels take the model stride), the others are contiguous copies on their device."""
-        n = preds.shape[1]
-        home = preds.device.index
-        devs = [home] + [d for d in range(torch.cuda.device_count()) if d != home]
-        devs = devs[:max(1, ngpus)]
-        out = []
-        for r in range(nshards):
-            lo, hi = shard_range(n, r, nshards)
-            d = devs[r * len(devs) // nshards]              # consecutive shards share a device when shards > GPUs
-            if isinstance(preds, torch.Tensor):
-                view = preds[:, lo:hi]
-                if d != home:
-                    view = view.to(torch.device("cuda", d)).contiguous()
-            else:                                           # CompactSlab
-                view = preds.narrow_items(lo, hi)
-                if d != home:
-                    view = view.to(torch.device("cuda", d))
-            out.append((view, lo))
-        for d in devs:                                      # the peer copies ran on the current streams; the shards use their own
-            torch.cuda.synchronize(d)
-        return out
+        return split_slab(preds, nshards, ngpus)
 
     @classmethod
     def from_args(cls, dataset, args):

@@ -358,7 +358,8 @@ int coda_b200_report_gather(const int64_t* rep, int rep_words, int64_t* rep_all,
                             uint32_t* flags, coda_stream_t stream);
 
 /* ---- competing selectors (coda/baselines/<name>.py), over the products of coda_b200_scan_slab ----------------------
- * One shard, dense slab.  Per-item vectors are [N] over all items; `labeled` [N] u8 marks the items already labeled. */
+ * Per-item vectors are [N] over the items of one shard (all items when there is one); `labeled` [N] u8 marks the items
+ * already labeled.  A compact slab is scanned by coda_b200_scan_compact; everything below reads only the scan. */
 
 /* ModelPicker acquisition, modelpicker.py:58-86 (the C-class loop at 74-86 with (N, H) temporaries per class).
  * For item n let Z_c be the models predicting class c, A_c = sum_{h in Z_c} p_h, Q_c = sum_{h in Z_c} p_h log2 p_h,
@@ -395,6 +396,39 @@ int coda_b200_select_extreme(const float* v, const uint8_t* labeled, int64_t N, 
                              int64_t* out /*[2]*/, coda_stream_t stream);
 int coda_b200_select_kth(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
                          const int64_t* best, int64_t k, int64_t* out_idx /*[1]*/, coda_stream_t stream);
+
+/* N-range shards of the same selection calls (one shard per GPU or several per GPU, each with its own stream).  Every
+ * shard makes the same calls in the same order; each call ends in ONE single-CTA kernel that stores this shard's record
+ * into every peer's mailbox (record channel of a box sized by coda_b200_xchg_box_bytes(world, H, C, ...)), waits for
+ * all of them (2 s bound, then CODA_B200_FLAG_XCHG_TIMEOUT in `flags`) and merges them in rank order, so every shard
+ * holds the same global answer.  Vectors, `labeled` and `partials` are this shard's; item indices in the outputs are
+ * global (n_offset + local).  x == NULL or world 1: no mailbox is touched and each call returns what its single-shard
+ * counterpart returns (out[2] = 0 and out[3] = the count for select_extreme_xchg; owner_share copies src to dst).
+ *   select_extreme_xchg: out = {float bits of the global extreme, global count of items equal to it, how many of them
+ *     lie on lower ranks, how many on this rank} -- the same {value, count} as one shard (vc_merge is exact);
+ *   select_kth_xchg: best = that out; the shard whose ties cover k picks its (k - lower)-th, out_idx = global item;
+ *   weighted_total_xchg: total = {sum over the shards in rank order of each shard's fp64 sum, unlabeled count};
+ *   weighted_draw_xchg: the shards' sums of w / (float)total[0] are exchanged; every shard forms the grand total in
+ *     rank order, target = u * grand and the owner shard, which draws inside its chunks starting from the lower ranks'
+ *     running sum and position; out = {global position among the unlabeled items, global item, q bits}.  A shard's
+ *     selection blocks and per-thread runs restart at its first item, so the fp64 partial sums group the items
+ *     differently from one shard: a pick can differ from one shard only when u * total lies within ~1e-16 relative of a
+ *     cumulative boundary. */
+int coda_b200_select_extreme_xchg(const float* v, const uint8_t* labeled, int64_t N, int want_max, int64_t* partials,
+                                  int64_t* out /*[4]*/, const coda_xchg_t* x, uint32_t* flags, coda_stream_t stream);
+int coda_b200_select_kth_xchg(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
+                              const int64_t* best /*[4]*/, int64_t k, int64_t n_offset, int64_t* out_idx /*[1]*/,
+                              const coda_xchg_t* x, uint32_t* flags, coda_stream_t stream);
+int coda_b200_weighted_total_xchg(const float* w, const uint8_t* labeled, int64_t N, double* partials,
+                                  double* total /*[2]*/, const coda_xchg_t* x, uint32_t* flags, coda_stream_t stream);
+int coda_b200_weighted_draw_xchg(const float* w, const uint8_t* labeled, int64_t N, const double* total, double u,
+                                 int64_t n_offset, double* partials, int64_t* out /*[3]*/, const coda_xchg_t* x,
+                                 uint32_t* flags, coda_stream_t stream);
+/* add_label on shards: the shard that holds the labeled item (own = 1; exactly one) sends `bytes` from src -- its hard
+ * row, or the per-model losses of its (H, C) column -- and every shard receives them in dst.  bytes + 16 must fit the
+ * record slot (2 * H * 2 + 64 bytes: an H-float vector does). */
+int coda_b200_owner_share(const void* src, int bytes, int own, void* dst, const coda_xchg_t* x, uint32_t* flags,
+                          coda_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -15,7 +15,7 @@ from . import build as _build
 _LIB = None
 
 OK = 0
-VERSION = 202
+VERSION = 203
 MAX_WORLD = 16
 REC_WORDS = 8
 FLAG_NONFINITE_INPUT = 0x01
@@ -117,9 +117,8 @@ SIGNATURES = {
     "coda_b200_pair_fill": (i32, [p, i32, i64, i32, p, p, p, p, p, p, p, p, p, p]),
     "coda_b200_pair_rows": (i32, [p, i32, i32, p, p, p, p, p, p, p, p, i32, p, p, p, p, p, p]),
     "coda_b200_pair_rows_tc": (i32, [p, i32, i32, p, p, p, p, p, p, p, i32, p, p, p, p, p, p]),
-    "coda_b200_template_gains": (i32, [p, i32, i32, p, p, p, p, p]),
     "coda_b200_eig_blocks": (i32, [i64, i32, i32]),
-    "coda_b200_gain_eig": (i32, [p, i64, i32, i32, p, p, p, p, p, p, p, p, p, p, p, i64, i32, p, p, i32, p, p, p, p]),
+    "coda_b200_gain_eig": (i32, [p, i64, i32, i32, p, p, p, p, p, p, i64, i32, p, p, i32, p, p, p, p]),
     "coda_b200_ell_build": (i32, [p, p, p, i64, i32, p, p, p]),
     "coda_b200_row_gains": (i32, [p, p, i64, i32, i32, p, p, p, p, p]),
     "coda_b200_step_select": (i32, [PS, PX, p]),
@@ -131,10 +130,6 @@ SIGNATURES = {
     "coda_b200_mp_entropy": (i32, [p, p, i32, i64, i32, f64, p, p, i32, p, p]),
     "coda_b200_static_scores": (i32, [p, p, i32, i64, i32, p, p, p]),
     "coda_b200_select_blocks": (i32, [i64]),
-    "coda_b200_weighted_total": (i32, [p, p, i64, p, p, p]),
-    "coda_b200_weighted_draw": (i32, [p, p, i64, p, f64, p, p, p]),
-    "coda_b200_select_extreme": (i32, [p, p, i64, i32, p, p, p]),
-    "coda_b200_select_kth": (i32, [p, p, i64, p, p, i64, p, p]),
     "coda_b200_select_extreme_xchg": (i32, [p, p, i64, i32, p, p, PX, p, p]),
     "coda_b200_select_kth_xchg": (i32, [p, p, i64, p, p, i64, i64, p, PX, p, p]),
     "coda_b200_weighted_total_xchg": (i32, [p, p, i64, p, p, PX, p, p]),

@@ -195,63 +195,28 @@ class _DeviceState:
             with self._on():
                 self.labeled[loc] = 1
 
-    # -- one shard: the selection calls, each followed by its host read ---------------------------------------------
+    # -- the selection calls: enqueue only (every shard is enqueued before the host waits on any), then ``read`` -------
     def extreme(self, v, want_max):
-        """-> (best value over the unlabeled items as a float, number of items exactly equal to it)."""
-        with self._on():
-            self._call("coda_b200_select_extreme", _ptr(v), _ptr(self.labeled), self.N, int(want_max),
-                       _ptr(self.part_i), _ptr(self.best), self._s())
-            bits, cnt = self.best[:2].tolist()
-        return _f32(bits), int(cnt)
-
-    def kth(self, v, k):
-        """The k-th unlabeled item (ascending index) equal to the value of the last ``extreme`` call."""
-        with self._on():
-            self._call("coda_b200_select_kth", _ptr(v), _ptr(self.labeled), self.N, _ptr(self.part_i), _ptr(self.best),
-                       int(k), _ptr(self.out), self._s())
-            idx = int(self.out[0].item())
-        if idx < 0:
-            raise RuntimeError(f"coda_b200: select_kth found no item {k}")
-        return idx
-
-    def total(self, w):
-        """-> (fp64 sum of w over the unlabeled items, their count)."""
-        with self._on():
-            self._call("coda_b200_weighted_total", _ptr(w), _ptr(self.labeled), self.N, _ptr(self.part_f),
-                       _ptr(self.total_buf), self._s())
-            s, n = self.total_buf.tolist()
-        return s, int(n)
-
-    def draw(self, w, u):
-        """random.choices over the unlabeled items with weights w / total (after ``total``) -> (item, its weight)."""
-        with self._on():
-            self._call("coda_b200_weighted_draw", _ptr(w), _ptr(self.labeled), self.N, _ptr(self.total_buf), float(u),
-                       _ptr(self.part_f), _ptr(self.out), self._s())
-            _pos, idx, qbits = self.out.tolist()
-        return int(idx), _f32(qbits)
-
-    # -- shards: enqueue only (every shard is enqueued before the host waits on any), then ``read`` ------------------
-    def extreme_x(self, v, want_max):
         with self._on():
             self._call("coda_b200_select_extreme_xchg", _ptr(v), _ptr(self.labeled), self.N, int(want_max),
                        _ptr(self.part_i), _ptr(self.best), self._x(), _ptr(self.flags), self._s())
 
-    def kth_x(self, v, k):
+    def kth(self, v, k):
         with self._on():
             self._call("coda_b200_select_kth_xchg", _ptr(v), _ptr(self.labeled), self.N, _ptr(self.part_i),
                        _ptr(self.best), int(k), self.n_offset, _ptr(self.out), self._x(), _ptr(self.flags), self._s())
 
-    def total_x(self, w):
+    def total(self, w):
         with self._on():
             self._call("coda_b200_weighted_total_xchg", _ptr(w), _ptr(self.labeled), self.N, _ptr(self.part_f),
                        _ptr(self.total_buf), self._x(), _ptr(self.flags), self._s())
 
-    def draw_x(self, w, u):
+    def draw(self, w, u):
         with self._on():
             self._call("coda_b200_weighted_draw_xchg", _ptr(w), _ptr(self.labeled), self.N, _ptr(self.total_buf),
                        float(u), self.n_offset, _ptr(self.part_f), _ptr(self.out), self._x(), _ptr(self.flags), self._s())
 
-    def share_x(self, src, own, dst):
+    def share(self, src, own, dst):
         """The owner shard's ``src`` (own = True on exactly one shard) -> ``dst`` on every shard."""
         with self._on():
             self._call("coda_b200_owner_share", _ptr(src) if own else None, dst.numel() * dst.element_size(),
@@ -357,8 +322,9 @@ class _Baseline(ModelSelector):
     entropies = property(lambda self: self._cat("ent"))
 
     def _check_exchanges(self):
-        """Raise if an exchange of any shard of this process timed out (its outputs are then not valid)."""
-        if any(st.timed_out() for st in self.states):
+        """Raise if an exchange of any shard of this process timed out (its outputs are then not valid).  One shard
+        has no peer to wait for, so there is no flag to read."""
+        if self._xs and any(st.timed_out() for st in self.states):
             raise RuntimeError("coda_b200.baselines: a peer shard did not reach an exchange within 2 s")
 
     def _read(self, t):
@@ -371,37 +337,28 @@ class _Baseline(ModelSelector):
     def _select_extreme(self, name, want_max, draw_k):
         """Arg-extreme of per-item vector ``name`` with the k-th tie drawn by ``draw_k(count)`` on the host -> (global
         item, extreme value)."""
-        if not self._xs:
-            st = self.state
-            v = getattr(st, name)
-            val, cnt = st.extreme(v, want_max)
-            return st.kth(v, draw_k(cnt)), val
         for st in self.states:
             st.enter()
-            st.extreme_x(getattr(st, name), want_max)
+            st.extreme(getattr(st, name), want_max)
         bits, cnt = self._read(self.state.best[:2])
         k = draw_k(int(cnt))
         for st in self.states:
-            st.kth_x(getattr(st, name), k)
+            st.kth(getattr(st, name), k)
         idx = int(self._read(self.state.out[:1])[0])
         if idx < 0:
             raise RuntimeError(f"coda_b200: select_kth found no item {k}")
         return idx, _f32(bits)
 
     def _total(self):
-        if not self._xs:
-            return self.state.total(self.state.score)
         for st in self.states:
             st.enter()
-            st.total_x(st.score)
+            st.total(st.score)
         s, n = self._read(self.state.total_buf)
         return s, int(n)
 
     def _weighted_draw(self, u):
-        if not self._xs:
-            return self.state.draw(self.state.score, u)
         for st in self.states:
-            st.draw_x(st.score, u)
+            st.draw(st.score, u)
         _pos, idx, qbits = self._read(self.state.out)
         return int(idx), _f32(qbits)
 
@@ -426,7 +383,7 @@ class _Baseline(ModelSelector):
                     src = src.reshape(-1).to(dst.dtype).contiguous()
             srcs.append(src)
         for st, src in zip(self.states, srcs):             # the exchanges back to back, nothing launched in between
-            st.share_x(src, src is not None, getattr(st, dst_name))
+            st.share(src, src is not None, getattr(st, dst_name))
         self.state.leave()
         self._check_exchanges()
         return getattr(self.state, dst_name)

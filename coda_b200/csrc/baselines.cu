@@ -239,13 +239,6 @@ __global__ void __launch_bounds__(BL_THREADS) k_wsum_blocks(const float* __restr
   }
 }
 
-__global__ void k_wsum_final(const double* __restrict__ partials, int nblocks, double* __restrict__ total) {
-  double s = 0.0, c = 0.0;
-  for (int b = 0; b < nblocks; ++b) { s += partials[2 * b]; c += partials[2 * b + 1]; }
-  total[0] = s;
-  total[1] = c;
-}
-
 // Every thread of one block: cum = base0 + running sum of the normalised weights in index order over this vector's
 // chunks; the pick is the first unlabeled item with cum > target (bisect_right), the last one when rounding leaves
 // none.  base0, pos0 (the weight and the number of unlabeled items before this vector) and target are read from
@@ -324,48 +317,7 @@ __device__ void wdraw_in_chunks(const float* __restrict__ w, const uint8_t* __re
   }
 }
 
-// One block: the draw over the whole vector (target = u * the sum of the block partials in block order).
-__global__ void __launch_bounds__(BL_THREADS) k_wdraw_pick(const float* __restrict__ w, const uint8_t* __restrict__ labeled,
-                                                          long long N, const double* __restrict__ total,
-                                                          const double* __restrict__ partials, int nblocks, double u,
-                                                          long long* __restrict__ out) {
-  double target = 0.0;
-  if (threadIdx.x == 0) {
-    double grand = 0.0;
-    for (int b = 0; b < nblocks; ++b) grand += partials[2 * b];
-    target = u * grand;
-  }
-  long long res[3];
-  wdraw_in_chunks(w, labeled, N, (float)total[0], partials, nblocks, 0.0, 0.0, target, res);
-  if (threadIdx.x == 0) { out[0] = res[0]; out[1] = res[1]; out[2] = res[2]; }
-}
-
 extern "C" int coda_b200_select_blocks(int64_t N) { return (int)((N + BL_CHUNK - 1) / BL_CHUNK); }
-
-extern "C" int coda_b200_weighted_total(const float* w, const uint8_t* labeled, int64_t N, double* partials,
-                                        double* total, coda_stream_t stream) {
-  CODA_CHECK_ARG(w && labeled && partials && total, "weighted_total: null pointer");
-  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40), "weighted_total: bad N=%lld", (long long)N);
-  const int nb = coda_b200_select_blocks(N);
-  k_wsum_blocks<false><<<nb, BL_THREADS, 0, as_stream(stream)>>>(w, labeled, N, nullptr, partials);
-  CODA_LAUNCH_OK("k_wsum_blocks");
-  k_wsum_final<<<1, 1, 0, as_stream(stream)>>>(partials, nb, total);
-  CODA_LAUNCH_OK("k_wsum_final");
-  return CODA_B200_OK;
-}
-
-extern "C" int coda_b200_weighted_draw(const float* w, const uint8_t* labeled, int64_t N, const double* total, double u,
-                                       double* partials, int64_t* out, coda_stream_t stream) {
-  CODA_CHECK_ARG(w && labeled && total && partials && out, "weighted_draw: null pointer");
-  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40), "weighted_draw: bad N=%lld", (long long)N);
-  CODA_CHECK_ARG(u >= 0.0 && u < 1.0, "weighted_draw: u must be in [0, 1)");
-  const int nb = coda_b200_select_blocks(N);
-  k_wsum_blocks<true><<<nb, BL_THREADS, 0, as_stream(stream)>>>(w, labeled, N, total, partials);
-  CODA_LAUNCH_OK("k_wsum_blocks");
-  k_wdraw_pick<<<1, BL_THREADS, 0, as_stream(stream)>>>(w, labeled, N, total, partials, nb, u, (long long*)out);
-  CODA_LAUNCH_OK("k_wdraw_pick");
-  return CODA_B200_OK;
-}
 
 // -- extreme value with exact ties (modelpicker.py:68-70 min, uncertainty.py:37-42 max) ---------------------------
 // {value, count} partials merge associatively: the better value wins, equal values add their counts.
@@ -401,13 +353,6 @@ __global__ void __launch_bounds__(BL_THREADS) k_extreme_blocks(const float* __re
     partials[2 * blockIdx.x] = (long long)__float_as_uint(t.v);
     partials[2 * blockIdx.x + 1] = t.n;
   }
-}
-
-__global__ void k_extreme_final(const long long* __restrict__ partials, int nblocks, int want_max, long long* __restrict__ out) {
-  ValCnt t{0.f, 0};
-  for (int b = 0; b < nblocks; ++b) vc_merge(t, ValCnt{__uint_as_float((unsigned)partials[2 * b]), partials[2 * b + 1]}, want_max);
-  out[0] = (long long)__float_as_uint(t.v);
-  out[1] = t.n;
 }
 
 // One block: the k-th (ascending index) unlabeled item whose value equals best[0].  Only blocks whose partial value is
@@ -448,43 +393,13 @@ __device__ long long kth_in_chunks(const float* __restrict__ v, const uint8_t* _
   return s_out;
 }
 
-__global__ void __launch_bounds__(BL_THREADS) k_select_kth(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
-                                                          long long N, const long long* __restrict__ partials, int nblocks,
-                                                          const long long* __restrict__ best, long long k,
-                                                          long long* __restrict__ out) {
-  const long long i = kth_in_chunks(v, labeled, N, partials, nblocks, __uint_as_float((unsigned)best[0]), k);
-  if (threadIdx.x == 0) out[0] = i;
-}
-
-extern "C" int coda_b200_select_extreme(const float* v, const uint8_t* labeled, int64_t N, int want_max,
-                                        int64_t* partials, int64_t* out, coda_stream_t stream) {
-  CODA_CHECK_ARG(v && labeled && partials && out, "select_extreme: null pointer");
-  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40), "select_extreme: bad N=%lld", (long long)N);
-  const int nb = coda_b200_select_blocks(N);
-  k_extreme_blocks<<<nb, BL_THREADS, 0, as_stream(stream)>>>(v, labeled, N, want_max, (long long*)partials);
-  CODA_LAUNCH_OK("k_extreme_blocks");
-  k_extreme_final<<<1, 1, 0, as_stream(stream)>>>((const long long*)partials, nb, want_max, (long long*)out);
-  CODA_LAUNCH_OK("k_extreme_final");
-  return CODA_B200_OK;
-}
-
-extern "C" int coda_b200_select_kth(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
-                                    const int64_t* best, int64_t k, int64_t* out_idx, coda_stream_t stream) {
-  CODA_CHECK_ARG(v && labeled && partials && best && out_idx, "select_kth: null pointer");
-  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40) && k >= 0, "select_kth: bad N=%lld k=%lld", (long long)N, (long long)k);
-  k_select_kth<<<1, BL_THREADS, 0, as_stream(stream)>>>(v, labeled, N, (const long long*)partials,
-                                                        coda_b200_select_blocks(N), (const long long*)best, k,
-                                                        (long long*)out_idx);
-  CODA_LAUNCH_OK("k_select_kth");
-  return CODA_B200_OK;
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// N-range shards.  Each call below runs the shard-local pass, then ONE single-CTA kernel that stores this shard's
+// The selection calls.  Each runs the shard-local pass, then ONE single-CTA kernel that stores this shard's
 // record into every peer's mailbox (record channel of xchg.cuh), waits for every peer's record and merges them in rank
 // order, so every shard leaves with the same global answer.  Selection merges are exact integer / compare operations;
 // the weighted draw adds per-shard fp64 sums in rank order (DESIGN.md §6 (ix)).  With world 1 (x NULL) the kernels
-// touch no mailbox and merge their own record only, which gives the answers of the single-shard entry points.  A peer that never arrives sets CODA_B200_FLAG_XCHG_TIMEOUT in `flags`.
+// touch no mailbox and merge their own record only.  A peer that never arrives sets CODA_B200_FLAG_XCHG_TIMEOUT in
+// `flags`.
 // ---------------------------------------------------------------------------------------------------------------
 // the epoch of this kernel's (first) exchange; without peers there is no mailbox and no epoch counter to read (the
 // view's epoch pointer is NULL), and the epoch is never used

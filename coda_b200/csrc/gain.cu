@@ -1,18 +1,14 @@
-// The per-step scoring pass, item-major: information gain of every hypothetical (item, class) update and the
-// per-item expected information gain, one kernel.
+// The per-step scoring pass, item-major: per-item expected information gain from the gain of every row.
 //
 //   gain(b, c) = H_before - H_after(b, c) = sum_h f(m0_h) - f(m0_h + pi_hat[c] * (PH[b,c,h] - PB[c,h]))   coda.py:254, 274-276
 //   eig[b]     = sum_c pi_hat_xi[b,c] * gain(b, c)                                                          coda.py:278
 //              = (sum_c U[b,c] * g0[c] + sum_{entries} U[b,c_e] * (gain_e - g0[c_e])) / max(sum_c U[b,c], 1e-12)
 //
 // with g0[c] the gain of the "no model predicts c" template row and one entry per distinct predicted class of
-// the item (template row: gain looked up; heavy row: computed here from the cached P(best | hypothetical) row).
-// The heavy rows of an item are contiguous in HBM, so are its entries and its U row: a warp that walks items in
-// order streams three sequential arrays.  PB (C x Hp fp32, 100 KB at cfg3) lives in shared memory.
+// the item.  The gains of all rows come from row_gains (cached rows) or pair_rows (no cache); the assembly looks
+// them up.  An item's entries and its U row are contiguous in HBM: a warp that walks items in order streams them.
 // Candidate filter (coda.py:215-219, 239) and the arg-max with runner-up (coda.py:306-309) ride along.
 #include "common.cuh"
-
-#include <stdlib.h>
 
 #define GE_THREADS 384
 #define GE_WARPS (GE_THREADS / 32)
@@ -20,23 +16,17 @@
 struct GainEigArgs {
   const float* U;
   long long N;
-  int C, H, Hp, T;
+  int C, H;
   const int32_t* ent_off;
-  const int32_t* heavy_off;
   const int32_t* ent_row;
   const uint16_t* ent_cls;
-  const float* ph_cache;
   const float* gain;
-  const float* PB;
-  const float* m0;
-  const float* pi_hat;
   const uint8_t* labeled;
   const uint8_t* disagree;
   long long n_offset;
   float* eig;
   long long* partials;
   uint32_t* flags;
-  int pb_smem;
   const int32_t* ell_row;     // optional ELL copy of the entry lists: [N][ell_k] row ids (-1 = empty) ...
   const uint16_t* ell_cls;    // ... and classes
   int ell_k;
@@ -50,55 +40,18 @@ __device__ __forceinline__ float gain4(const float4 ph, const float4 pb, const f
   return g;
 }
 
-// NQ: Hp == 128 * NQ keeps m0 / f(m0) in registers (NQ = 0: any Hp, shared-memory copies).
-// KC: C <= 32 * KC keeps the item's U row in registers (KC = 0: any C, the row is re-read).
-template <int NQ, int KC, bool FROM_CACHE, bool PBS>
+// one warp per item, any C and any number of entries per item (the 8-lane assembly below takes C <= 128 and
+// <= 32 entries).  KC: C <= 32 * KC keeps the item's U row in registers (KC = 0: any C, the row is re-read).
+template <int KC>
 __global__ void __launch_bounds__(GE_THREADS, 2) k_gain_eig(GainEigArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int C = a.C, H = a.H, Hp = a.Hp, T = a.T;
-  // [PB copy (C x Hp, FROM_CACHE && pb_smem)] [m0, f(m0) (NQ == 0)] [g0 (C)] [pi_hat (C)] -- float4-read parts first
-  float* pbs = reinterpret_cast<float*>(smem_raw);
-  float* m0s = pbs + ((FROM_CACHE && PBS) ? (size_t)C * Hp : 0);   // [Hp]  (NQ == 0 only)
-  float* fm0 = m0s + (NQ == 0 ? Hp : 0);                                 // [Hp]  (NQ == 0 only)
-  float* g0 = fm0 + (NQ == 0 ? Hp : 0);                                  // [C]   gain of the empty-set template row
-  float* pis = g0 + C;                                                   // [C]   pi_hat
+  const int C = a.C, H = a.H;
+  float* g0 = reinterpret_cast<float*>(smem_raw);                        // [C]   gain of the empty-set template row
   __shared__ float s_v[2][GE_WARPS], s_v2[2][GE_WARPS];
   __shared__ long long s_i[2][GE_WARPS], s_c[GE_WARPS];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int c = tid; c < C; c += GE_THREADS) {
-    g0[c] = a.gain[(size_t)c * (1 + H)];
-    pis[c] = a.pi_hat[c];
-  }
-  if (NQ == 0) {
-    for (int h = tid; h < Hp; h += GE_THREADS) {
-      const float m = h < H ? a.m0[h] : 0.f;
-      m0s[h] = m;
-      fm0[h] = ent_term(m);
-    }
-  }
-  if (FROM_CACHE && PBS) {
-    const float4* src = reinterpret_cast<const float4*>(a.PB);
-    float4* dst = reinterpret_cast<float4*>(pbs);
-    for (int i = tid; i < C * Hp / 4; i += GE_THREADS) dst[i] = __ldg(src + i);
-  }
+  for (int c = tid; c < C; c += GE_THREADS) g0[c] = a.gain[(size_t)c * (1 + H)];
   __syncthreads();
-  const float* pbt = a.PB;   // PBS: the shared-memory copy `pbs` is used instead (kept apart so the loads are LDS)
-
-  constexpr int NQR = NQ > 0 ? NQ : 1;
-  float4 m[NQR], fm[NQR];
-  if (NQ > 0) {
-#pragma unroll
-    for (int q = 0; q < NQR; ++q) {
-      const int h = (q * 32 + lane) * 4;
-      float4 v = __ldg(reinterpret_cast<const float4*>(a.m0) + q * 32 + lane);
-      if (h + 0 >= H) v.x = 0.f;
-      if (h + 1 >= H) v.y = 0.f;
-      if (h + 2 >= H) v.z = 0.f;
-      if (h + 3 >= H) v.w = 0.f;
-      m[q] = v;
-      fm[q] = make_float4(ent_term(v.x), ent_term(v.y), ent_term(v.z), ent_term(v.w));
-    }
-  }
 
   Best2 bA = best2_empty(), bB = best2_empty();
   long long cntA = 0;
@@ -106,18 +59,16 @@ __global__ void __launch_bounds__(GE_THREADS, 2) k_gain_eig(GainEigArgs a) {
   constexpr int KR = KC > 0 ? KC : 1;
   const long long nw = (long long)gridDim.x * GE_WARPS;
   long long n = (long long)blockIdx.x * GE_WARPS + warp;
-  int e0 = 0, e1 = 0, h0 = 0, h1 = 0;
+  int e0 = 0, e1 = 0;
   if (n < a.N) {
     e0 = __ldg(a.ent_off + n); e1 = __ldg(a.ent_off + n + 1);
-    h0 = __ldg(a.heavy_off + n); h1 = __ldg(a.heavy_off + n + 1);
   }
   while (n < a.N) {
     // offsets of the next item this warp will visit: one memory latency ahead
     const long long nn = n + nw;
-    int ne0 = 0, ne1 = 0, nh0 = 0, nh1 = 0;
+    int ne0 = 0, ne1 = 0;
     if (nn < a.N) {
       ne0 = __ldg(a.ent_off + nn); ne1 = __ldg(a.ent_off + nn + 1);
-      nh0 = __ldg(a.heavy_off + nn); nh1 = __ldg(a.heavy_off + nn + 1);
     }
     const float* urow = a.U + (size_t)n * C;
     float u[KR];
@@ -129,83 +80,13 @@ __global__ void __launch_bounds__(GE_THREADS, 2) k_gain_eig(GainEigArgs a) {
         u[k] = c < C ? __ldg(urow + c) : 0.f;
       }
     }
-    int hrow = T + h0;     // next heavy row of this item
     for (int eb = e0; eb < e1; eb += 32) {       // one trip unless an item has > 32 distinct predicted classes
       int r = -1, c = 0;
       if (eb + lane < e1) {
         r = __ldg(a.ent_row + eb + lane);
         c = __ldg(a.ent_cls + eb + lane);
       }
-      float myg = 0.f;
-      if (!FROM_CACHE) {
-        if (r >= 0) myg = __ldg(a.gain + r);
-      } else {
-        // the row addresses follow from the offsets alone: when the item has one entry chunk (the usual case) the
-        // row loads are issued BEFORE the entry loads are waited for -- one dependent memory level less
-        const bool single = (e1 - e0) <= 32;
-        uint32_t hm = 0;
-        int nh = h1 - h0;
-        if (!single) {
-          hm = __ballot_sync(CODA_FULL, r >= T);
-          nh = __popc(hm);
-        }
-        if (NQ > 0) {
-          for (int i = 0; i < nh; i += 4) {
-            float4 row[4][NQR];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int rr = hrow + min(i + j, nh - 1);
-              const float4* rp = reinterpret_cast<const float4*>(a.ph_cache + (size_t)rr * Hp);
-#pragma unroll
-              for (int q = 0; q < NQR; ++q) row[j][q] = __ldg(rp + q * 32 + lane);
-            }
-            if (single && i == 0) {
-              hm = __ballot_sync(CODA_FULL, r >= T);
-              if (r >= 0 && r < T) myg = __ldg(a.gain + r);
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              if (i + j < nh) {
-                const int li = __ffs(hm) - 1;
-                hm &= hm - 1;
-                const int cj = __shfl_sync(CODA_FULL, c, li);
-                const float pic = pis[cj];
-                const float4* pb = reinterpret_cast<const float4*>((PBS ? pbs : pbt) + (size_t)cj * Hp);
-                float g = 0.f;
-#pragma unroll
-                for (int q = 0; q < NQR; ++q) g += gain4(row[j][q], pb[q * 32 + lane], m[q], fm[q], pic);
-                g = warp_sum(g);
-                if (lane == li) myg = g;
-              }
-            }
-          }
-          if (!single || nh == 0) {
-            if (r >= 0 && r < T) myg = __ldg(a.gain + r);
-          }
-        } else {
-          if (single) hm = __ballot_sync(CODA_FULL, r >= T);
-          if (r >= 0 && r < T) myg = __ldg(a.gain + r);
-          for (int i = 0; i < nh; ++i) {
-            const int li = __ffs(hm) - 1;
-            hm &= hm - 1;
-            const int cj = __shfl_sync(CODA_FULL, c, li);
-            const float pic = pis[cj];
-            const float* rp = a.ph_cache + (size_t)(hrow + i) * Hp;
-            const float* pb = (PBS ? pbs : pbt) + (size_t)cj * Hp;
-            float g = 0.f;
-            for (int hq = lane * 4; hq < Hp; hq += 128) {
-              const float4 ph = __ldg(reinterpret_cast<const float4*>(rp + hq));
-              const float4 p4 = *reinterpret_cast<const float4*>(pb + hq);
-              const float4 m4 = *reinterpret_cast<const float4*>(m0s + hq);
-              const float4 f4 = *reinterpret_cast<const float4*>(fm0 + hq);
-              g += gain4(ph, p4, m4, f4, pic);
-            }
-            g = warp_sum(g);
-            if (lane == li) myg = g;
-          }
-        }
-        hrow += nh;
-      }
+      const float myg = r >= 0 ? __ldg(a.gain + r) : 0.f;
       // correction of this chunk's entries: xi_c * (gain - gain of the empty-set template)
       float ucls = 0.f;
       if (KC > 0) {
@@ -247,7 +128,7 @@ __global__ void __launch_bounds__(GE_THREADS, 2) k_gain_eig(GainEigArgs a) {
         }
       }
     }
-    n = nn; e0 = ne0; e1 = ne1; h0 = nh0; h1 = nh1;
+    n = nn; e0 = ne0; e1 = ne1;
   }
   if (lane == 0) {
     s_v[0][warp] = bA.v; s_i[0][warp] = bA.i; s_v2[0][warp] = bA.v2;
@@ -401,8 +282,11 @@ extern "C" int coda_b200_row_gains(const float* ph_cache, const uint16_t* row_cl
 // instruction, IT8 batches in flight; three dependent load levels (offsets -> entries + U row -> gains), each
 // issued for all items of the batch before the first use.
 // ---------------------------------------------------------------------------------------
-template <int KC8, int IT8>
-__global__ void __launch_bounds__(256, (IT8 == 1 ? 3 : 2)) k_eig_assemble_g8(GainEigArgs a, int nblocks_rec) {
+// The arguments are read in place from the parameter bank (__grid_constant__): left free to copy them, ptxas schedules
+// the C <= 64 and C <= 104 instantiations differently, about 1 us per step slower at cfg3 on an H100 (700 W).
+constexpr int IT8 = 2;     // items per 8-lane group and iteration
+template <int KC8>
+__global__ void __launch_bounds__(256, 2) k_eig_assemble_g8(const __grid_constant__ GainEigArgs a, int nblocks_rec) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* g0 = reinterpret_cast<float*>(smem_raw);   // [C]
   __shared__ float s_v[2][8], s_v2[2][8];
@@ -523,14 +407,6 @@ __global__ void __launch_bounds__(256, (IT8 == 1 ? 3 : 2)) k_eig_assemble_g8(Gai
   if (bad) atomicOr(a.flags, bad);
 }
 
-static size_t gain_eig_smem(int C, int Hp, bool nq0, bool pb_smem) {
-  size_t b = (size_t)2 * C * 4 + (nq0 ? (size_t)2 * Hp * 4 : 0) + 16;
-  if (pb_smem) b += (size_t)C * Hp * 4;
-  return b;
-}
-
-static bool gain_eig_pb_in_smem(int C, int Hp) { return (size_t)C * Hp * 4 <= 104 * 1024; }
-
 extern "C" int coda_b200_eig_blocks(int64_t N, int H, int C) {
   (void)H; (void)C;
   long long want = (N + GE_WARPS - 1) / GE_WARPS;
@@ -539,44 +415,29 @@ extern "C" int coda_b200_eig_blocks(int64_t N, int H, int C) {
 }
 
 extern "C" int coda_b200_gain_eig(const float* U, int64_t N, int C, int H, const int32_t* ent_off,
-                                  const int32_t* heavy_off, const int32_t* ent_row, const uint16_t* ent_cls,
-                                  const float* ph_cache, const float* gain, const float* PB, const float* m0,
-                                  const float* pi_hat, const uint8_t* labeled, const uint8_t* disagree,
-                                  int64_t n_offset, int max_entries, const int32_t* ell_row, const uint16_t* ell_cls,
-                                  int ell_k, float* eig, int64_t* partials, uint32_t* flags, coda_stream_t stream) {
-  CODA_CHECK_ARG(U && ent_off && heavy_off && ent_row && ent_cls && gain && PB && m0 && pi_hat && labeled && disagree &&
-                     eig && partials && flags,
+                                  const int32_t* ent_row, const uint16_t* ent_cls, const float* gain,
+                                  const uint8_t* labeled, const uint8_t* disagree, int64_t n_offset, int max_entries,
+                                  const int32_t* ell_row, const uint16_t* ell_cls, int ell_k, float* eig,
+                                  int64_t* partials, uint32_t* flags, coda_stream_t stream) {
+  CODA_CHECK_ARG(U && ent_off && ent_row && ent_cls && gain && labeled && disagree && eig && partials && flags,
                  "gain_eig: null pointer");
   CODA_CHECK_ARG(N >= 1 && C >= 2 && H >= 1, "gain_eig: bad dims");
   GainEigArgs a;
-  a.U = U; a.N = N; a.C = C; a.H = H; a.Hp = (H + 31) / 32 * 32; a.T = C * (1 + H);
-  a.ent_off = ent_off; a.heavy_off = heavy_off; a.ent_row = ent_row; a.ent_cls = ent_cls;
-  a.ph_cache = ph_cache; a.gain = gain; a.PB = PB; a.m0 = m0; a.pi_hat = pi_hat;
+  a.U = U; a.N = N; a.C = C; a.H = H;
+  a.ent_off = ent_off; a.ent_row = ent_row; a.ent_cls = ent_cls; a.gain = gain;
   a.labeled = labeled; a.disagree = disagree; a.n_offset = n_offset; a.eig = eig;
   a.partials = reinterpret_cast<long long*>(partials); a.flags = flags;
   a.ell_row = (ell_row && ell_cls && ell_k >= 1 && ell_k <= 32) ? ell_row : nullptr;
   a.ell_cls = ell_cls; a.ell_k = ell_k;
-  const bool from_cache = ph_cache != nullptr;
-  const int nq = !from_cache ? 0 : ((a.Hp == 128) ? 1 : (a.Hp == 256 ? 2 : 0));   // NQ = 0: m0 / f(m0) copies in shared memory
-  const int kc = C <= 32 ? 1 : (C <= 64 ? 2 : (C <= 128 ? 4 : 0));
-  a.pb_smem = from_cache && gain_eig_pb_in_smem(C, a.Hp);
-  const size_t smem = gain_eig_smem(C, a.Hp, nq == 0, a.pb_smem);
+  const size_t smem = (size_t)C * 4;                     // g0
   CODA_CHECK_ARG(smem <= 220 * 1024, "gain_eig: C=%d does not fit shared memory", C);
   const int grid = coda_b200_eig_blocks(N, H, C);
   cudaStream_t st = as_stream(stream);
-  if (!from_cache && C <= 128 && max_entries >= 0 && max_entries <= 32) {
+  if (C <= 128 && max_entries >= 0 && max_entries <= 32) {
     // 8-lane groups: the grid may be smaller than the record count the caller merges (block 0 writes empty records)
-    // CODA_B200_ASM=it1: one item per 8-lane group and iteration (fewer registers, three CTAs per SM) -- A/B knob
-    const char* asm_env = getenv("CODA_B200_ASM");
-    const bool it1 = asm_env && asm_env[0] == 'i' && asm_env[2] == '1';
-    int g8 = (int)min((long long)(N + 31) / 32, (long long)min(grid, coda_sm_count() * (it1 ? 3 : 2)));
+    int g8 = (int)min((long long)(N + 31) / 32, (long long)min(grid, coda_sm_count() * 2));
     if (g8 < 1) g8 = 1;
-    const size_t sm8 = (size_t)C * 4;
-#define LAUNCH_G8(K8)                                                         \
-  do {                                                                        \
-    if (it1) k_eig_assemble_g8<K8, 1><<<g8, 256, sm8, st>>>(a, grid);         \
-    else k_eig_assemble_g8<K8, 2><<<g8, 256, sm8, st>>>(a, grid);             \
-  } while (0)
+#define LAUNCH_G8(K8) k_eig_assemble_g8<K8><<<g8, 256, smem, st>>>(a, grid)
     if (C <= 32) LAUNCH_G8(4);
     else if (C <= 64) LAUNCH_G8(8);
     else if (C <= 104) LAUNCH_G8(13);
@@ -585,75 +446,17 @@ extern "C" int coda_b200_gain_eig(const float* U, int64_t N, int C, int H, const
     CODA_LAUNCH_OK("k_eig_assemble_g8");
     return CODA_B200_OK;
   }
-#define LAUNCH_GE2(NQ, KC, FC, PBS)                                                                                      \
-  do {                                                                                                                   \
-    CODA_CUDA_OK(cudaFuncSetAttribute(k_gain_eig<NQ, KC, FC, PBS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    k_gain_eig<NQ, KC, FC, PBS><<<grid, GE_THREADS, smem, st>>>(a);                                                       \
+#define LAUNCH_GE(KC)                                                                                        \
+  do {                                                                                                       \
+    CODA_CUDA_OK(cudaFuncSetAttribute(k_gain_eig<KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    k_gain_eig<KC><<<grid, GE_THREADS, smem, st>>>(a);                                                        \
   } while (0)
-#define LAUNCH_GE(NQ, KC, FC)                                \
-  do {                                                       \
-    if (FC && a.pb_smem) LAUNCH_GE2(NQ, KC, FC, FC);          \
-    else LAUNCH_GE2(NQ, KC, FC, false);                      \
-  } while (0)
-#define PICK_KC(NQ, FC)                          \
-  do {                                           \
-    if (kc == 1) LAUNCH_GE(NQ, 1, FC);           \
-    else if (kc == 2) LAUNCH_GE(NQ, 2, FC);      \
-    else if (kc == 4) LAUNCH_GE(NQ, 4, FC);      \
-    else LAUNCH_GE(NQ, 0, FC);                   \
-  } while (0)
-  if (!from_cache) PICK_KC(0, false);
-  else if (nq == 1) PICK_KC(1, true);
-  else if (nq == 2) PICK_KC(2, true);
-  else PICK_KC(0, true);
-#undef PICK_KC
+  if (C <= 32) LAUNCH_GE(1);
+  else if (C <= 64) LAUNCH_GE(2);
+  else if (C <= 128) LAUNCH_GE(4);
+  else LAUNCH_GE(0);
 #undef LAUNCH_GE
-#undef LAUNCH_GE2
   CODA_LAUNCH_OK("k_gain_eig");
-  return CODA_B200_OK;
-}
-
-// gain of the T template rows (class-major: row = c * (1 + H) + k) from their cached rows: one warp per row.
-__global__ void __launch_bounds__(256) k_template_gains(const float* __restrict__ ph_cache, int H, int Hp, int T,
-                                                        const float* __restrict__ PB, const float* __restrict__ m0,
-                                                        const float* __restrict__ pi_hat, float* __restrict__ gain) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  float* m0s = reinterpret_cast<float*>(smem_raw);   // [Hp]
-  float* fm0 = m0s + Hp;                             // [Hp]  f(m0); padded models carry f(0) so they cancel
-  for (int h = threadIdx.x; h < Hp; h += blockDim.x) {
-    const float m = h < H ? m0[h] : 0.f;
-    m0s[h] = m;
-    fm0[h] = ent_term(m);
-  }
-  __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int r = blockIdx.x * 8 + warp; r < T; r += gridDim.x * 8) {
-    const int c = r / (1 + H);
-    const float pic = pi_hat[c];
-    const float* row = ph_cache + (size_t)r * Hp;
-    const float* pb = PB + (size_t)c * Hp;
-    float g = 0.f;
-    for (int hq = lane * 4; hq < Hp; hq += 128) {
-      const float4 ph = __ldg(reinterpret_cast<const float4*>(row + hq));
-      const float4 p4 = __ldg(reinterpret_cast<const float4*>(pb + hq));
-      const float4 m4 = *reinterpret_cast<const float4*>(m0s + hq);
-      const float4 f4 = *reinterpret_cast<const float4*>(fm0 + hq);
-      g += gain4(ph, p4, m4, f4, pic);
-    }
-    g = warp_sum(g);
-    if (lane == 0) gain[r] = g;
-  }
-}
-
-extern "C" int coda_b200_template_gains(const float* ph_cache, int H, int C, const float* PB, const float* m0,
-                                        const float* pi_hat, float* gain, coda_stream_t stream) {
-  CODA_CHECK_ARG(ph_cache && PB && m0 && pi_hat && gain, "template_gains: null pointer");
-  const int Hp = (H + 31) / 32 * 32, T = C * (1 + H);
-  int grid = (T + 7) / 8;
-  const int cap = coda_sm_count() * 8;
-  if (grid > cap) grid = cap;
-  k_template_gains<<<grid, 256, (size_t)2 * Hp * 4, as_stream(stream)>>>(ph_cache, H, Hp, T, PB, m0, pi_hat, gain);
-  CODA_LAUNCH_OK("k_template_gains");
   return CODA_B200_OK;
 }
 

@@ -12,7 +12,6 @@
 #include "common.cuh"
 #include "terms.cuh"
 
-#include <stdlib.h>
 #include <type_traits>
 
 // ---------------------------------------------------------------------------------------
@@ -730,13 +729,13 @@ __device__ __forceinline__ void rows_accumulate_reg(float* __restrict__ U, long 
 __constant__ R1Term c_terms_bank[R1_CONST_TERMS];
 
 #define R1_TN 256
-// GU: gathers in flight per lane, NR: U rows in flight per warp (more of both = more bytes in flight per SM at
-// the price of registers / resident warps)
+#define R1_GU 16                                   // gathers in flight per lane
+#define R1_NR 4                                    // U rows in flight per warp
 // T: slab element type.  A 16-bit slab keeps the ensemble sums in fp32 behind their own base pointer `ensb`: the first
 // term of a list with a majority class (hdr[1] >= 0) is read from there, every other term from the slab.  For fp32 both
 // live behind `preds` (ensb is not read).  Term order and the fmaf chain are the same either way.
-template <typename T, int KC, int GU = 16, int NR = 4, bool CONST_TERMS = false>
-__global__ void __launch_bounds__(256, (GU > 16 ? 3 : 4)) k_pi_rank1(const T* __restrict__ preds, const float* __restrict__ ensb,
+template <typename T, int KC, bool CONST_TERMS = false>
+__global__ void __launch_bounds__(256, 4) k_pi_rank1(const T* __restrict__ preds, const float* __restrict__ ensb,
                                                   long long N, int C, const long long* __restrict__ sel,
                                                   const int32_t* __restrict__ hdr, const R1Term* __restrict__ gterms,
                                                   int const_base, float lr, float fxs,
@@ -771,23 +770,23 @@ __global__ void __launch_bounds__(256, (GU > 16 ? 3 : 4)) k_pi_rank1(const T* __
         d = fmaf(c_terms[0].sg, __ldg(ensb + c_terms[0].off + n * c_terms[0].str), d);
         k = 1;
       }
-      for (; k + GU <= nt; k += GU) {
-        float v[GU];
+      for (; k + R1_GU <= nt; k += R1_GU) {
+        float v[R1_GU];
 #pragma unroll
-        for (int q = 0; q < GU; ++q) v[q] = ldg_f(preds + c_terms[k + q].off + n * c_terms[k + q].str);
+        for (int q = 0; q < R1_GU; ++q) v[q] = ldg_f(preds + c_terms[k + q].off + n * c_terms[k + q].str);
 #pragma unroll
-        for (int q = 0; q < GU; ++q) d = fmaf(c_terms[k + q].sg, v[q], d);
+        for (int q = 0; q < R1_GU; ++q) d = fmaf(c_terms[k + q].sg, v[q], d);
       }
       for (; k < nt; ++k) d = fmaf(c_terms[k].sg, ldg_f(preds + c_terms[k].off + n * c_terms[k].str), d);
     }
     const float dl = lr * d;
     const int rows = (int)min(32LL, N - n0);
     if (KC > 0) {
-      for (int r = 0; r < rows; r += NR) {
-        float dv[NR];
+      for (int r = 0; r < rows; r += R1_NR) {
+        float dv[R1_NR];
 #pragma unroll
-        for (int i = 0; i < NR; ++i) dv[i] = __shfl_sync(CODA_FULL, dl, (r + i) & 31);
-        rows_accumulate_reg<(KC > 0 ? KC : 1), NR>(U, n0 + r, rows - r, 1, C, lane, fxs, t, dv, racc, bad);
+        for (int i = 0; i < R1_NR; ++i) dv[i] = __shfl_sync(CODA_FULL, dl, (r + i) & 31);
+        rows_accumulate_reg<(KC > 0 ? KC : 1), R1_NR>(U, n0 + r, rows - r, 1, C, lane, fxs, t, dv, racc, bad);
       }
     } else {
       for (int r = 0; r < rows; ++r) {
@@ -812,321 +811,6 @@ __global__ void __launch_bounds__(256, (GU > 16 ? 3 : 4)) k_pi_rank1(const T* __
   if (bad) atomicOr(flags, bad);
 }
 
-// pi_rank1 with four consecutive items per lane (C <= 128): a warp owns 128 consecutive items, so every gather
-// from the class-major shadow is one 512-byte contiguous run per term (float4 per lane) instead of 128 bytes --
-// four times fewer DRAM page switches for the same bytes.  Same arithmetic, same order as k_pi_rank1.
-#define R1V_WI 128     // items per warp
-// four consecutive items of one class-major column (16-byte aligned for fp32, 8-byte for 16-bit) -> fp32
-__device__ __forceinline__ void ldg4_f(const float* p, float (&v)[4]) {
-  const float4 x = __ldg(reinterpret_cast<const float4*>(p));
-  v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
-}
-__device__ __forceinline__ void ldg4_f(const __half* p, float (&v)[4]) {
-  const uint2 x = __ldg(reinterpret_cast<const uint2*>(p));
-  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&x.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&x.y));
-  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
-}
-__device__ __forceinline__ void ldg4_f(const __nv_bfloat16* p, float (&v)[4]) {
-  const uint2 x = __ldg(reinterpret_cast<const uint2*>(p));
-  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&x.x));
-  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&x.y));
-  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
-}
-
-template <int KC, typename T>
-__global__ void __launch_bounds__(256, 3) k_pi_rank1_v4(const T* __restrict__ preds, const float* __restrict__ ensb,
-                                                     long long N, int C, const long long* __restrict__ sel,
-                                                     const int32_t* __restrict__ hdr, const R1Term* __restrict__ gterms,
-                                                     float lr, float fxs, float* __restrict__ U,
-                                                     unsigned long long* __restrict__ pisum_fx,
-                                                     uint32_t* __restrict__ flags) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  long long* wacc_all = reinterpret_cast<long long*>(smem_raw);                 // [8][C]
-  R1Term* c_terms = reinterpret_cast<R1Term*>(wacc_all + (size_t)8 * C);        // [nt]
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int t = (int)sel[1];
-  const int nt = hdr[0];
-  const bool ens_f32 = !std::is_same<T, float>::value && hdr[1] >= 0;      // see k_pi_rank1
-  for (int k = threadIdx.x; k < nt; k += blockDim.x) c_terms[k] = gterms[k];
-  long long racc[KC];
-#pragma unroll
-  for (int k = 0; k < KC; ++k) racc[k] = 0;
-  __syncthreads();
-  uint32_t bad = 0;
-  const long long cta_items = (long long)8 * R1V_WI;
-  for (long long n0 = (long long)blockIdx.x * cta_items + (long long)warp * R1V_WI; n0 < N; n0 += (long long)gridDim.x * cta_items) {
-    const long long nl = n0 + 4 * lane;
-    const bool full4 = nl + 3 < N;
-    float d[4] = {0.f, 0.f, 0.f, 0.f};
-    int k = 0;
-    if (ens_f32) {
-      const R1Term tm = c_terms[0];
-      float v[4];
-      if (tm.str == 1 && full4) {
-        ldg4_f(ensb + tm.off + nl, v);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) v[i] = (nl + i < N) ? __ldg(ensb + tm.off + (nl + i) * tm.str) : 0.f;
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) d[i] = fmaf(tm.sg, v[i], d[i]);
-      k = 1;
-    }
-    for (; k + 8 <= nt; k += 8) {
-      float v[8][4];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const R1Term tm = c_terms[k + q];
-        if (tm.str == 1 && full4) {
-          ldg4_f(preds + tm.off + nl, v[q]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) v[q][i] = (nl + i < N) ? ldg_f(preds + tm.off + (nl + i) * tm.str) : 0.f;
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float sg = c_terms[k + q].sg;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) d[i] = fmaf(sg, v[q][i], d[i]);
-      }
-    }
-    for (; k < nt; ++k) {
-      const R1Term tm = c_terms[k];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float x = (nl + i < N) ? ldg_f(preds + tm.off + (nl + i) * tm.str) : 0.f;
-        d[i] = fmaf(tm.sg, x, d[i]);
-      }
-    }
-    float dl[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) dl[i] = lr * d[i];
-    const int rows = (int)min((long long)R1V_WI, N - n0);
-    for (int r = 0; r < rows; r += 4) {
-      float dv[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) dv[i] = __shfl_sync(CODA_FULL, dl[i], r >> 2);
-      rows_accumulate_reg<KC, 4>(U, n0 + r, rows - r, 1, C, lane, fxs, t, dv, racc, bad);
-    }
-  }
-  long long* wacc = wacc_all + (size_t)warp * C;
-#pragma unroll
-  for (int k = 0; k < KC; ++k) {
-    const int c = lane + 32 * k;
-    if (c < C) wacc[c] = racc[k];
-  }
-  __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    long long s2 = 0;
-    for (int w = 0; w < 8; ++w) s2 += wacc_all[(size_t)w * C + c];
-    if (s2) atomicAdd(pisum_fx + c, (unsigned long long)s2);
-  }
-  if (bad) atomicOr(flags, bad);
-}
-
-// ---------------------------------------------------------------------------------------
-// pi_rank1, bulk-TMA pipeline (C <= 128): the same arithmetic in the same order as k_pi_rank1, fed differently.
-// A persistent CTA walks tiles of TR items.  Everything a tile needs is contiguous in HBM:
-//   * the U rows of the tile            TR*C floats   -> ONE cp.async.bulk into shared memory (warp 9)
-//   * per shadow term, the TR increments  TR floats    -> one cp.async.bulk each into a ring of ST stages x TB terms (warp 8)
-// so the memory system runs ahead of the arithmetic without holding anything in registers.  Consumer warp w owns
-// items [32w, 32w+32) of the tile: lane i sums item i's terms in list order (ring slots by LDS, the few terms of
-// models without a shadow slot by a direct gather), then the warp walks its 32 rows of the U tile (increment handed
-// over by shuffle), renormalises, accumulates the int64 column sums in registers and stores column t back.
-// ---------------------------------------------------------------------------------------
-#define R1X_THREADS 320      // 8 consumer warps + ring producer warp + U producer warp
-#define R1X_ST 4
-#define R1X_TB 16
-
-template <int KC, typename T>
-__global__ void __launch_bounds__(R1X_THREADS, 1) k_pi_rank1_tma(const T* __restrict__ preds,
-                                                                 const float* __restrict__ ensb,
-                                                                 long long N, int C, int TR,
-                                                                 const long long* __restrict__ sel,
-                                                                 const int32_t* __restrict__ hdr,
-                                                                 const R1Term* __restrict__ gterms, float lr, float fxs,
-                                                                 float* __restrict__ U,
-                                                                 unsigned long long* __restrict__ pisum_fx,
-                                                                 uint32_t* __restrict__ flags) {
-  extern __shared__ __align__(128) unsigned char smem_r1x[];
-  unsigned char* smem_raw = smem_r1x;
-  const int nt = hdr[0];
-  const int t = (int)sel[1];
-  const bool ens_f32 = !std::is_same<T, float>::value && hdr[1] >= 0;      // term 0 is fp32 behind ensb (k_pi_rank1)
-  const size_t u_bytes = ((size_t)TR * C * 4 + 127) & ~(size_t)127;
-  float* Ut = reinterpret_cast<float*>(smem_raw);                                        // [TR][C]
-  float* ring = reinterpret_cast<float*>(smem_raw + u_bytes);                            // [ST][TB][TR]
-  R1Term* terms = reinterpret_cast<R1Term*>(ring + (size_t)R1X_ST * R1X_TB * TR);        // [nt]
-  long long* wacc_all = reinterpret_cast<long long*>(terms + nt);                        // [8][C]
-  int* shl = reinterpret_cast<int*>(wacc_all + (size_t)8 * C);                           // [nt] indices of the shadow terms
-  uint64_t* bars = reinterpret_cast<uint64_t*>((reinterpret_cast<uintptr_t>(shl + nt) + 7) & ~(uintptr_t)7);
-  uint64_t* fullU = bars, *emptyU = bars + 1, *full = bars + 2, *empty = bars + 2 + R1X_ST;
-  __shared__ int s_nsh;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nwarp_act = TR >> 5;                                                         // consumer warps with rows
-  for (int k = tid; k < nt; k += R1X_THREADS) terms[k] = gterms[k];
-  for (int c = tid; c < 8 * C; c += R1X_THREADS) wacc_all[c] = 0;
-  if (tid == 0) {
-    mbar_init(fullU, 1);
-    mbar_init(emptyU, nwarp_act);
-    for (int s = 0; s < R1X_ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], nwarp_act); }
-    mbar_fence_init();
-  }
-  __syncthreads();
-  if (tid == 0) {                               // shadow terms in list order (cheap: nt <= 2H)
-    int n = 0;
-    for (int k = 0; k < nt; ++k)
-      if (terms[k].str == 1) shl[n++] = k;
-    s_nsh = n;
-  }
-  __syncthreads();
-  const int nsh = s_nsh;
-  const int nch = (nsh + R1X_TB - 1) / R1X_TB;                                            // ring chunks per tile
-  const long long ntiles = (N + TR - 1) / TR;
-
-  if (warp == 8) {                              // ---- ring producer ----
-    if (lane == 0) {
-      long long gch = 0;
-      for (long long ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
-        const long long n0 = ti * TR;
-        const int rows = (int)min((long long)TR, N - n0);
-        // columns are padded to whole 16-byte units: 4 fp32 items, 8 16-bit items
-        const uint32_t rb = (uint32_t)((rows + 3) & ~3) * 4u;
-        constexpr int E16 = 16 / sizeof(T);
-        const uint32_t rbt = (uint32_t)((rows + E16 - 1) / E16 * E16) * (uint32_t)sizeof(T);
-        for (int c = 0; c < nch; ++c, ++gch) {
-          const int s = (int)(gch % R1X_ST);
-          if (gch >= R1X_ST) mbar_wait(&empty[s], (uint32_t)(((gch / R1X_ST) - 1) & 1));
-          const int cnt = min(R1X_TB, nsh - c * R1X_TB);
-          const bool e0 = ens_f32 && shl[c * R1X_TB] == 0;
-          mbar_expect_tx(&full[s], (uint32_t)cnt * rbt + (e0 ? rb - rbt : 0u));
-          for (int j = 0; j < cnt; ++j) {
-            const int k = shl[c * R1X_TB + j];
-            float* dst = ring + ((size_t)s * R1X_TB + j) * TR;
-            if (ens_f32 && k == 0) tma_load_1d(dst, ensb + terms[k].off + n0, rb, &full[s]);
-            else tma_load_1d(dst, preds + terms[k].off + n0, rbt, &full[s]);
-          }
-        }
-      }
-    }
-    return;
-  }
-  if (warp == 9) {                              // ---- U tile producer ----
-    if (lane == 0) {
-      long long it = 0;
-      for (long long ti = blockIdx.x; ti < ntiles; ti += gridDim.x, ++it) {
-        const long long n0 = ti * TR;
-        const int rows = (int)min((long long)TR, N - n0);
-        const uint32_t ub = ((uint32_t)rows * C * 4u + 15u) & ~15u;                       // U carries 16 bytes of slack
-        if (it > 0) mbar_wait(emptyU, (uint32_t)((it - 1) & 1));
-        mbar_expect_tx(fullU, ub);
-        tma_load_1d(Ut, U + (size_t)n0 * C, ub, fullU);
-      }
-    }
-    return;
-  }
-  if (warp >= nwarp_act) return;
-  // ---- consumers ----
-  long long racc[KC];
-#pragma unroll
-  for (int k = 0; k < KC; ++k) racc[k] = 0;
-  uint32_t bad = 0;
-  long long gch = 0, it = 0;
-  for (long long ti = blockIdx.x; ti < ntiles; ti += gridDim.x, ++it) {
-    const long long n0 = ti * TR;
-    const int rows = (int)min((long long)TR, N - n0);
-    const int li = warp * 32 + lane;                 // this lane's item within the tile
-    const long long n = n0 + li;
-    const bool valid = li < rows;
-    float d = 0.f;
-    int shi = 0;                                     // shadow terms consumed in this tile
-    const float* slot = ring;
-    for (int k = 0; k < nt; ++k) {
-      const R1Term tm = terms[k];
-      float v = 0.f;
-      if (tm.str == 1) {
-        const int j = shi % R1X_TB;
-        if (j == 0) {
-          const long long g = gch + shi / R1X_TB;
-          const int s = (int)(g % R1X_ST);
-          mbar_wait(&full[s], (uint32_t)((g / R1X_ST) & 1));
-          slot = ring + (size_t)s * R1X_TB * TR;
-        }
-        v = (ens_f32 && k == 0) ? slot[(size_t)j * TR + li] : slab_f(reinterpret_cast<const T*>(slot + (size_t)j * TR)[li]);
-        ++shi;
-        if (j == R1X_TB - 1 || shi == nsh) {         // last read of this stage by this warp
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty[(int)((gch + (shi - 1) / R1X_TB) % R1X_ST)]);
-        }
-      } else if (valid) {
-        v = (ens_f32 && k == 0) ? __ldg(ensb + tm.off + n * tm.str) : ldg_f(preds + tm.off + n * tm.str);
-      }
-      d = fmaf(tm.sg, v, d);
-    }
-    gch += nch;
-    const float dl = valid ? lr * d : 0.f;
-    // ---- row pass over this warp's 32 rows of the U tile ----
-    mbar_wait(fullU, (uint32_t)(it & 1));
-    const int wrows = min(32, rows - warp * 32);
-    for (int r = 0; r < wrows; r += 4) {
-      float u[4][KC], dv[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        dv[i] = __shfl_sync(CODA_FULL, dl, (r + i) & 31);
-        const float* urow = Ut + (size_t)(warp * 32 + min(r + i, wrows - 1)) * C;
-#pragma unroll
-        for (int k = 0; k < KC; ++k) {
-          const int c = lane + 32 * k;
-          u[i][k] = c < C ? urow[c] : 0.f;
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        if (r + i >= wrows) break;
-        float s = 0.f;
-#pragma unroll
-        for (int k = 0; k < KC; ++k) {
-          const int c = lane + 32 * k;
-          if (c == t) {
-            u[i][k] += dv[i];
-            U[(size_t)(n0 + warp * 32 + r + i) * C + c] = u[i][k];
-          }
-          s += u[i][k];
-        }
-        s = warp_sum(s);
-        if (!isfinite(s)) bad |= CODA_B200_FLAG_NONFINITE_PI;
-        const float den = fmaxf(s, 1e-12f);                             // coda.py:230 clamp_(min=1e-12)
-        const float rden = 1.0f / den;
-#pragma unroll
-        for (int k = 0; k < KC; ++k) racc[k] += to_fx(row_quot(u[i][k], den, rden), fxs);
-      }
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(emptyU);
-  }
-  long long* wacc = wacc_all + (size_t)warp * C;
-#pragma unroll
-  for (int k = 0; k < KC; ++k) {
-    const int c = lane + 32 * k;
-    if (c < C) wacc[c] = racc[k];
-  }
-  // consumer-only barrier (the producer warps have left): named barrier 1
-  asm volatile("bar.sync 1, %0;" ::"r"(nwarp_act * 32) : "memory");
-  for (int c = tid; c < C; c += nwarp_act * 32) {
-    long long s2 = 0;
-    for (int w = 0; w < nwarp_act; ++w) s2 += wacc_all[(size_t)w * C + c];
-    if (s2) atomicAdd(pisum_fx + c, (unsigned long long)s2);
-  }
-  if (bad) atomicOr(flags, bad);
-}
-
-static int r1x_tile_rows(int C) {     // rows per tile: U tile <= ~104 KB, multiple of 32, <= 256
-  int tr = (int)((104 * 1024) / ((size_t)C * 4)) / 32 * 32;
-  if (tr > 256) tr = 256;
-  return tr;
-}
-
 template <typename T>
 static int pi_rank1(const T* preds, const float* ensb, int H, int64_t N, int C, const int64_t* sel, double lr,
                     int fx_shift, const int32_t* terms /*[2 + 8H]*/, float* U, int64_t* pisum_fx, uint32_t* flags,
@@ -1137,62 +821,8 @@ static int pi_rank1(const T* preds, const float* ensb, int H, int64_t N, int C, 
   const int32_t* hdr = terms;                                                  // 2 ints
   const R1Term* tlist = reinterpret_cast<const R1Term*>(terms + 2);            // <= 2H x 16 bytes
   cudaStream_t st = as_stream(stream);
-  // bulk-TMA pipeline: C <= 128, 16-byte aligned U / preds / E, item counts that keep every bulk copy aligned
-  // variants (identical bits): "v1" one item per lane (default), "v4" four items per lane / 512-byte runs per term,
-  // "tma" the bulk-TMA pipeline (8 consumer warps per SM in lock-step phases).  On an H100 (400 W) at cfg3 with 140
-  // shadow models, whole-step rates of the graph loop: v1 580-620 steps/s, v1d 583-598, v4 548-563, tma 486-497; v1 at
-  // 8 CTAs per SM or one CTA per 256 items instead of 4 per SM, and a grid that leaves an eighth of the SMs to the side
-  // stream (527-530), were not better.  CODA_B200_R1 selects one for A/B runs.
-  const char* r1env = getenv("CODA_B200_R1");
-  const bool want_tma = r1env && r1env[0] == 't';
-  const bool want_v1 = !(r1env && r1env[0] == 'v' && r1env[1] == '4');
-  const bool want_deep = r1env && r1env[0] == 'v' && r1env[1] == '1' && r1env[2] == 'd';   // "v1d": 32 gathers / 8 rows in flight
-  const bool no_tma = !want_tma;
-  const int TR = C <= 128 ? r1x_tile_rows(C) : 0;
-  if (!no_tma && TR >= 32 && (reinterpret_cast<uintptr_t>(U) & 15) == 0) {
-    const size_t u_bytes = ((size_t)TR * C * 4 + 127) & ~(size_t)127;
-    const size_t smem_x = u_bytes + (size_t)R1X_ST * R1X_TB * TR * 4 + (size_t)2 * H * sizeof(R1Term) + (size_t)8 * C * 8 +
-                          (size_t)2 * H * 4 + 8 + (2 + 2 * R1X_ST) * 8;
-    if (smem_x <= 220 * 1024) {
-      long long tiles = (N + TR - 1) / TR;
-      int cap = coda_sm_count();
-      if (ctas_per_sm >= 1 && ctas_per_sm < 8) cap = cap - cap / 8;   // a concurrent stream keeps a few SMs
-      int gridx = (int)min(tiles, (long long)cap);
-#define LAUNCH_R1X(KC)                                                                                              \
-  do {                                                                                                              \
-    CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1_tma<KC, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_x)); \
-    k_pi_rank1_tma<KC, T><<<gridx, R1X_THREADS, smem_x, st>>>(preds, ensb, N, C, TR, reinterpret_cast<const long long*>(sel), \
-                                                          hdr, tlist, (float)lr, exp2f((float)fx_shift), U,        \
-                                                          reinterpret_cast<unsigned long long*>(pisum_fx), flags); \
-  } while (0)
-      if (C <= 32) LAUNCH_R1X(1);
-      else if (C <= 64) LAUNCH_R1X(2);
-      else LAUNCH_R1X(4);
-#undef LAUNCH_R1X
-      CODA_LAUNCH_OK("k_pi_rank1_tma");
-      return CODA_B200_OK;
-    }
-  }
   size_t smem = (size_t)8 * C * 8 + (size_t)2 * H * sizeof(R1Term);
   CODA_CHECK_ARG(smem <= 200 * 1024, "pi_rank1: C=%d too large", C);
-  if (!want_v1 && C <= 128) {
-    long long want4 = (N + 8 * R1V_WI - 1) / (8 * R1V_WI);
-    int cps = (ctas_per_sm < 1 || ctas_per_sm > 8) ? 8 : ctas_per_sm;
-    int grid4 = (int)min(want4, (long long)coda_sm_count() * cps);
-#define LAUNCH_R1V(KC)                                                                                            \
-  do {                                                                                                            \
-    CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1_v4<KC, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    k_pi_rank1_v4<KC, T><<<grid4, 256, smem, st>>>(preds, ensb, N, C, reinterpret_cast<const long long*>(sel), hdr,   \
-                                               tlist, (float)lr, exp2f((float)fx_shift), U,                       \
-                                               reinterpret_cast<unsigned long long*>(pisum_fx), flags);           \
-  } while (0)
-    if (C <= 32) LAUNCH_R1V(1);
-    else if (C <= 64) LAUNCH_R1V(2);
-    else LAUNCH_R1V(4);
-#undef LAUNCH_R1V
-    CODA_LAUNCH_OK("k_pi_rank1_v4");
-    return CODA_B200_OK;
-  }
   long long want = (N + R1_TN - 1) / R1_TN;
   if (ctas_per_sm < 1 || ctas_per_sm > 8) ctas_per_sm = 8;
   int grid = (int)min(want, (long long)coda_sm_count() * ctas_per_sm);
@@ -1206,8 +836,8 @@ static int pi_rank1(const T* preds, const float* ensb, int H, int64_t N, int C, 
 #define LAUNCH_R1(KC)                                                                                          \
   do {                                                                                                         \
     if (use_const) {                                                                                           \
-      CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1<T, KC, 16, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-      k_pi_rank1<T, KC, 16, 4, true><<<grid, 256, smem, st>>>(preds, ensb, N, C, reinterpret_cast<const long long*>(sel), hdr, \
+      CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1<T, KC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+      k_pi_rank1<T, KC, true><<<grid, 256, smem, st>>>(preds, ensb, N, C, reinterpret_cast<const long long*>(sel), hdr, \
                                             tlist, const_base, (float)lr, exp2f((float)fx_shift), U,           \
                                             reinterpret_cast<unsigned long long*>(pisum_fx), flags);           \
       break;                                                                                                   \
@@ -1217,14 +847,6 @@ static int pi_rank1(const T* preds, const float* ensb, int H, int64_t N, int C, 
                                             tlist, 0, (float)lr, exp2f((float)fx_shift), U,                    \
                                             reinterpret_cast<unsigned long long*>(pisum_fx), flags);           \
   } while (0)
-  if (want_deep && C > 64 && C <= 128) {
-    CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_rank1<T, 4, 32, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_pi_rank1<T, 4, 32, 8><<<grid, 256, smem, st>>>(preds, ensb, N, C, reinterpret_cast<const long long*>(sel), hdr, tlist, 0,
-                                                  (float)lr, exp2f((float)fx_shift), U,
-                                                  reinterpret_cast<unsigned long long*>(pisum_fx), flags);
-    CODA_LAUNCH_OK("k_pi_rank1<deep>");
-    return CODA_B200_OK;
-  }
   if (C <= 32) LAUNCH_R1(1);
   else if (C <= 64) LAUNCH_R1(2);
   else if (C <= 128) LAUNCH_R1(4);

@@ -17,7 +17,7 @@ One acquisition step on the device (host-free loop, ``run_steps``; everything be
     ---- fork ----  side stream: beta_tables(class t) -> pair_rows(class t)        main: pi_rank1 (marginal refresh)
     step_mixture  exchange the marginal sums, pi_hat, P(best), H_before, argmax         (needs PB[t] from the side)
     ---- join ----
-    template_gains + gain_eig   the scoring pass for the NEXT selection -> block records
+    row_gains + gain_eig        the scoring pass for the NEXT selection -> block records
 """
 from __future__ import annotations
 
@@ -494,9 +494,6 @@ class Engine:
             self._call("coda_b200_ell_build", _ptr(self.ent_off), _ptr(self.ent_row), _ptr(self.ent_cls), N, self.ell_k,
                        _ptr(self.ell_row), _ptr(self.ell_cls), s)
         self.gain = self._z((self.npairs,), torch.float32)      # information gain of every row (templates first)
-        # CODA_B200_FUSED_SCORE=1: one kernel computes the row gains and assembles the per-item EIG (measured slower
-        # than the streaming row-gain kernel followed by the 8-lane assembly)
-        self.fused_score = os.environ.get("CODA_B200_FUSED_SCORE", "0") == "1"
         self.ph_cache = None
         if self.mode == "incremental":
             need = self.npairs * self.Hp * 4
@@ -607,22 +604,18 @@ class Engine:
             if self.pending:
                 self._cur().wait_event(self.ev_join)            # the class-t rows of the side stream
                 self.pending = False
-            if self.fused_score:
-                self._call("coda_b200_template_gains", _ptr(self.ph_cache), self.H, self.C, _ptr(self.PB), _ptr(self.m0),
-                           _ptr(self.pi_hat), _ptr(self.gain), self._s())
-            else:                                               # template rows + heavy rows in one stream
-                self._call("coda_b200_row_gains", _ptr(self.ph_cache), _ptr(self.row_cls), self.n_heavy, self.H, self.C,
-                           _ptr(self.PB), _ptr(self.m0), _ptr(self.pi_hat), _ptr(self.gain), self._s())
+            # template rows + heavy rows in one stream
+            self._call("coda_b200_row_gains", _ptr(self.ph_cache), _ptr(self.row_cls), self.n_heavy, self.H, self.C,
+                       _ptr(self.PB), _ptr(self.m0), _ptr(self.pi_hat), _ptr(self.gain), self._s())
         else:
             if self.pending:
                 self._cur().wait_event(self.ev_join)
                 self.pending = False
             self._pair_rows(0, self.ntiles)
-        self._call("coda_b200_gain_eig", _ptr(self.U), self.N, self.C, self.H, _ptr(self.ent_off), _ptr(self.heavy_off),
-                   _ptr(self.ent_row), _ptr(self.ent_cls), _ptr(self.ph_cache) if self.fused_score else None,
-                   _ptr(self.gain), _ptr(self.PB), _ptr(self.m0), _ptr(self.pi_hat), _ptr(self.labeled),
-                   _ptr(self.disagree), self.n_offset, self.max_entries, _ptr(self.ell_row), _ptr(self.ell_cls),
-                   self.ell_k, _ptr(self.eig), _ptr(self.partials), _ptr(self.flags), self._s())
+        self._call("coda_b200_gain_eig", _ptr(self.U), self.N, self.C, self.H, _ptr(self.ent_off), _ptr(self.ent_row),
+                   _ptr(self.ent_cls), _ptr(self.gain), _ptr(self.labeled), _ptr(self.disagree), self.n_offset,
+                   self.max_entries, _ptr(self.ell_row), _ptr(self.ell_cls), self.ell_k, _ptr(self.eig),
+                   _ptr(self.partials), _ptr(self.flags), self._s())
         self.scored = True
 
     def _post_label(self):

@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define CODA_B200_VERSION 202
+#define CODA_B200_VERSION 203
 #define CODA_B200_NODES 256 /* quadrature nodes, coda/coda.py:79 */
 #define CODA_B200_MAX_WORLD 16
 #define CODA_B200_REC_WORDS 8 /* arg-max record: {bits vA, iA, cntA, bits vB, iB, bits v2A, bits v2B, 0} */
@@ -266,30 +266,24 @@ int coda_b200_pair_rows_tc(const int32_t* tiles128, int tile_lo, int tile_hi, co
                            const int32_t* row_of, const void* dLb, const void* Gb, const float* PB, const float* m0,
                            const float* pi_hat, int H, float* ph_cache, float* gain, const int64_t* sel,
                            const int64_t* tile_off, uint32_t* flags, coda_stream_t stream);
-/* gain[r] (coda.py:274-276) of the T = C*(1+H) template rows from their cached P(best | hypothetical) rows. */
-int coda_b200_template_gains(const float* ph_cache, int H, int C, const float* PB, const float* m0,
-                             const float* pi_hat, float* gain /*[T]*/, coda_stream_t stream);
 
 /* ---- the per-step scoring pass (eig_batched coda.py:253-278 + _prefilter coda.py:215-219 + the arg-max of
  *      get_next_item_to_label coda.py:306/309), one kernel, item-major ---------------------------------
- * For every item: information gain of each of its heavy rows straight from the cached row (ph_cache != NULL) or
- * from gain[row] (ph_cache == NULL: the row kernels just wrote it), template gains from gain[0..T), then
- * eig[n] = sum_c pi_hat_xi[n][c] * gain(n, c)  (== H_before - sum_c xi * H_after because sum_c xi = 1), the
- * candidate arg-max (first index wins) and runner-up value per block -> partials [blocks][REC_WORDS]. */
+ * For every item: the information gain of each of its rows from gain[row] (row_gains or pair_rows wrote it; template
+ * rows in gain[0..T)), then eig[n] = sum_c pi_hat_xi[n][c] * gain(n, c)  (== H_before - sum_c xi * H_after because
+ * sum_c xi = 1), the candidate arg-max (first index wins) and runner-up value per block -> partials [blocks][REC_WORDS]. */
 int coda_b200_eig_blocks(int64_t N, int H, int C); /* number of partial records gain_eig writes */
 /* max_entries: the longest entry list (or -1 if unknown); short lists and C <= 128 take an 8-lanes-per-item kernel,
  * which reads the lists from the optional ELL copy (coda_b200_ell_build; ell_k = padded list length <= 32). */
-int coda_b200_gain_eig(const float* U, int64_t N, int C, int H, const int32_t* ent_off, const int32_t* heavy_off,
-                       const int32_t* ent_row, const uint16_t* ent_cls, const float* ph_cache, const float* gain,
-                       const float* PB, const float* m0, const float* pi_hat, const uint8_t* labeled,
-                       const uint8_t* disagree, int64_t n_offset, int max_entries, const int32_t* ell_row,
-                       const uint16_t* ell_cls, int ell_k, float* eig, int64_t* partials, uint32_t* flags,
-                       coda_stream_t stream);
+int coda_b200_gain_eig(const float* U, int64_t N, int C, int H, const int32_t* ent_off, const int32_t* ent_row,
+                       const uint16_t* ent_cls, const float* gain, const uint8_t* labeled, const uint8_t* disagree,
+                       int64_t n_offset, int max_entries, const int32_t* ell_row, const uint16_t* ell_cls, int ell_k,
+                       float* eig, int64_t* partials, uint32_t* flags, coda_stream_t stream);
 int coda_b200_ell_build(const int32_t* ent_off, const int32_t* ent_row, const uint16_t* ent_cls, int64_t N, int K,
                         int32_t* ell_row /*[N][K], -1 = empty*/, uint16_t* ell_cls /*[N][K]*/, coda_stream_t stream);
 /* gain[r] (coda.py:274-276) of ALL T + n_heavy rows from their cached rows -- the template rows (class = r / (1+H))
  * and the heavy rows (class = row_cls[r - T]) in one stream: the HBM-bound kernel of the two-kernel scoring pass
- * (row_gains, then gain_eig with ph_cache == NULL).  Item-major heavy rows make the per-item gains contiguous for the
+ * (row_gains, then gain_eig).  Item-major heavy rows make the per-item gains contiguous for the
  * assembly that follows. */
 int coda_b200_row_gains(const float* ph_cache, const uint16_t* row_cls, int64_t n_heavy, int H, int C,
                         const float* PB, const float* m0, const float* pi_hat, float* gain, coda_stream_t stream);
@@ -379,41 +373,31 @@ int coda_b200_static_scores(const uint16_t* hard, const float* ens, int H, int64
                             float* vma_score, coda_stream_t stream);
 /* number of partial records of the selection calls below (per-block chunks of the item axis) */
 int coda_b200_select_blocks(int64_t N);
-/* random.choices(d_u_idxs, weights) (activetesting.py:45-48, vma.py:44-60).  weighted_total: total[0] = fp64 sum of w
- * over the unlabeled items, total[1] = their count.  weighted_draw: the weights w / (float)total[0] (fp32 division,
- * the normalisation of activetesting.py:44), their running fp64 sum cum in index order, and the first unlabeled item
- * with cum > u * cum_total (bisect_right, the last one if none) -> out = {position among the unlabeled items, item,
- * float bits of its normalised weight}.  u = random.random() drawn by the caller.  partials: 2 * select_blocks doubles. */
-int coda_b200_weighted_total(const float* w, const uint8_t* labeled, int64_t N, double* partials, double* total /*[2]*/,
-                             coda_stream_t stream);
-int coda_b200_weighted_draw(const float* w, const uint8_t* labeled, int64_t N, const double* total, double u,
-                            double* partials, int64_t* out /*[3]*/, coda_stream_t stream);
-/* Minimum (want_max = 0, modelpicker.py:68-69) or maximum (uncertainty.py:37-38) of v over the unlabeled items and the
- * number of items exactly equal to it: out = {float bits, count}; partials: 2 * select_blocks int64.  select_kth: the
- * k-th (ascending index, from 0) unlabeled item equal to best[0] (modelpicker.py:70, uncertainty.py:39-43), from the
- * partials of the select_extreme call that produced `best`; -1 if there is none. */
-int coda_b200_select_extreme(const float* v, const uint8_t* labeled, int64_t N, int want_max, int64_t* partials,
-                             int64_t* out /*[2]*/, coda_stream_t stream);
-int coda_b200_select_kth(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
-                         const int64_t* best, int64_t k, int64_t* out_idx /*[1]*/, coda_stream_t stream);
-
-/* N-range shards of the same selection calls (one shard per GPU or several per GPU, each with its own stream).  Every
- * shard makes the same calls in the same order; each call ends in ONE single-CTA kernel that stores this shard's record
- * into every peer's mailbox (record channel of a box sized by coda_b200_xchg_box_bytes(world, H, C, ...)), waits for
- * all of them (2 s bound, then CODA_B200_FLAG_XCHG_TIMEOUT in `flags`) and merges them in rank order, so every shard
- * holds the same global answer.  Vectors, `labeled` and `partials` are this shard's; item indices in the outputs are
- * global (n_offset + local).  x == NULL or world 1: no mailbox is touched and each call returns what its single-shard
- * counterpart returns (out[2] = 0 and out[3] = the count for select_extreme_xchg; owner_share copies src to dst).
- *   select_extreme_xchg: out = {float bits of the global extreme, global count of items equal to it, how many of them
- *     lie on lower ranks, how many on this rank} -- the same {value, count} as one shard (vc_merge is exact);
- *   select_kth_xchg: best = that out; the shard whose ties cover k picks its (k - lower)-th, out_idx = global item;
- *   weighted_total_xchg: total = {sum over the shards in rank order of each shard's fp64 sum, unlabeled count};
- *   weighted_draw_xchg: the shards' sums of w / (float)total[0] are exchanged; every shard forms the grand total in
- *     rank order, target = u * grand and the owner shard, which draws inside its chunks starting from the lower ranks'
- *     running sum and position; out = {global position among the unlabeled items, global item, q bits}.  A shard's
- *     selection blocks and per-thread runs restart at its first item, so the fp64 partial sums group the items
- *     differently from one shard: a pick can differ from one shard only when u * total lies within ~1e-16 relative of a
- *     cumulative boundary. */
+/* Selection over the unlabeled items of N-range shards (one shard, or several per GPU or one per GPU, each with its own
+ * stream).  Every shard makes the same calls in the same order; each call ends in ONE single-CTA kernel that stores this
+ * shard's record into every peer's mailbox (record channel of a box sized by coda_b200_xchg_box_bytes(world, H, C, ...)),
+ * waits for all of them (2 s bound, then CODA_B200_FLAG_XCHG_TIMEOUT in `flags`) and merges them in rank order, so every
+ * shard holds the same global answer.  Vectors, `labeled` and `partials` are this shard's (partials: 2 * select_blocks
+ * words); item indices in the outputs are global (n_offset + local).  x == NULL or world 1: one shard, no mailbox is
+ * touched and `flags` is never set.
+ *   select_extreme_xchg: minimum (want_max = 0, modelpicker.py:68-69) or maximum (uncertainty.py:37-38) of v over the
+ *     unlabeled items and the number of items exactly equal to it: out = {float bits of the global extreme, global count
+ *     of items equal to it, how many of them lie on lower ranks, how many on this rank} (vc_merge is exact, so the
+ *     {value, count} does not depend on the shard count);
+ *   select_kth_xchg: the k-th (ascending global index, from 0) unlabeled item equal to best[0] (modelpicker.py:70,
+ *     uncertainty.py:39-43), from the partials of the select_extreme_xchg call that produced best = its out; the shard
+ *     whose ties cover k picks its (k - lower)-th; out_idx = global item, -1 if there is none;
+ *   random.choices(d_u_idxs, weights) (activetesting.py:45-48, vma.py:44-60), u = random.random() drawn by the caller:
+ *   weighted_total_xchg: total = {sum over the shards in rank order of each shard's fp64 sum of w over its unlabeled
+ *     items, unlabeled count};
+ *   weighted_draw_xchg: the weights w / (float)total[0] (fp32 division, the normalisation of activetesting.py:44) and
+ *     their running fp64 sum cum in index order; the first unlabeled item with cum > u * cum_total (bisect_right, the
+ *     last one if none) -> out = {global position among the unlabeled items, global item, float bits of its normalised
+ *     weight}.  The shards' sums are exchanged; every shard forms the grand total in rank order, target = u * grand
+ *     and the owner shard, which draws inside its chunks starting from the lower ranks' running sum and position.  A
+ *     shard's selection blocks and per-thread runs restart at its first item, so the fp64 partial sums group the items
+ *     differently from one shard: a pick can differ from one shard only when u * total lies within ~1e-16 relative of
+ *     a cumulative boundary. */
 int coda_b200_select_extreme_xchg(const float* v, const uint8_t* labeled, int64_t N, int want_max, int64_t* partials,
                                   int64_t* out /*[4]*/, const coda_xchg_t* x, uint32_t* flags, coda_stream_t stream);
 int coda_b200_select_kth_xchg(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
@@ -426,7 +410,7 @@ int coda_b200_weighted_draw_xchg(const float* w, const uint8_t* labeled, int64_t
                                  uint32_t* flags, coda_stream_t stream);
 /* add_label on shards: the shard that holds the labeled item (own = 1; exactly one) sends `bytes` from src -- its hard
  * row, or the per-model losses of its (H, C) column -- and every shard receives them in dst.  bytes + 16 must fit the
- * record slot (2 * H * 2 + 64 bytes: an H-float vector does). */
+ * record slot (2 * H * 2 + 64 bytes: an H-float vector does).  x == NULL or world 1: src is copied to dst. */
 int coda_b200_owner_share(const void* src, int bytes, int own, void* dst, const coda_xchg_t* x, uint32_t* flags,
                           coda_stream_t stream);
 

@@ -87,7 +87,7 @@ def test_grouped_vma_sum_equals_the_pairwise_sum():
 
 
 def draw_model(weights, labeled, u, chunk=4096, ipt=16):
-    """k_wsum_blocks + k_wdraw_pick: fp64 sums per thread run, per block, then the first item with cum > u * total."""
+    """k_wsum_blocks + k_wdraw_xchg on one shard: fp64 sums per thread run, per block, then the first item with cum > u * total."""
     n = len(weights)
     items = [i for i in range(n) if not labeled[i]]
     blocks = []

@@ -436,53 +436,76 @@ def test_sharding_arguments_are_rejected_under_one_process_per_gpu():
         IID(TensorDataset(p.cuda(), l.cuda()), None, shards=2, comm=_FakeComm([(0, 50, 50), (50, 50, 100)]))
 
 
+def _dyadic_weights(g, labeled):
+    """Small integer weights whose sum over the unlabeled items is a power of two P: every w / P is exact in fp32 and
+    every running sum of them is exact in fp64, so a draw has one right answer whatever the summation order."""
+    w = torch.randint(0, 4, labeled.shape, generator=g).double()
+    unl = torch.nonzero(labeled == 0).flatten()
+    if len(unl):
+        s = int(w[unl].sum())
+        p = 1 << max(0, (s - 1).bit_length())
+        d = p - s
+        w[unl] += d // len(unl)
+        w[unl[torch.randperm(len(unl), generator=g)[:d % len(unl)]]] += 1
+        assert int(w[unl].sum()) == p
+    return w.float()
+
+
 @pytest.mark.gpu
-def test_exchange_entry_points_without_peers_equal_the_single_shard_ones():
-    """Each *_xchg entry point with x == NULL (world 1) returns what its single-shard counterpart returns."""
+def test_exchange_entry_points_without_peers_match_a_host_evaluation():
+    """Each selection entry point with x == NULL (world 1) against an evaluation on the host: the extreme and its ties,
+    the k-th tie, the weighted total and the weighted draw.  With one shard no exchange waits, so no flag is set."""
     from coda_b200 import _native as nat
     lib = nat.load()
     dev = torch.device("cuda:0")
     g = torch.Generator().manual_seed(9)
     for N in (1, 37, 4096, 70_001):
-        v = torch.randint(0, 6, (N,), generator=g).float().to(dev)         # many exact ties
-        w = torch.rand(N, generator=g).to(dev)
-        labeled = (torch.rand(N, generator=g) < 0.3).to(torch.uint8).to(dev)
+        v = torch.randint(0, 6, (N,), generator=g).float()                # many exact ties
+        labeled = (torch.rand(N, generator=g) < 0.3).to(torch.uint8)
+        w = _dyadic_weights(g, labeled)
+        unl = labeled == 0
         nb = int(lib.coda_b200_select_blocks(N))
-        pi = [torch.empty(2 * nb, dtype=torch.int64, device=dev) for _ in range(2)]
-        pf = [torch.empty(2 * nb, dtype=torch.float64, device=dev) for _ in range(2)]
+        pi = torch.empty(2 * nb, dtype=torch.int64, device=dev)
+        pf = torch.empty(2 * nb, dtype=torch.float64, device=dev)
         flags = torch.zeros(1, dtype=torch.int32, device=dev)
         s = torch.cuda.current_stream(dev).cuda_stream
+        vd, wd, ld = v.to(dev), w.to(dev), labeled.to(dev)
         for want_max in (0, 1):
-            best = torch.empty(2, dtype=torch.int64, device=dev)
             bx = torch.full((4,), -7, dtype=torch.int64, device=dev)
-            nat.call("coda_b200_select_extreme", v.data_ptr(), labeled.data_ptr(), N, want_max, pi[0].data_ptr(),
-                     best.data_ptr(), s)
-            nat.call("coda_b200_select_extreme_xchg", v.data_ptr(), labeled.data_ptr(), N, want_max, pi[1].data_ptr(),
+            nat.call("coda_b200_select_extreme_xchg", vd.data_ptr(), ld.data_ptr(), N, want_max, pi.data_ptr(),
                      bx.data_ptr(), None, flags.data_ptr(), s)
-            b, bxl = best.tolist(), bx.tolist()
-            assert bxl == [b[0], b[1], 0, b[1]]
-            for k in sorted({0, b[1] // 2, max(0, b[1] - 1)}):
-                o1 = torch.empty(1, dtype=torch.int64, device=dev)
-                o2 = torch.full((1,), -7, dtype=torch.int64, device=dev)
-                nat.call("coda_b200_select_kth", v.data_ptr(), labeled.data_ptr(), N, pi[0].data_ptr(),
-                         best.data_ptr(), k, o1.data_ptr(), s)
-                nat.call("coda_b200_select_kth_xchg", v.data_ptr(), labeled.data_ptr(), N, pi[1].data_ptr(),
-                         bx.data_ptr(), k, 0, o2.data_ptr(), None, flags.data_ptr(), s)
-                assert o1.tolist() == o2.tolist()
-        t1 = torch.empty(2, dtype=torch.float64, device=dev)
-        t2 = torch.empty(2, dtype=torch.float64, device=dev)
-        nat.call("coda_b200_weighted_total", w.data_ptr(), labeled.data_ptr(), N, pf[0].data_ptr(), t1.data_ptr(), s)
-        nat.call("coda_b200_weighted_total_xchg", w.data_ptr(), labeled.data_ptr(), N, pf[1].data_ptr(), t2.data_ptr(),
-                 None, flags.data_ptr(), s)
-        assert t1.tolist() == t2.tolist()
+            ties = torch.empty(0, dtype=torch.int64)
+            bits, cnt = 0, 0
+            if unl.any():
+                best = v[unl].max() if want_max else v[unl].min()
+                ties = torch.nonzero(unl & (v == best)).flatten()
+                bits, cnt = int(np.float32(best.item()).view(np.uint32)), len(ties)
+            assert bx.tolist() == [bits, cnt, 0, cnt], (N, want_max)
+            for k in sorted({0, cnt // 2, max(0, cnt - 1)}):
+                o = torch.full((1,), -7, dtype=torch.int64, device=dev)
+                nat.call("coda_b200_select_kth_xchg", vd.data_ptr(), ld.data_ptr(), N, pi.data_ptr(), bx.data_ptr(), k, 0,
+                         o.data_ptr(), None, flags.data_ptr(), s)
+                assert o.tolist() == [int(ties[k]) if k < cnt else -1], (N, want_max, k)
+        t = torch.empty(2, dtype=torch.float64, device=dev)
+        nat.call("coda_b200_weighted_total_xchg", wd.data_ptr(), ld.data_ptr(), N, pf.data_ptr(), t.data_ptr(), None,
+                 flags.data_ptr(), s)
+        total = float(w[unl].double().sum())
+        assert t.tolist() == [total, float(unl.sum())], N
+        q = (w / np.float32(total)) if total else w                       # exact: total is a power of two
+        items = torch.nonzero(unl).flatten()
+        cum = torch.cumsum(q[items].double(), 0)
         for u in (0.0, 0.25, 0.5, 0.999999):
-            o1 = torch.empty(3, dtype=torch.int64, device=dev)
-            o2 = torch.full((3,), -7, dtype=torch.int64, device=dev)
-            nat.call("coda_b200_weighted_draw", w.data_ptr(), labeled.data_ptr(), N, t1.data_ptr(), u, pf[0].data_ptr(),
-                     o1.data_ptr(), s)
-            nat.call("coda_b200_weighted_draw_xchg", w.data_ptr(), labeled.data_ptr(), N, t1.data_ptr(), u, 0,
-                     pf[1].data_ptr(), o2.data_ptr(), None, flags.data_ptr(), s)
-            assert o1.tolist() == o2.tolist(), (N, u)
+            o = torch.full((3,), -7, dtype=torch.int64, device=dev)
+            nat.call("coda_b200_weighted_draw_xchg", wd.data_ptr(), ld.data_ptr(), N, t.data_ptr(), u, 0, pf.data_ptr(),
+                     o.data_ptr(), None, flags.data_ptr(), s)
+            if not len(items):
+                want = [-1, -1, 0]
+            else:
+                past = torch.nonzero(cum > u * float(cum[-1])).flatten()       # bisect_right, the last item if none
+                pos = int(past[0]) if len(past) else len(items) - 1
+                i = int(items[pos])
+                want = [pos, i, int(np.float32(q[i].item()).view(np.uint32))]
+            assert o.tolist() == want, (N, u)
         src = torch.arange(13, dtype=torch.int16, device=dev)
         dst = torch.zeros(13, dtype=torch.int16, device=dev)
         nat.call("coda_b200_owner_share", src.data_ptr(), 26, 1, dst.data_ptr(), None, flags.data_ptr(), s)

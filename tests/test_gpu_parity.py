@@ -628,31 +628,38 @@ def test_best_model_prediction_is_a_fresh_tensor():
 
 @pytest.mark.parametrize("shape", [(64, 20000, 20, 5), (37, 3001, 7, 11), (256, 6000, 100, 3), (12, 333, 33, 4)])
 def test_marginal_refresh_variants_carry_identical_bits(shape, monkeypatch):
-    """The three kernels of the rank-1 marginal refresh (four items per lane -- the default --, the bulk-TMA pipeline,
-    one item per lane) do the same arithmetic in the same order: U, the fixed-point column sums and pi_hat carry
-    identical bits after every label, for item counts / class counts that are not multiples of the tile or of four,
-    with and without shadow slots."""
+    """The two term paths of the rank-1 marginal refresh (the gather list in a constant-bank slot -- the default --, or
+    in shared memory, which a selector gets once its device's slots are used up; CODA_B200_R1_CONST=0 at construction)
+    do the same arithmetic in the same order: U, the fixed-point column sums and pi_hat carry identical bits after every
+    label, for item counts / class counts that are not multiples of the tile or of four, with and without shadow slots."""
+    import gc
     from coda_b200.synth import synth
     H, N, C, seed = shape
     preds, labels = synth(H, N, C, seed=seed)
+    monkeypatch.setenv("CODA_B200_GRAPH", "0")
     for shadow_models in (None, "3"):
         if shadow_models:
             monkeypatch.setenv("CODA_B200_SHADOW_MODELS", shadow_models)
         else:
             monkeypatch.delenv("CODA_B200_SHADOW_MODELS", raising=False)
-        monkeypatch.setenv("CODA_B200_GRAPH", "0")           # the variant is chosen per launch: keep launches eager
-        sels = {v: _mk(preds, labels) for v in ("v4", "tma", "v1")}
+        gc.collect()                                          # selectors of earlier tests give their slots back
+        monkeypatch.delenv("CODA_B200_R1_CONST", raising=False)
+        sels = {"const": _mk(preds, labels)}
+        monkeypatch.setenv("CODA_B200_R1_CONST", "0")
+        sels["smem"] = _mk(preds, labels)
+        monkeypatch.delenv("CODA_B200_R1_CONST")
+        assert sels["const"].engine.const_slot >= 0 and sels["smem"].engine.const_slot == -1
         for k, i in enumerate([3, N // 2, N - 1, 17, N // 3]):
-            for v, s in sels.items():
-                monkeypatch.setenv("CODA_B200_R1", v)
+            for s in sels.values():
                 s.add_label(i, int(labels[i]), 0.0)
                 torch.cuda.synchronize()
-            for v in ("tma", "v1"):
-                assert torch.equal(sels["v4"].engine.U, sels[v].engine.U), (shape, shadow_models, k, v)
-                assert torch.equal(sels["v4"].engine.pisum, sels[v].engine.pisum) and torch.equal(sels["v4"].pi_hat, sels[v].pi_hat)
-        monkeypatch.delenv("CODA_B200_R1")
+            assert torch.equal(sels["const"].engine.U, sels["smem"].engine.U), (shape, shadow_models, k)
+            assert torch.equal(sels["const"].engine.pisum, sels["smem"].engine.pisum)
+            assert torch.equal(sels["const"].pi_hat, sels["smem"].pi_hat)
         picks = {v: s.get_next_item_to_label() for v, s in sels.items()}
-        assert picks["v4"] == picks["tma"] == picks["v1"]
+        assert picks["const"] == picks["smem"]
+        for s in sels.values():
+            s.close()
 
 
 @pytest.mark.parametrize("shape", [(256, 1000, 100, 1.0), (5, 128, 16, 1.0), (9, 700, 128, 1.0), (30, 257, 20, 3e5),

@@ -20,9 +20,9 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/coda_b200.h but not exported"
     assert declared == set(nat.SIGNATURES), declared ^ set(nat.SIGNATURES)
-    assert lib.coda_b200_version() == nat.VERSION == 202
+    assert lib.coda_b200_version() == nat.VERSION == 203
     raw = ctypes.CDLL(nat.lib_path())
-    assert raw.coda_b200_version() == 202
+    assert raw.coda_b200_version() == 203
 
 
 def test_no_gpu_means_loud_failure():

@@ -191,11 +191,11 @@ def test_coda_identical_on_16bit_slab(dt, shape, shards, monkeypatch):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("dt", DTYPES)
-@pytest.mark.parametrize("env", [{"CODA_B200_R1": "v4"}, {"CODA_B200_R1": "tma"}, {"CODA_B200_R1_CONST": "0"},
-                                 {"CODA_B200_SHADOW": "0"}, {"CODA_B200_SHADOW_MODELS": "3"}, {"CODA_B200_TC": "0"},
-                                 {"CODA_B200_ENS": "0"}, {"CODA_B200_PI_FULL": "simt"}])
+@pytest.mark.parametrize("env", [{"CODA_B200_R1_CONST": "0"}, {"CODA_B200_SHADOW": "0"},
+                                 {"CODA_B200_SHADOW_MODELS": "3"}, {"CODA_B200_TC": "0"}, {"CODA_B200_ENS": "0"},
+                                 {"CODA_B200_PI_FULL": "simt"}])
 def test_coda_identical_across_kernel_paths(dt, env, monkeypatch):
-    """Each rank-1 refresh kernel and term path (constant bank / shared memory), the shadow off, capped and full."""
+    """Each rank-1 refresh term path (constant bank / shared memory), the shadow off, capped and full."""
     monkeypatch.setenv("CODA_B200_GRAPH", "0")
     for k, v in env.items():
         monkeypatch.setenv(k, v)

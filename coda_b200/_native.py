@@ -69,7 +69,20 @@ class StepStruct(C.Structure):
     ]
 
 
-PX, PS = C.POINTER(XchgStruct), C.POINTER(StepStruct)
+class BlLoopStruct(C.Structure):
+    """coda_bl_loop_t (include/coda_b200.h): one shard of a competing selector's device loop."""
+    _fields_ = [
+        ("method", i32), ("H", i32), ("N", i64), ("n_offset", i64), ("n_global", i64),
+        ("hard", p), ("disagree", p), ("labeled", p), ("labels", p), ("pre", p), ("ls", p), ("best", p), ("pick", p),
+        ("total", p), ("counts", p), ("s1", p), ("s2", p), ("post", p), ("gamma", f32), ("hist_cap", i64),
+        ("hist_idx", p), ("hist_q", p), ("hist_tie", p), ("hist_best", p), ("hist_best_tie", p), ("hist_loss", p),
+        ("flags", p),
+    ]
+
+
+BL_IID, BL_UNCERTAINTY, BL_ACTIVETESTING, BL_VMA, BL_MODELPICKER = 0, 1, 2, 3, 4
+
+PX, PS, PL = C.POINTER(XchgStruct), C.POINTER(StepStruct), C.POINTER(BlLoopStruct)
 
 # name -> (restype, argtypes); mirrors include/coda_b200.h one to one
 SIGNATURES = {
@@ -125,6 +138,7 @@ SIGNATURES = {
     "coda_b200_step_merge": (i32, [PS, PX, p]),
     "coda_b200_step_label": (i32, [PS, PX, p]),
     "coda_b200_step_mixture": (i32, [PS, PX, p]),
+    "coda_b200_record_best": (i32, [p, p, p, i64, p]),
     "coda_b200_ties": (i32, [p, i64, p, p, i64, p, i32, p, p, p, p]),
     "coda_b200_report_gather": (i32, [p, i32, p, PX, p, p]),
     "coda_b200_mp_entropy": (i32, [p, p, i32, i64, i32, f64, p, p, i32, p, p]),
@@ -135,6 +149,11 @@ SIGNATURES = {
     "coda_b200_weighted_total_xchg": (i32, [p, p, i64, p, p, PX, p, p]),
     "coda_b200_weighted_draw_xchg": (i32, [p, p, i64, p, f64, i64, p, p, PX, p, p]),
     "coda_b200_owner_share": (i32, [p, i32, i32, p, PX, p, p]),
+    "coda_b200_select_kth_xchg_dev": (i32, [p, p, i64, p, p, p, p, i64, p, PX, p, p]),
+    "coda_b200_weighted_draw_xchg_dev": (i32, [p, p, i64, p, p, p, i64, p, p, PX, p, p]),
+    "coda_b200_mp_entropy_dev": (i32, [p, p, i32, i64, i32, f64, p, p, p, p, p]),
+    "coda_b200_bl_draw": (i32, [PL, p]),
+    "coda_b200_bl_step": (i32, [PL, PX, p]),
 }
 
 

@@ -16,11 +16,20 @@ with world > 1 the dataset is this rank's N-range and every rank makes the same 
 is no size-based rule.  Each selection call ends in one exchange kernel per shard (``*_xchg`` entry points) that
 leaves the same global answer on every shard; ``add_label`` ships the owner's hard row or losses the same way.  The
 host bookkeeping (``d_u_idxs``, risks, the posterior, RNG draws) is global and replicated.
+
+Host-free loop: ``run_steps(k, labels, seed=...)`` runs ``k`` steps of main.py:91-94 (select, oracle, add_label,
+best model) as one CUDA-graph replay per step and shard, with one host sync at the end; ``history()`` /
+``best_history()`` read back the picks and per-step best models and bring the host-side state up to date, so API calls
+and device loops can follow each other.  Draws whose consumption is known up front (IID's ``random.choice``, the
+``random.random()`` of ActiveTesting and VMA) are made on the host before the loop with the API's own calls; tie
+breaks are drawn on the device from a Philox4x32-10 stream (``include/coda_b200.h``, DESIGN.md §5b).
 """
 from __future__ import annotations
 
 import bisect
 import contextlib
+import ctypes
+import functools
 import os
 import random
 
@@ -50,6 +59,37 @@ def _f32(bits):
     return float(np.array([bits], dtype=np.int64).astype(np.uint32).view(np.float32)[0])
 
 
+HIST_CAP = 1 << 16          # device-loop history ring (slot = device-loop step % HIST_CAP), as CODA's
+_LS_WORDS = 16              # loop words of coda_bl_loop_t (include/coda_b200.h)
+
+
+def predraw(kind, k, n0):
+    """The Python ``random`` draws of ``k`` steps, made with the calls the API path makes, in step order:
+    ``kind = "choice"`` (IID, ``n0`` unlabeled items before the first step): ``random.choice(range(n0 - s))``;
+    ``"random"`` (ActiveTesting, VMA): ``random.random()``; ``None``: nothing."""
+    if kind == "choice":
+        return [float(random.choice(range(n0 - s))) for s in range(k)]
+    if kind == "random":
+        return [random.random() for _ in range(k)]
+    return []
+
+
+def rewind(state, kind, j, n0):
+    """Python ``random`` as after the first ``j`` steps' draws from ``state`` (the state before ``predraw``)."""
+    random.setstate(state)
+    predraw(kind, j, n0)
+
+
+def _synced(fn):
+    """API calls after a device loop first bring the host-side state up to date (``history()``)."""
+    @functools.wraps(fn)
+    def call(self, *args, **kwargs):
+        if self._loop_dirty:
+            self.history()
+        return fn(self, *args, **kwargs)
+    return call
+
+
 class _UnlabeledItems(_Unlabeled):
     """``d_u_idxs``: the unlabeled items in ascending order, list-like, with O(labels) positional access."""
 
@@ -73,6 +113,14 @@ class _UnlabeledItems(_Unlabeled):
                 break
             k += 1
         return k
+
+    def remove_marked(self, idx):
+        """remove() of an item the device has already marked labeled."""
+        idx = int(idx)
+        if idx not in self:
+            raise ValueError("list.remove(x): x not in list")
+        self._removed.add(idx)
+        bisect.insort(self._sorted, idx)
 
     def index(self, idx):
         if idx not in self:
@@ -222,6 +270,110 @@ class _DeviceState:
             self._call("coda_b200_owner_share", _ptr(src) if own else None, dst.numel() * dst.element_size(),
                        int(own), _ptr(dst), self._x(), _ptr(self.flags), self._s())
 
+    # -- the device loop (coda_b200_bl_* entry points) ------------------------------------------------------------
+    def loop_alloc(self, method, n_global, gamma):
+        """Loop words, per-method sums and history rings of this shard (once per selector)."""
+        H = self.H
+        with self._on():
+            if getattr(self, "hard", None) is None:          # IID, Uncertainty, AT and VMA dropped their scan
+                self.hard, self.disagree, _ = self.scan(ens=False)
+            z = lambda *shape, dt: torch.zeros(shape, dtype=dt, device=self.dev)
+            self.ls = z(_LS_WORDS, dt=torch.int64)
+            self.pre = z(1, dt=torch.float64)
+            self.counts = z(H, dt=torch.int32)
+            lure = method in (nat.BL_ACTIVETESTING, nat.BL_VMA)
+            self.s1, self.s2 = (z(H, dt=torch.float64), z(H, dt=torch.float64)) if lure else (None, None)
+            self.lpost = z(H, dt=torch.float32) if method == nat.BL_MODELPICKER else None
+            self.lzeros = z(self.N, dt=torch.float32) if method == nat.BL_IID else None
+            self.h_idx = z(HIST_CAP, dt=torch.int64)
+            self.h_q = z(HIST_CAP, dt=torch.float64)
+            self.h_tie = z(HIST_CAP, dt=torch.int32)
+            self.h_best = z(HIST_CAP, dt=torch.int32)
+            self.h_btie = z(HIST_CAP, dt=torch.int32)
+            self.h_loss = z(HIST_CAP, H, dt=torch.uint8) if lure else None
+        self.lmethod, self.lgraph, self.lstruct = method, None, None
+        self.lgamma_f32 = float(np.float32(gamma))            # gamma enters modelpicker.py:78 as a float32 factor
+        self.n_global = int(n_global)
+        # the vector the arg-extreme selection runs over (IID: all zeros, so the k-th tie is the k-th unlabeled item)
+        self.lvec = {nat.BL_IID: self.lzeros, nat.BL_UNCERTAINTY: getattr(self, "score", None),
+                     nat.BL_MODELPICKER: getattr(self, "ent", None)}.get(method)
+
+    def loop_bind(self, labels, pre_len):
+        """(Re)build the loop struct for these labels and a pre-draw buffer of at least ``pre_len``; a new struct
+        drops the captured graph (its kernels hold the old pointers)."""
+        if self.pre.numel() < pre_len:
+            with self._on():
+                self.pre = torch.zeros(max(pre_len, 2 * self.pre.numel()), dtype=torch.float64, device=self.dev)
+            self.lstruct = None
+        if self.lstruct is not None and self.lstruct.labels == labels.data_ptr():
+            return
+        a = nat.BlLoopStruct()
+        a.method, a.H, a.N, a.n_offset, a.n_global = self.lmethod, self.H, self.N, self.n_offset, self.n_global
+        a.hard, a.disagree, a.labeled, a.labels = _ptr(self.hard), _ptr(self.disagree), _ptr(self.labeled), _ptr(labels)
+        a.pre, a.ls, a.best, a.total = _ptr(self.pre), _ptr(self.ls), _ptr(self.best), _ptr(self.total_buf)
+        a.pick = _ptr(self.out)
+        a.counts, a.s1, a.s2, a.post = _ptr(self.counts), _ptr(self.s1), _ptr(self.s2), _ptr(self.lpost)
+        a.gamma = self.lgamma_f32
+        a.hist_cap = HIST_CAP
+        a.hist_idx, a.hist_q, a.hist_tie = _ptr(self.h_idx), _ptr(self.h_q), _ptr(self.h_tie)
+        a.hist_best, a.hist_best_tie, a.hist_loss = _ptr(self.h_best), _ptr(self.h_btie), _ptr(self.h_loss)
+        a.flags = _ptr(self.flags)
+        self.lstruct, self.lgraph, self._labels_keep = a, None, labels
+
+    def _lw(self, i):
+        return self.ls.data_ptr() + 8 * i                     # address of loop word i
+
+    def loop_phase(self, phase):
+        """Enqueue phase 0-3 of one device-loop step: the selection pass, the draw, the pick, the step kernel."""
+        m, a = self.lmethod, ctypes.byref(self.lstruct)
+        lure = m in (nat.BL_ACTIVETESTING, nat.BL_VMA)
+        with self._on():
+            if phase == 0:
+                if lure:
+                    self.total(self.score)
+                    return
+                if m == nat.BL_MODELPICKER:
+                    self._call("coda_b200_mp_entropy_dev", _ptr(self.hard), _ptr(self.lpost), self.H, self.N, self.C,
+                               self.lgamma_f32, _ptr(self.labeled), _ptr(self.disagree), self._lw(7), _ptr(self.ent),
+                               self._s())
+                self.extreme(self.lvec, m != nat.BL_MODELPICKER)
+            elif phase == 1:
+                self._call("coda_b200_bl_draw", a, self._s())
+            elif phase == 2:
+                if lure:
+                    self._call("coda_b200_weighted_draw_xchg_dev", _ptr(self.score), _ptr(self.labeled), self.N,
+                               _ptr(self.total_buf), self._lw(8), self._lw(2), self.n_offset, _ptr(self.part_f),
+                               _ptr(self.out), self._x(), _ptr(self.flags), self._s())
+                else:
+                    self._call("coda_b200_select_kth_xchg_dev", _ptr(self.lvec), _ptr(self.labeled), self.N,
+                               _ptr(self.part_i),
+                               _ptr(self.best), self._lw(3), self._lw(2), self.n_offset, _ptr(self.out), self._x(),
+                               _ptr(self.flags), self._s())
+            else:
+                self._call("coda_b200_bl_step", a, self._x(), self._s())
+
+    def loop_body(self):
+        for phase in range(4):
+            self.loop_phase(phase)
+
+    def loop_capture(self):
+        """Capture one step as a CUDA graph (nothing runs during the capture)."""
+        torch.cuda.synchronize(self.dev)
+        g = torch.cuda.CUDAGraph()
+        cap = self.stream or torch.cuda.Stream(device=self.dev)
+        with torch.cuda.device(self.dev):
+            with torch.cuda.graph(g, stream=cap, capture_error_mode="relaxed"):
+                self.loop_body()
+        torch.cuda.synchronize(self.dev)
+        self.lgraph = g
+
+    def loop_replay(self):
+        with self._on():
+            if self.lgraph is None:
+                self.loop_body()
+            else:
+                self.lgraph.replay()
+
     def read(self, t):
         """Host copy of ``t`` (a result of the calls above) as a list."""
         with self._on():
@@ -233,6 +385,7 @@ class _DeviceState:
             return bool(int(self.flags.item()) & nat.FLAG_XCHG_TIMEOUT)
 
     def close(self):
+        self.lgraph = self.lstruct = self._labels_keep = None
         if self._mailbox is not None:
             self._mailbox.close()
             self._mailbox = None
@@ -302,6 +455,13 @@ class _Baseline(ModelSelector):
         self.d_l_idxs = []
         self.d_l_ys = []
         self.d_u_idxs = _UnlabeledItems(self.N, self._mark)
+        self._loop_dirty = False        # device-loop steps not yet mirrored into the host-side state
+        self._loop_ready = False
+        self._dev_steps = 0             # device-loop steps ever
+        self._hist_seen = 0             # of which mirrored by history()
+        self._dev_nlab = -1             # labels the device-side sums hold (-1: never written)
+        self._hist = {k: [] for k in ("idx", "q", "tie", "best", "best_tie")}
+        self._loop_labels = None
 
     def _mark(self, idx):
         for st in self.states:
@@ -416,6 +576,212 @@ class _Baseline(ModelSelector):
             self.stochastic = True
         return best
 
+    # -- host-free loop ---------------------------------------------------------------------------------------------
+    _loop_method = None             # nat.BL_* of the class
+    _loop_draw = None               # predraw kind of the class
+
+    def _loop_check(self, k, labels):
+        from coda.options import accuracy_loss
+        if isinstance(self.group, ProcessGroup):
+            raise NotImplementedError("coda_b200.baselines: run_steps drives the shards of one process; with one "
+                                      "process per GPU use the API loop, or gpus= / shards= in a single process")
+        if getattr(self, "loss_fn", accuracy_loss) is not accuracy_loss:
+            raise NotImplementedError("coda_b200.baselines: run_steps computes the loss on the device as "
+                                      "hard[idx, h] != label (coda.options.accuracy_loss); use the API loop "
+                                      "(get_next_item_to_label / add_label) for another loss_fn")
+        if not isinstance(labels, torch.Tensor) or labels.dim() != 1 or labels.numel() != self.N:
+            raise ValueError(f"coda_b200.baselines: labels must be a 1-d tensor of all {self.N} labels")
+        left = len(self.d_u_idxs) - (self._dev_steps - self._hist_seen)
+        if not 0 <= k <= left:
+            raise ValueError(f"coda_b200.baselines: run_steps({k}) with {left} unlabeled items left")
+
+    def _loop_bind_labels(self, labels):
+        cache = self._loop_labels
+        if cache is None or cache[0] is not labels:
+            per_dev = {}
+            for st in self.states:
+                if st.dev not in per_dev:
+                    per_dev[st.dev] = labels.to(st.dev, torch.int64).contiguous()
+            for d in per_dev:
+                torch.cuda.synchronize(d)
+            self._loop_labels = cache = (labels, per_dev)
+        return cache[1]
+
+    def _loop_upload(self, seed):
+        """Write the host-side state (labels so far, the method's sums) into every shard's loop buffers."""
+        m, H, nlab = self._loop_method, self.H, len(self.d_l_idxs)
+        words = torch.zeros(_LS_WORDS, dtype=torch.int64)
+        words[0], words[5], words[6] = nlab, self._dev_steps, seed
+        sums = {}                                      # staged on the host: no shard stream reads the caller's tensors
+        if m in (nat.BL_IID, nat.BL_UNCERTAINTY):
+            sums["counts"] = self._risk_sum.round().to(torch.int32).cpu()
+        elif m == nat.BL_MODELPICKER:
+            words[7] = int(self._n_disagree)
+            sums["counts"] = self.correct_counts.to(torch.int32).cpu()
+            sums["lpost"] = self.posterior.cpu()
+        else:                                        # the LURE sums, in the order bl_step adds them
+            s1, s2 = np.zeros(H), np.zeros(H)
+            Ng = float(self.N)
+            for mm, (L, q) in enumerate(zip(self.losses, self.qs), start=1):
+                L = L.reshape(-1).double().cpu().numpy() != 0
+                a = 1.0 / ((Ng - mm + 1.0) * float(q)) - 1.0
+                t = a / (Ng - mm) if Ng - mm > 0 else 0.0
+                s1 = s1 + np.where(L, 1.0, 0.0)
+                s2 = s2 + np.where(L, t, 0.0)
+            sums["s1"], sums["s2"] = torch.from_numpy(s1), torch.from_numpy(s2)
+        for st in self.states:
+            st.enter()
+            with st._on():
+                st.ls.copy_(words)
+                for name, v in sums.items():
+                    getattr(st, name).copy_(v)
+        self._dev_nlab = nlab
+
+    def run_steps(self, k, labels, *, seed=None):
+        """``k`` steps of main.py:91-94 (get_next_item_to_label, oracle, add_label, get_best_model_prediction) on the
+        device: after a warm-up step, one CUDA-graph replay per step and shard (``CODA_B200_GRAPH=0``: the same
+        kernels launched one by one), one host sync at the end.  ``labels``: int64 tensor of all N labels (cached per
+        device).  ``seed``: key of the Philox stream of the tie draws (``None``: one ``torch.randint`` on the CPU
+        generator).  Python ``random`` is consumed as by ``k`` API steps.  When a step needs what the device loop does
+        not do (VMA's uniform fallback, ActiveTesting's zero total), the remaining steps run on the API path, with the
+        API's result or error.  Returns the number of steps performed (``k``); read ``history()`` /
+        ``best_history()`` afterwards."""
+        k = int(k)
+        self._loop_check(k, labels)
+        if k == 0:
+            return 0
+        per_dev = self._loop_bind_labels(labels)
+        if seed is None:
+            seed = int(torch.randint(0, 1 << 62, (1,)).item())
+        seed = int(seed) & ((1 << 64) - 1)
+        seed = seed - (1 << 64) if seed >= 1 << 63 else seed
+        if not self._loop_ready:
+            gamma = getattr(self, "gamma", 1.0)
+            for st in self.states:
+                st.loop_alloc(self._loop_method, self.N, gamma)
+            self._loop_ready = True
+        n0 = len(self.d_u_idxs) - (self._dev_steps - self._hist_seen)
+        state0 = random.getstate()
+        pre = predraw(self._loop_draw, k, n0)
+        pre_host = torch.tensor(pre or [0.0], dtype=torch.float64).pin_memory()
+        for st in self.states:
+            st.enter()                                # after what the caller's stream enqueued (API-path state)
+            st.loop_bind(per_dev[st.dev], k)
+        if not self._loop_dirty and self._dev_nlab != len(self.d_l_idxs):
+            self._loop_upload(seed)
+        for st in self.states:
+            with st._on():
+                st.pre[:pre_host.numel()].copy_(pre_host, non_blocking=True)
+                st.ls[1:3].zero_()
+                st.ls[6].fill_(seed)
+        use_graph = os.environ.get("CODA_B200_GRAPH", "1") != "0"
+        done_before = self._dev_steps
+        left = k
+        while left:
+            if self._dev_steps - self._hist_seen >= HIST_CAP:
+                self._pull()                          # the ring is full: mirror it before it wraps
+            n = min(left, HIST_CAP - (self._dev_steps - self._hist_seen))
+            j = 0
+            if use_graph and any(st.lgraph is None for st in self.states):
+                for phase in range(4):                # warm-up, in lock-step phases over the shards: a kernel's first
+                    for st in self.states:            # launch may load its module while a peer's exchange spins
+                        st.loop_phase(phase)
+                for st in self.states:
+                    st.loop_capture()
+                j = 1
+            for _ in range(n - j):
+                if use_graph:
+                    for st in self.states:
+                        st.loop_replay()
+                else:
+                    for phase in range(4):
+                        for st in self.states:
+                            st.loop_phase(phase)
+            left -= n
+            self._dev_steps += n                      # provisional; corrected from the device below
+            self._loop_dirty = True
+        with self.state._on():
+            done = int(self.state.ls[1].item())
+        self._check_exchanges()
+        self._dev_steps = done_before + done
+        self._dev_nlab = len(self.d_l_idxs) + (self._dev_steps - self._hist_seen)
+        self._loop_dirty = self._dev_steps > self._hist_seen
+        if done < k:                                   # the API path takes over where the device loop stopped
+            self.history()
+            rewind(state0, self._loop_draw, done, n0)
+            lab = self._loop_labels[0]
+            for _ in range(k - done):
+                idx, q = self.get_next_item_to_label()
+                self.add_label(idx, int(lab[idx]), q)
+                self.get_best_model_prediction()
+        return k
+
+    def _pull(self):
+        """Mirror the device-loop steps not yet seen into the host-side state."""
+        st = self.state
+        with st._on():
+            ls = st.ls.cpu().tolist()
+        n0, n1 = self._hist_seen, int(ls[5])                # ls[5]: device-loop steps ever
+        self._dev_steps = n1
+        if n1 <= n0:
+            self._loop_dirty = False
+            return
+        with st._on():
+            slots = torch.arange(n0, n1, device=st.dev) % HIST_CAP
+            got = {k: getattr(st, "h_" + k)[slots].cpu().numpy() for k in ("idx", "q", "tie", "best", "btie")}
+            loss = st.h_loss[slots].to(torch.float32) if st.h_loss is not None else None
+        self._check_exchanges()
+        idx = got["idx"].astype(np.int64)
+        lab = self._loop_labels[0]
+        ys = lab[torch.as_tensor(idx, device=lab.device)].cpu().tolist() if lab.is_cuda else lab[idx].tolist()
+        for i, y in zip(idx.tolist(), ys):
+            self.d_u_idxs.remove_marked(i)
+            self.d_l_idxs.append(int(i))
+            self.d_l_ys.append(int(y))
+        for key, v in (("idx", idx), ("q", got["q"]), ("tie", got["tie"]), ("best", got["best"]),
+                       ("best_tie", got["btie"])):
+            self._hist[key].append(v)
+        m = self._loop_method
+        with st._on():
+            if m in (nat.BL_IID, nat.BL_UNCERTAINTY):
+                self._risk_sum = st.counts.to(torch.float32)
+            elif m == nat.BL_MODELPICKER:
+                self.posterior = st.lpost.clone()
+                self.correct_counts = st.counts.to(torch.int64)
+                self._n_disagree = int(ls[7])
+            else:
+                self.losses.extend(loss.unbind(0))
+                self.qs.extend(float(q) for q in got["q"])
+                self.M += n1 - n0
+        if got["tie"].any() or got["btie"].any():
+            self.stochastic = True
+        st.leave()                                     # the caller's stream reads what shard 0's stream produced
+        self._hist_seen = n1
+        self._dev_nlab = len(self.d_l_idxs)
+        self._loop_dirty = False
+
+    def _hist_arrays(self, *keys):
+        out = []
+        for key in keys:
+            parts = self._hist[key]
+            out.append(np.concatenate(parts) if parts else np.zeros(0, np.float64 if key == "q" else np.int64))
+        return tuple(out)
+
+    def history(self):
+        """(idx, q, tie) of every device-loop step so far (``tie[s] = 1``: the item was drawn among exactly tied items);
+        also brings the host-side state (``d_l_idxs``, ``d_l_ys``, ``d_u_idxs``, the method's sums, ``stochastic``) up
+        to date."""
+        if self._loop_dirty:
+            self._pull()
+        return self._hist_arrays("idx", "q", "tie")
+
+    def best_history(self):
+        """(best, best_tie) of every device-loop step: the model ``get_best_model_prediction()`` would have returned
+        after that step, and 1 where it was drawn among exactly tied models."""
+        if self._loop_dirty:
+            self._pull()
+        return self._hist_arrays("best", "best_tie")
+
     def close(self):
         """Free the device buffers and mailboxes of every shard now (a script can then build the next selector on the
         same card)."""
@@ -433,6 +799,8 @@ class _Baseline(ModelSelector):
 class IID(_Baseline):
     """Uniform sampling of the unlabeled items; the best model has the lowest mean loss on the labels (iid.py)."""
 
+    _loop_method, _loop_draw = nat.BL_IID, "choice"
+
     def __init__(self, dataset, loss_fn, *, gpus=None, shards=None, comm=None):
         self._setup(dataset, gpus, shards, comm)
         self.loss_fn = loss_fn
@@ -442,30 +810,36 @@ class IID(_Baseline):
     def _loss(self, col, true_class, dev):
         return self.loss_fn(col, torch.tensor([true_class], device=dev).expand(self.H))
 
+    @_synced
     def get_next_item_to_label(self):
         self.stochastic = True
         n = len(self.d_u_idxs)
         idx = self.d_u_idxs[random.choice(range(n))]      # the same draw as random.choice over the list
         return idx, 1.0 / n
 
+    @_synced
     def add_label(self, chosen_idx, true_class, selection_prob=None):
         self._record(chosen_idx, true_class)
         # the per-label losses added in label order: the sum iid.py:37-43 recomputes from scratch
         # (a 16-bit slab's scores are widened first: the loss sees the fp32 values the reference loader would produce)
         self._risk_sum += self._label_losses(chosen_idx, true_class)
 
+    @_synced
     def get_risk_estimates(self):
         risk = self._risk_sum.clone()
         if self.d_l_idxs:
             risk /= len(self.d_l_idxs)
         return risk
 
+    @_synced
     def get_best_model_prediction(self):
         return self._min_risk_model(self.get_risk_estimates())
 
 
 class Uncertainty(IID):
     """The unlabeled item of highest ensemble-mean entropy (uncertainty.py); a static score."""
+
+    _loop_method, _loop_draw = nat.BL_UNCERTAINTY, None
 
     def __init__(self, dataset, loss_fn, *, gpus=None, shards=None, comm=None):
         super().__init__(dataset, loss_fn, gpus=gpus, shards=shards, comm=comm)
@@ -476,6 +850,7 @@ class Uncertainty(IID):
             del _hard, _dis, ens
         self.stochastic = False
 
+    @_synced
     def get_next_item_to_label(self):
         if not len(self.d_u_idxs):
             raise IndexError("max(): Expected reduction dim 0 to have non-zero size.")
@@ -493,6 +868,7 @@ class ActiveTesting(IID):
     surrogate, summed over the models; risks by the LURE estimator (activetesting.py)."""
 
     _vma = False
+    _loop_method, _loop_draw = nat.BL_ACTIVETESTING, "random"
 
     def __init__(self, dataset, loss_fn, *, gpus=None, shards=None, comm=None):
         super().__init__(dataset, loss_fn, gpus=gpus, shards=shards, comm=comm)
@@ -516,6 +892,7 @@ class ActiveTesting(IID):
             raise ValueError("Total of weights must be finite")
         return self._weighted_draw(random.random())
 
+    @_synced
     def get_next_item_to_label(self):
         return self._draw()
 
@@ -524,20 +901,24 @@ class ActiveTesting(IID):
         N, M = self.N, self.M
         return [1 + ((N - M) / (N - m)) * (1 / ((N - m + 1) * q) - 1) for m, q in enumerate(self.qs, start=1)]
 
+    @_synced
     def get_lure_risks_and_vars(self):
         losses = torch.stack(self.losses, dim=1).view(self.H, -1)
         weighted = torch.tensor(self.get_vs(), device=self.device).unsqueeze(0) * losses
         return weighted.mean(dim=1), weighted.var(dim=1, unbiased=True) / self.M
 
+    @_synced
     def add_label(self, chosen_idx, true_class, selection_prob=None):
         self._record(chosen_idx, true_class)
         self.losses.append(self._label_losses(chosen_idx, true_class))
         self.qs.append(selection_prob)
         self.M += 1
 
+    @_synced
     def get_risk_estimates(self):
         return self.get_lure_risks_and_vars()[0]
 
+    @_synced
     def get_best_model_prediction(self):
         if self.losses:
             return self._min_risk_model(self.get_risk_estimates())
@@ -549,7 +930,9 @@ class VMA(ActiveTesting):
     ensemble-mean surrogate (vma.py); uniform when every score is 0."""
 
     _vma = True
+    _loop_method = nat.BL_VMA
 
+    @_synced
     def get_next_item_to_label(self):
         total, n = self._total()
         if np.float32(total) < np.float32(1e-12):
@@ -560,6 +943,8 @@ class VMA(ActiveTesting):
 class ModelPicker(_Baseline):
     """Karimi et al. (2021): the unlabeled item of least expected posterior entropy over the models, the best model
     the one with the most correct labels (modelpicker.py)."""
+
+    _loop_method = nat.BL_MODELPICKER
 
     def __init__(self, dataset, epsilon=0.46, *, gpus=None, shards=None, comm=None):
         self._setup(dataset, gpus, shards, comm)
@@ -597,6 +982,7 @@ class ModelPicker(_Baseline):
             out[off:off + n] = allv[r, :n]
         return out
 
+    @_synced
     def get_next_item_to_label(self):
         n = len(self.d_u_idxs)
         if n == 0:
@@ -618,6 +1004,7 @@ class ModelPicker(_Baseline):
         idx, _val = self._select_extreme("ent", False, lambda cnt: int(torch.randint(cnt, (1,))[0]))
         return idx, 1.0 / float(n)
 
+    @_synced
     def add_label(self, chosen_idx, true_class, selection_prob=None):
         self._record(chosen_idx, true_class)
         if self._disagree_host[int(chosen_idx)]:
@@ -635,6 +1022,7 @@ class ModelPicker(_Baseline):
         post = posterior * (gamma ** (predictions_i == oracle_i).float())
         return post / post.sum()
 
+    @_synced
     def get_best_model_prediction(self):
         if not self.d_l_idxs:
             return torch.randint(self.H, (1,), device=self.device).item()

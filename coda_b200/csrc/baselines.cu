@@ -4,6 +4,7 @@
 // the mailboxes of xchg.cuh (record channel), so every shard ends a selection call with the same global answer.
 #include "xchg.cuh"
 
+#include <curand_philox4x32_x.h>
 #include <limits.h>
 
 #define BL_THREADS 256
@@ -45,11 +46,15 @@ __device__ __forceinline__ void for_each_group(const uint16_t* row, int H, int l
 // ModelPicker acquisition (modelpicker.py:58-86) in closed form over the groups Z_c of an item (see the header).
 // Block prologue: p_h and p_h log2 p_h (0 log 0 = 0) in shared memory, S and B by every warp in the same order.
 // ---------------------------------------------------------------------------------------------------------------
+// DEV: the mask switch is *mask_dev > 0 (device loop) instead of mask_agreeing
+template <bool DEV>
 __global__ void __launch_bounds__(BL_THREADS) k_mp_entropy(const uint16_t* __restrict__ hard, const float* __restrict__ post,
                                                            int H, long long N, int C, double gamma,
                                                            const uint8_t* __restrict__ labeled,
                                                            const uint8_t* __restrict__ disagree, int mask_agreeing,
+                                                           const long long* __restrict__ mask_dev,
                                                            float* __restrict__ ent) {
+  if (DEV) mask_agreeing = *mask_dev > 0;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double* sp = reinterpret_cast<double*>(smem_raw);
   double* spl = sp + H;
@@ -107,8 +112,8 @@ extern "C" int coda_b200_mp_entropy(const uint16_t* hard, const float* posterior
   const size_t smem = (size_t)2 * H * sizeof(double) + (size_t)(BL_THREADS / 32) * Hp * sizeof(uint16_t);
   long long grid = (N + BL_THREADS / 32 - 1) / (BL_THREADS / 32);
   grid = min(grid, (long long)coda_sm_count() * 8);
-  k_mp_entropy<<<(unsigned)grid, BL_THREADS, smem, as_stream(stream)>>>(hard, posterior, H, N, C, gamma, labeled,
-                                                                         disagree, mask_agreeing, ent);
+  k_mp_entropy<false><<<(unsigned)grid, BL_THREADS, smem, as_stream(stream)>>>(hard, posterior, H, N, C, gamma, labeled,
+                                                                                disagree, mask_agreeing, nullptr, ent);
   CODA_LAUNCH_OK("k_mp_entropy");
   return CODA_B200_OK;
 }
@@ -460,11 +465,10 @@ __global__ void __launch_bounds__(BL_THREADS) k_extreme_xchg(const long long* __
 }
 
 // the k-th tied item over all shards: the shard whose ties cover k picks its local (k - lower)-th, all get n_offset + it
-__global__ void __launch_bounds__(BL_THREADS) k_select_kth_xchg(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
-                                                               long long N, const long long* __restrict__ partials,
-                                                               int nblocks, const long long* __restrict__ best, long long k,
-                                                               long long n_offset, XchgView x, long long* __restrict__ out,
-                                                               uint32_t* __restrict__ flags) {
+__device__ __forceinline__ void kth_xchg_body(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
+                                              long long N, const long long* __restrict__ partials, int nblocks,
+                                              const long long* __restrict__ best, long long k, long long n_offset,
+                                              const XchgView& x, long long* __restrict__ out, uint32_t* __restrict__ flags) {
   __shared__ __align__(16) long long stage[2];
   const long long kk = k - best[2];
   long long i = -1;
@@ -485,6 +489,24 @@ __global__ void __launch_bounds__(BL_THREADS) k_select_kth_xchg(const float* __r
     out[0] = g;
   }
   bl_exchange_done(x, ep);
+}
+__global__ void __launch_bounds__(BL_THREADS) k_select_kth_xchg(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
+                                                               long long N, const long long* __restrict__ partials,
+                                                               int nblocks, const long long* __restrict__ best, long long k,
+                                                               long long n_offset, XchgView x, long long* __restrict__ out,
+                                                               uint32_t* __restrict__ flags) {
+  kth_xchg_body(v, labeled, N, partials, nblocks, best, k, n_offset, x, out, flags);
+}
+// device loop: k and the stop word from device memory (the stop word is the same on every shard: no exchange is skipped
+// on one shard only)
+__global__ void __launch_bounds__(BL_THREADS) k_select_kth_dev(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
+                                                              long long N, const long long* __restrict__ partials,
+                                                              int nblocks, const long long* __restrict__ best,
+                                                              const long long* __restrict__ k, const long long* __restrict__ stop,
+                                                              long long n_offset, XchgView x, long long* __restrict__ out,
+                                                              uint32_t* __restrict__ flags) {
+  if (*stop) return;
+  kth_xchg_body(v, labeled, N, partials, nblocks, best, *k, n_offset, x, out, flags);
 }
 
 // total = {fp64 sum over the shards (rank order) of each shard's block-ordered sum, number of unlabeled items}
@@ -516,11 +538,11 @@ __global__ void __launch_bounds__(BL_THREADS) k_wsum_xchg(const double* __restri
 // total in rank order, target = u * grand, and the owner shard (the first one whose running sum passes target, the
 // last non-empty one when rounding leaves none).  The owner draws inside its chunks from the lower ranks' running sum
 // and position.  Exchange 2: {owner?, position, global item, q bits} -> out on every shard.
-__global__ void __launch_bounds__(BL_THREADS) k_wdraw_xchg(const float* __restrict__ w, const uint8_t* __restrict__ labeled,
-                                                          long long N, const double* __restrict__ total,
-                                                          const double* __restrict__ partials, int nblocks, double u,
-                                                          long long n_offset, XchgView x, long long* __restrict__ out,
-                                                          uint32_t* __restrict__ flags) {
+__device__ __forceinline__ void wdraw_xchg_body(const float* __restrict__ w, const uint8_t* __restrict__ labeled,
+                                                long long N, const double* __restrict__ total,
+                                                const double* __restrict__ partials, int nblocks, double u,
+                                                long long n_offset, const XchgView& x, long long* __restrict__ out,
+                                                uint32_t* __restrict__ flags) {
   __shared__ __align__(16) double stage[2];
   __shared__ __align__(16) long long pick[4];
   __shared__ int s_own;
@@ -578,6 +600,22 @@ __global__ void __launch_bounds__(BL_THREADS) k_wdraw_xchg(const float* __restri
     }
   }
   bl_exchange_done(x, ep2);
+}
+__global__ void __launch_bounds__(BL_THREADS) k_wdraw_xchg(const float* __restrict__ w, const uint8_t* __restrict__ labeled,
+                                                          long long N, const double* __restrict__ total,
+                                                          const double* __restrict__ partials, int nblocks, double u,
+                                                          long long n_offset, XchgView x, long long* __restrict__ out,
+                                                          uint32_t* __restrict__ flags) {
+  wdraw_xchg_body(w, labeled, N, total, partials, nblocks, u, n_offset, x, out, flags);
+}
+__global__ void __launch_bounds__(BL_THREADS) k_wdraw_dev(const float* __restrict__ w, const uint8_t* __restrict__ labeled,
+                                                         long long N, const double* __restrict__ total,
+                                                         const double* __restrict__ partials, int nblocks,
+                                                         const double* __restrict__ u, const long long* __restrict__ stop,
+                                                         long long n_offset, XchgView x, long long* __restrict__ out,
+                                                         uint32_t* __restrict__ flags) {
+  if (*stop) return;
+  wdraw_xchg_body(w, labeled, N, total, partials, nblocks, *u, n_offset, x, out, flags);
 }
 
 // The owner's `bytes` from src -> dst on every shard (header {owner?, 0, 0, 0} + payload; the others send the header).
@@ -686,5 +724,294 @@ extern "C" int coda_b200_owner_share(const void* src, int bytes, int own, void* 
   k_owner_share<<<1, BL_THREADS, smem, as_stream(stream)>>>((const unsigned char*)src, bytes, own, (unsigned char*)dst,
                                                             xv, flags);
   CODA_LAUNCH_OK("k_owner_share");
+  return CODA_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Host-free loop of the competing selectors (include/coda_b200.h, coda_bl_loop_t).  Per step and shard: the
+// selection pass of the method, bl_draw (k or u of the step), the *_dev selection kernel, bl_step.  Every per-step
+// scalar is read from the loop words, so one captured graph serves every step.
+// ---------------------------------------------------------------------------------------------------------------
+extern "C" int coda_b200_select_kth_xchg_dev(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
+                                             const int64_t* best, const int64_t* k, const int64_t* stop,
+                                             int64_t n_offset, int64_t* out_idx, const coda_xchg_t* x, uint32_t* flags,
+                                             coda_stream_t stream) {
+  CODA_CHECK_ARG(v && labeled && partials && best && k && stop && out_idx && flags, "select_kth_xchg_dev: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40) && n_offset >= 0, "select_kth_xchg_dev: bad N=%lld", (long long)N);
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 16, "select_kth_xchg_dev")) return rc;
+  k_select_kth_dev<<<1, BL_THREADS, 0, as_stream(stream)>>>(v, labeled, N, (const long long*)partials,
+                                                            coda_b200_select_blocks(N), (const long long*)best,
+                                                            (const long long*)k, (const long long*)stop, n_offset, xv,
+                                                            (long long*)out_idx, flags);
+  CODA_LAUNCH_OK("k_select_kth_dev");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_weighted_draw_xchg_dev(const float* w, const uint8_t* labeled, int64_t N, const double* total,
+                                                const double* u, const int64_t* stop, int64_t n_offset, double* partials,
+                                                int64_t* out, const coda_xchg_t* x, uint32_t* flags,
+                                                coda_stream_t stream) {
+  CODA_CHECK_ARG(w && labeled && total && u && stop && partials && out && flags, "weighted_draw_xchg_dev: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << 40) && n_offset >= 0, "weighted_draw_xchg_dev: bad N=%lld", (long long)N);
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 32, "weighted_draw_xchg_dev")) return rc;
+  const int nb = coda_b200_select_blocks(N);
+  k_wsum_blocks<true><<<nb, BL_THREADS, 0, as_stream(stream)>>>(w, labeled, N, total, partials);
+  CODA_LAUNCH_OK("k_wsum_blocks");
+  k_wdraw_dev<<<1, BL_THREADS, 0, as_stream(stream)>>>(w, labeled, N, total, partials, nb, u, (const long long*)stop,
+                                                       n_offset, xv, (long long*)out, flags);
+  CODA_LAUNCH_OK("k_wdraw_dev");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_mp_entropy_dev(const uint16_t* hard, const float* posterior, int H, int64_t N, int C,
+                                        double gamma, const uint8_t* labeled, const uint8_t* disagree,
+                                        const int64_t* n_disagree, float* ent, coda_stream_t stream) {
+  CODA_CHECK_ARG(hard && posterior && labeled && disagree && n_disagree && ent, "mp_entropy_dev: null pointer");
+  CODA_CHECK_ARG(H >= 1 && H <= 1024 && N >= 1 && C >= 1, "mp_entropy_dev: bad shape H=%d N=%lld C=%d", H, (long long)N, C);
+  CODA_CHECK_ARG(gamma > 0.0, "mp_entropy_dev: gamma must be > 0");
+  const int Hp = (H + 31) & ~31;
+  const size_t smem = (size_t)2 * H * sizeof(double) + (size_t)(BL_THREADS / 32) * Hp * sizeof(uint16_t);
+  long long grid = (N + BL_THREADS / 32 - 1) / (BL_THREADS / 32);
+  grid = min(grid, (long long)coda_sm_count() * 8);
+  k_mp_entropy<true><<<(unsigned)grid, BL_THREADS, smem, as_stream(stream)>>>(hard, posterior, H, N, C, gamma, labeled,
+                                                                               disagree, 0, (const long long*)n_disagree,
+                                                                               ent);
+  CODA_LAUNCH_OK("k_mp_entropy");
+  return CODA_B200_OK;
+}
+
+// r.x of Philox4x32-10 at key = the 64-bit seed, counter = {label count, purpose, 0, 0}
+__device__ __forceinline__ unsigned bl_philox(long long seed, long long count, unsigned purpose) {
+  const unsigned long long k = (unsigned long long)seed;
+  return curand_Philox4x32_10(make_uint4((unsigned)count, purpose, 0u, 0u), make_uint2((unsigned)k, (unsigned)(k >> 32))).x;
+}
+// (r * cnt) >> 32 in 96-bit arithmetic: the tie j in [0, cnt) in ascending index order
+__device__ __forceinline__ long long bl_tie_pick(unsigned r, long long cnt) {
+  const unsigned long long c = (unsigned long long)cnt, lo = (unsigned long long)r * (c & 0xffffffffull);
+  return (long long)(((unsigned long long)r * (c >> 32)) + (lo >> 32));
+}
+
+#define BL_STOP_VMA_UNIFORM 1
+#define BL_STOP_AT_TOTAL 2
+#define BL_STOP_NO_ITEM 3
+
+__global__ void k_bl_draw(const coda_bl_loop_t a) {
+  long long* ls = reinterpret_cast<long long*>(a.ls);
+  if (ls[2]) return;
+  const long long s = ls[1];
+  switch (a.method) {
+    case CODA_B200_BL_IID:
+      ls[3] = (long long)a.pre[s];
+      ls[4] = 0;
+      break;
+    case CODA_B200_BL_UNCERTAINTY:
+    case CODA_B200_BL_MODELPICKER: {
+      const long long cnt = a.best[1];
+      if (cnt < 1) { ls[2] = BL_STOP_NO_ITEM; return; }
+      ls[3] = cnt > 1 ? bl_tie_pick(bl_philox(ls[6], ls[0], 0u), cnt) : 0;
+      ls[4] = cnt > 1;
+      break;
+    }
+    default: {                                        // ActiveTesting, VMA: the API's checks on the fp32 total
+      const float t = (float)a.total[0];
+      if (a.method == CODA_B200_BL_VMA ? t < 1e-12f : !(t > 0.f)) {
+        ls[2] = a.method == CODA_B200_BL_VMA ? BL_STOP_VMA_UNIFORM : BL_STOP_AT_TOTAL;
+        return;
+      }
+      reinterpret_cast<double*>(ls)[8] = a.pre[s];
+      ls[4] = 0;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(BL_THREADS) k_bl_step(const coda_bl_loop_t a, XchgView x) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int H = a.H, nwords = (H + 31) >> 5;
+  const uint32_t hrow = xch_align16((uint32_t)H * 2);
+  unsigned char* stage = smem_raw;                                   // {owner?, disagree bit, 0, 0} + hard row
+  uint16_t* row = reinterpret_cast<uint16_t*>(smem_raw + 16 + hrow);
+  double* rv = reinterpret_cast<double*>(smem_raw + 16 + 2 * hrow);  // the value the best model minimises
+  __shared__ unsigned tie_w[32];
+  __shared__ double s_red[BL_THREADS / 32];
+  __shared__ long long s_idx, s_lab;
+  __shared__ double s_q, s_min, s_sum;
+  __shared__ int s_stop, s_src, s_dis;
+  long long* ls = reinterpret_cast<long long*>(a.ls);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool lure = a.method == CODA_B200_BL_ACTIVETESTING || a.method == CODA_B200_BL_VMA;
+  if (threadIdx.x == 0) {
+    s_stop = ls[2] != 0;
+    if (!s_stop) {
+      const long long idx = lure ? a.pick[1] : a.pick[0];
+      if (idx < 0 || idx >= a.n_global) {             // every shard holds the same global pick: all stop together
+        ls[2] = BL_STOP_NO_ITEM;
+        s_stop = 1;
+      } else {
+        s_idx = idx;
+        s_lab = a.labels[idx];
+        s_q = lure ? (double)__uint_as_float((unsigned)a.pick[2])
+                   : (a.method == CODA_B200_BL_UNCERTAINTY ? (double)__uint_as_float((unsigned)a.best[0])
+                                                           : 1.0 / (double)(a.n_global - ls[0]));
+      }
+    }
+  }
+  __syncthreads();
+  if (s_stop) return;
+  // the owner's hard row (and disagree bit) to every shard
+  const long long idx = s_idx, loc = idx - a.n_offset;
+  const bool own = loc >= 0 && loc < a.N;
+  int* hdr = reinterpret_cast<int*>(stage);
+  uint16_t* srow = reinterpret_cast<uint16_t*>(stage + 16);
+  if (threadIdx.x < 4)
+    hdr[threadIdx.x] = threadIdx.x == 0 ? (int)own : (threadIdx.x == 1 && own && a.disagree ? (int)a.disagree[loc] : 0);
+  for (int i = threadIdx.x; i < (int)(hrow >> 1); i += blockDim.x) srow[i] = (own && i < H) ? a.hard[(size_t)loc * H + i] : 0;
+  if (own && threadIdx.x == 0) a.labeled[loc] = 1;
+  __syncthreads();
+  const unsigned long long ep = bl_exchange(x, bl_epoch(x), stage, own ? 16u + hrow : 16u, a.flags);
+  if (threadIdx.x == 0) {
+    int from = -1;
+    for (int s = 0; s < x.world; ++s)
+      if (reinterpret_cast<const int*>(bl_rec(x, ep, s, stage))[0] == 1) from = s;
+    s_src = from;
+    s_dis = from >= 0 ? reinterpret_cast<const int*>(bl_rec(x, ep, from, stage))[1] : 0;
+  }
+  __syncthreads();
+  {
+    const uint16_t* src = s_src >= 0 ? reinterpret_cast<const uint16_t*>(
+                                           reinterpret_cast<const unsigned char*>(bl_rec(x, ep, s_src, stage)) + 16)
+                                     : nullptr;                       // a peer timed out (flag set): no row
+    for (int h = threadIdx.x; h < H; h += blockDim.x) row[h] = src ? src[h] : (uint16_t)0xFFFF;
+  }
+  bl_exchange_done(x, ep);
+  // the method's sums
+  const long long lab = s_lab, M = ls[0] + 1, slot = ls[5] % a.hist_cap;
+  if (lure) {
+    // LURE (activetesting.py:61-90) from running fp64 sums: sum_m v_m L_m = S1 + (N - M) S2, with
+    // S2 = sum_m L_m a_m / (N - m) and a_m = 1 / ((N - m + 1) q_m) - 1
+    const double Ng = (double)a.n_global, m = (double)M;
+    const double am = 1.0 / ((Ng - m + 1.0) * s_q) - 1.0;
+    const double t = Ng - m > 0.0 ? am / (Ng - m) : 0.0;
+    for (int h = threadIdx.x; h < H; h += blockDim.x) {
+      const bool L = (long long)row[h] != lab;
+      const double s1 = a.s1[h] + (L ? 1.0 : 0.0), s2 = a.s2[h] + (L ? t : 0.0);
+      a.s1[h] = s1;
+      a.s2[h] = s2;
+      if (a.hist_loss) a.hist_loss[(size_t)slot * H + h] = L;
+      rv[h] = (s1 + (Ng - m) * s2) / m;
+    }
+  } else if (a.method == CODA_B200_BL_MODELPICKER) {
+    // modelpicker.py:89-95: post * gamma^agree / sum (fp32 products, the sum in fp64 in a fixed order, rounded once)
+    double part = 0.0;
+    for (int h = threadIdx.x; h < H; h += blockDim.x) {
+      const bool agree = (long long)row[h] == lab;
+      const int c = a.counts[h] + (agree ? 1 : 0);
+      a.counts[h] = c;
+      const float p = agree ? __fmul_rn(a.post[h], a.gamma) : a.post[h];
+      rv[h] = (double)p;
+      part += (double)p;
+    }
+    part = warp_sum(part);
+    if (lane == 0) s_red[warp] = part;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double t = 0.0;
+      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_red[w];
+      s_sum = t;
+    }
+    __syncthreads();
+    const float sf = (float)s_sum;
+    for (int h = threadIdx.x; h < H; h += blockDim.x) {
+      a.post[h] = __fdiv_rn((float)rv[h], sf);
+      rv[h] = -(double)a.counts[h];                        // most correct labels
+    }
+  } else {                                                 // IID, Uncertainty: the mean loss is count / M
+    for (int h = threadIdx.x; h < H; h += blockDim.x) {
+      const int c = a.counts[h] + ((long long)row[h] != lab ? 1 : 0);
+      a.counts[h] = c;
+      rv[h] = (double)c;
+    }
+  }
+  __syncthreads();
+  // the best model: the lowest rv, a Philox draw among exact ties
+  double mn = INFINITY;
+  for (int h = threadIdx.x; h < H; h += blockDim.x) mn = fmin(mn, rv[h]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mn = fmin(mn, __shfl_xor_sync(CODA_FULL, mn, o));
+  if (lane == 0) s_red[warp] = mn;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = INFINITY;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t = fmin(t, s_red[w]);
+    s_min = t;
+  }
+  __syncthreads();
+  for (int base = 0; base < H; base += blockDim.x) {       // block-uniform trip count
+    const int h = base + threadIdx.x;
+    const unsigned b = __ballot_sync(CODA_FULL, h < H && rv[h] == s_min);
+    if (lane == 0 && (base >> 5) + warp < nwords) tie_w[(base >> 5) + warp] = b;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int cnt = 0;
+    for (int w = 0; w < nwords; ++w) cnt += __popc(tie_w[w]);
+    long long j = cnt > 1 ? bl_tie_pick(bl_philox(ls[6], M, 1u), cnt) : 0;
+    int best = -1;
+    for (int w = 0; w < nwords && best < 0; ++w) {
+      unsigned b = tie_w[w];
+      const int c = __popc(b);
+      if (j < c) {
+        for (; j > 0; --j) b &= b - 1;
+        best = w * 32 + __ffs(b) - 1;
+      } else {
+        j -= c;
+      }
+    }
+    a.hist_idx[slot] = idx;
+    a.hist_q[slot] = s_q;
+    a.hist_tie[slot] = (int)ls[4];
+    a.hist_best[slot] = best;
+    a.hist_best_tie[slot] = cnt > 1;
+    if (a.method == CODA_B200_BL_MODELPICKER && s_dis) ls[7] -= 1;
+    ls[0] = M;
+    ls[1] += 1;
+    ls[5] += 1;
+  }
+}
+
+static int bl_loop_ok(const coda_bl_loop_t* a, const char* what) {
+  CODA_CHECK_ARG(a && a->ls && a->flags, "%s: null pointer", what);
+  CODA_CHECK_ARG(a->method >= CODA_B200_BL_IID && a->method <= CODA_B200_BL_MODELPICKER, "%s: bad method %d", what,
+                 a->method);
+  CODA_CHECK_ARG(a->H >= 1 && a->H <= 1024 && a->N >= 1 && a->n_global >= a->N && a->n_offset >= 0,
+                 "%s: bad shape H=%d N=%lld", what, a->H, (long long)a->N);
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_bl_draw(const coda_bl_loop_t* a, coda_stream_t stream) {
+  if (int rc = bl_loop_ok(a, "bl_draw")) return rc;
+  const bool lure = a->method == CODA_B200_BL_ACTIVETESTING || a->method == CODA_B200_BL_VMA;
+  CODA_CHECK_ARG((a->method == CODA_B200_BL_UNCERTAINTY || a->method == CODA_B200_BL_MODELPICKER || a->pre) &&
+                 (!lure || a->total) && (lure || a->best), "bl_draw: null pointer");
+  k_bl_draw<<<1, 1, 0, as_stream(stream)>>>(*a);
+  CODA_LAUNCH_OK("k_bl_draw");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_bl_step(const coda_bl_loop_t* a, const coda_xchg_t* x, coda_stream_t stream) {
+  if (int rc = bl_loop_ok(a, "bl_step")) return rc;
+  const bool lure = a->method == CODA_B200_BL_ACTIVETESTING || a->method == CODA_B200_BL_VMA;
+  const bool mp = a->method == CODA_B200_BL_MODELPICKER;
+  CODA_CHECK_ARG(a->hard && a->labeled && a->labels && a->pick && a->best && a->hist_idx && a->hist_q && a->hist_tie &&
+                 a->hist_best && a->hist_best_tie && (lure ? (a->s1 && a->s2) : a->counts != nullptr) &&
+                 (!mp || (a->post && a->disagree)), "bl_step: null pointer");
+  CODA_CHECK_ARG(a->hist_cap >= 1, "bl_step: bad hist_cap");
+  const uint32_t hrow = xch_align16((uint32_t)a->H * 2);
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 16u + hrow, "bl_step")) return rc;
+  const size_t smem = 16 + 2 * (size_t)hrow + (size_t)a->H * sizeof(double);
+  k_bl_step<<<1, BL_THREADS, smem, as_stream(stream)>>>(*a, xv);
+  CODA_LAUNCH_OK("k_bl_step");
   return CODA_B200_OK;
 }

@@ -423,6 +423,22 @@ extern "C" int coda_b200_step_mixture(const coda_step_t* st, const coda_xchg_t* 
   return CODA_B200_OK;
 }
 
+__global__ void k_record_best(const long long* __restrict__ best_model, const long long* __restrict__ step_ctr,
+                              int* __restrict__ hist_best, long long hist_cap) {
+  const long long k = *step_ctr - 1;
+  if (k >= 0) hist_best[k % hist_cap] = (int)*best_model;
+}
+
+extern "C" int coda_b200_record_best(const int64_t* best_model, const int64_t* step_ctr, int32_t* hist_best,
+                                     int64_t hist_cap, coda_stream_t stream) {
+  CODA_CHECK_ARG(best_model && step_ctr && hist_best, "record_best: null pointer");
+  CODA_CHECK_ARG(hist_cap >= 1, "record_best: bad hist_cap %lld", (long long)hist_cap);
+  k_record_best<<<1, 1, 0, as_stream(stream)>>>((const long long*)best_model, (const long long*)step_ctr, hist_best,
+                                                hist_cap);
+  CODA_LAUNCH_OK("k_record_best");
+  return CODA_B200_OK;
+}
+
 // ---- tie scan against the GLOBAL record ---------------------------------------------------------------
 // tie_hdr: {count, min tied global index}; tie_idx/tie_val hold up to `cap` entries (unordered).
 __global__ void __launch_bounds__(256) k_ties(const float* __restrict__ eig, long long N,

@@ -678,12 +678,22 @@ class Engine:
             self.labels_ptr = labels_dev.data_ptr()
             self._labels_keep = labels_dev
             self.graphs.pop("loop", None)
+            self.graphs.pop("loop_best", None)
 
     def _loop_body(self):
         """select -> posterior update -> scoring pass for the next selection (one graph)."""
         self._call("coda_b200_step_select", self.st, self._x(), self._s())
         self._post_label()
         self._score()
+
+    def _loop_body_best(self):
+        """The loop body, then best_model (written by step_mixture on this stream) -> hist_best[step_ctr - 1]."""
+        self._loop_body()
+        self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
+                   HIST_CAP, self._s())
+
+    def _loop_key(self, record_best):
+        return ("loop_best", self._loop_body_best) if record_best else ("loop", self._loop_body)
 
     def device_step(self, labels_dev: torch.Tensor, step: int | None = None, hist_idx=None, hist_q=None):
         """One acquisition step with no host round trip: pick the arg-max (first index on equal values, coda.py:309;
@@ -703,17 +713,21 @@ class Engine:
 
     # The graph loop in phases, so that a front end driving several shards from one thread never blocks on a shard
     # whose peers have not been enqueued yet: prepare (no exchange inside) -> one eager step -> capture -> replays.
-    def loop_prepare(self, labels_dev: torch.Tensor):
+    # record_best: a separately captured graph that also records the best model of every step (hist_best); the
+    # default graph is the plain loop body.
+    def loop_prepare(self, labels_dev: torch.Tensor, record_best: bool = False):
         with self._on():
             self._bind_labels(labels_dev)
+            if record_best and getattr(self, "hist_best", None) is None:
+                self.hist_best = torch.full((HIST_CAP,), -1, dtype=torch.int32, device=self.dev)
             self._score()
 
-    def loop_ready(self) -> bool:
-        return (not self.use_graph) or self.graphs.get("loop") is not None
+    def loop_ready(self, record_best: bool = False) -> bool:
+        return (not self.use_graph) or self.graphs.get(self._loop_key(record_best)[0]) is not None
 
-    def loop_eager(self):
+    def loop_eager(self, record_best: bool = False):
         with self._on():
-            self._loop_body()
+            self._loop_key(record_best)[1]()
 
     def _try_capture(self, key, body):
         """Capture `body` as graph `key`; a failed capture (driver / allocator state) falls back to eager launches."""
@@ -729,32 +743,39 @@ class Engine:
         self.graphs[key] = g
         return g, n
 
-    def loop_capture(self):
+    def loop_capture(self, record_best: bool = False):
+        key, body = self._loop_key(record_best)
         with self._on():
-            _g, self.launches_per_step = self._try_capture("loop", self._loop_body)
+            _g, n = self._try_capture(key, body)
+            if record_best:
+                self.launches_per_step_best = n
+            else:
+                self.launches_per_step = n
 
-    def loop_replay(self, k: int = 1):
+    def loop_replay(self, k: int = 1, record_best: bool = False):
+        key, body = self._loop_key(record_best)
         with self._on():
-            g = self.graphs.get("loop")
+            g = self.graphs.get(key)
             for _ in range(k):
                 if g is None:
-                    self._loop_body()
+                    body()
                 else:
                     g.replay()
             if g is not None:
-                self.counters["launches"] += k * self.launches_per_step
+                self.counters["launches"] += k * (self.launches_per_step_best if record_best else self.launches_per_step)
 
-    def run_steps(self, k: int, labels_dev: torch.Tensor):
+    def run_steps(self, k: int, labels_dev: torch.Tensor, record_best: bool = False):
         """``k`` acquisition steps as ``k`` replays of one captured CUDA graph (SURVEY.md 8f rank 2; replaces the
-        host loop of main.py:89-94 for offline runs).  History: ``hist_idx/hist_q/hist_tie[step_ctr % HIST_CAP]``."""
+        host loop of main.py:89-94 for offline runs).  History: ``hist_idx/hist_q/hist_tie[step_ctr % HIST_CAP]``,
+        with ``record_best`` also ``hist_best``."""
         if k <= 0:
             return
-        self.loop_prepare(labels_dev)
-        if not self.loop_ready():
-            self.loop_eager()                                   # warm-up (module loading, attributes) outside capture
+        self.loop_prepare(labels_dev, record_best)
+        if not self.loop_ready(record_best):
+            self.loop_eager(record_best)                        # warm-up (module loading, attributes) outside capture
             k -= 1
-            self.loop_capture()
-        self.loop_replay(k)
+            self.loop_capture(record_best)
+        self.loop_replay(k, record_best)
 
     def _capture(self, body):
         torch.cuda.synchronize(self.dev)

@@ -302,11 +302,13 @@ class CODA(ModelSelector):
         return out
 
     # -- host-free loop (SURVEY.md 8f rank 2) ----------------------------------------------------
-    def run_steps(self, k, labels):
+    def run_steps(self, k, labels, *, record_best=False):
         """``k`` acquisition steps with the oracle's labels resident on the device(s): main.py:89-94 without a host
         round trip (arg-max pick, first index on equal values; a step where the reference would have drawn from
         ``random.choice`` because of an isclose tie is flagged in ``history()``).  ``labels``: int64 tensor of all N
-        labels.  Returns nothing; read ``history()`` / ``get_pbest()`` afterwards."""
+        labels.  ``record_best``: replay a graph that also records every step's best model (``best_history()``, the
+        regret curve of main.py:94-103); the default graph does not.  Returns nothing; read ``history()`` /
+        ``get_pbest()`` afterwards."""
         cache = getattr(self, "_labels_dev", None)
         if cache is None or cache[0] is not labels:
             per_dev = {}
@@ -322,16 +324,16 @@ class CODA(ModelSelector):
         self._loop_dirty = True
         # phases in lock-step over the shards: nobody waits on the host for a peer that has not been enqueued
         for e in self.engines:
-            e.loop_prepare(per_dev[e.dev])
-        if not all(e.loop_ready() for e in self.engines):
+            e.loop_prepare(per_dev[e.dev], record_best)
+        if not all(e.loop_ready(record_best) for e in self.engines):
             for e in self.engines:
-                e.loop_eager()
+                e.loop_eager(record_best)
             k -= 1
             for e in self.engines:
-                e.loop_capture()
+                e.loop_capture(record_best)
         for _ in range(k):
             for e in self.engines:
-                e.loop_replay(1)
+                e.loop_replay(1, record_best)
 
     def history(self):
         """(idx, q, tie) arrays of the device-loop steps so far (the last HIST_CAP of them); also mirrors them into the
@@ -354,6 +356,18 @@ class CODA(ModelSelector):
             self._hist_seen = n
         self._loop_dirty = False
         return idx, q, tie
+
+    def best_history(self):
+        """(best, best_tie) of the device-loop steps so far: the model ``get_best_model_prediction()`` returns after
+        each step (-1 for a step run without ``record_best``), and ``best_tie``, always 0 (the best model is
+        torch.argmax's first index, coda.py:346, in the reference too).  Also does what ``history()`` does."""
+        idx, _q, _tie = self.history()
+        n = len(idx)
+        e = self.engine
+        hb = getattr(e, "hist_best", None)
+        with e._on():
+            best = hb[:n].cpu().numpy() if hb is not None else np.full(n, -1, np.int32)
+        return best, np.zeros(n, np.int32)
 
     # -- checkpoint / resume (SURVEY.md 8f rank 4; the reference restarts a killed seed from step 0) ------
     def state_dict(self):

@@ -342,6 +342,10 @@ int coda_b200_step_label(const coda_step_t* st, const coda_xchg_t* x, coda_strea
 /* pi_hat (coda.py:232-233; the shards' sums are exchanged and added here), P(best) vector m0 == get_pbest()
  * (coda.py:253, 325-332), H_before (coda.py:254) and argmax (coda.py:346). */
 int coda_b200_step_mixture(const coda_step_t* st, const coda_xchg_t* x, coda_stream_t stream);
+/* One thread: hist_best[(*step_ctr - 1) % hist_cap] = *best_model, the best model (coda.py:334-346) after the step
+ * step_select counted.  Enqueued after step_mixture by the device loop that records the per-step best models. */
+int coda_b200_record_best(const int64_t* best_model, const int64_t* step_ctr, int32_t* hist_best, int64_t hist_cap,
+                          coda_stream_t stream);
 
 /* tie scan (coda.py:307 torch.isclose(q, best, rtol=1e-8[, atol=1e-8]) in fp32) against the global record. */
 int coda_b200_ties(const float* eig, int64_t N, const uint8_t* labeled, const uint8_t* disagree, int64_t n_offset,
@@ -413,6 +417,70 @@ int coda_b200_weighted_draw_xchg(const float* w, const uint8_t* labeled, int64_t
  * record slot (2 * H * 2 + 64 bytes: an H-float vector does).  x == NULL or world 1: src is copied to dst. */
 int coda_b200_owner_share(const void* src, int bytes, int own, void* dst, const coda_xchg_t* x, uint32_t* flags,
                           coda_stream_t stream);
+
+/* ---- Host-free loop of the competing selectors (one captured graph per step and shard) ----------------------------
+ * Every per-step scalar lives in device memory, so one graph serves every step.  Loop words `ls` (int64, per shard,
+ * identical on every shard):
+ *   ls[0] labels so far (global), ls[1] steps done in this run, ls[2] stop word (0 = running, 1 = VMA's weights fell
+ *   below 1e-12, 2 = ActiveTesting's total is not > 0, 3 = no item was picked), ls[3] the k of this step's k-th tie,
+ *   ls[4] 1 when this step's item was drawn among several exact ties, ls[5] device-loop steps ever (history slot),
+ *   ls[6] the 64-bit Philox key, ls[7] unlabeled items some model disagrees on (ModelPicker), ls[8] this step's u
+ *   (the bits of a double).  Once ls[2] is set every kernel below returns at once.
+ * Tie draws: Philox4x32-10 (curand_Philox4x32_10), key = ls[6], counter = {label count at the draw, purpose (0 = item
+ * tie, 1 = best-model tie), 0, 0}; the item tie is drawn before the step's label is added, the best-model tie after it;
+ * the j-th tie in ascending index order is taken, j = (uint64)r.x * count >> 32. */
+#define CODA_B200_BL_IID 0
+#define CODA_B200_BL_UNCERTAINTY 1
+#define CODA_B200_BL_ACTIVETESTING 2
+#define CODA_B200_BL_VMA 3
+#define CODA_B200_BL_MODELPICKER 4
+
+typedef struct coda_bl_loop { /* host struct: one shard of a competing selector's device loop */
+  int method;                 /* CODA_B200_BL_* */
+  int H;
+  int64_t N, n_offset, n_global;
+  const uint16_t* hard;       /* [N][H] this shard's hard predictions */
+  const uint8_t* disagree;    /* [N] (ModelPicker) */
+  uint8_t* labeled;           /* [N] */
+  const int64_t* labels;      /* [n_global] the oracle's labels on this shard's device */
+  const double* pre;          /* [steps] pre-drawn per step: IID position among the unlabeled items, AT / VMA u */
+  int64_t* ls;                /* [16] loop words, see above */
+  const int64_t* best;        /* select_extreme_xchg out [4] */
+  const int64_t* pick;        /* select_kth_xchg out [1] (IID, Uncertainty, ModelPicker) / weighted_draw out [3] */
+  const double* total;        /* weighted_total_xchg total [2] (AT / VMA) */
+  int32_t* counts;            /* [H] loss counts (IID, Uncertainty) / correct counts (ModelPicker) */
+  double* s1;                 /* [H] LURE sum_m L_m (AT / VMA) */
+  double* s2;                 /* [H] LURE sum_m L_m a_m / (N - m) */
+  float* post;                /* [H] ModelPicker posterior */
+  float gamma;                /* ModelPicker gamma as fp32 */
+  int64_t hist_cap;
+  int64_t* hist_idx;          /* [hist_cap] rings, slot = ls[5] % hist_cap */
+  double* hist_q;
+  int32_t* hist_tie;
+  int32_t* hist_best;
+  int32_t* hist_best_tie;
+  uint8_t* hist_loss;         /* [hist_cap][H] the step's loss bits (AT / VMA), may be NULL otherwise */
+  uint32_t* flags;
+} coda_bl_loop_t;
+
+/* select_kth_xchg with k = *k read on the device; nothing (no exchange either) when *stop != 0 */
+int coda_b200_select_kth_xchg_dev(const float* v, const uint8_t* labeled, int64_t N, const int64_t* partials,
+                                  const int64_t* best, const int64_t* k, const int64_t* stop, int64_t n_offset,
+                                  int64_t* out_idx, const coda_xchg_t* x, uint32_t* flags, coda_stream_t stream);
+/* weighted_draw_xchg with u = *u read on the device; nothing (no exchange either) when *stop != 0 */
+int coda_b200_weighted_draw_xchg_dev(const float* w, const uint8_t* labeled, int64_t N, const double* total,
+                                     const double* u, const int64_t* stop, int64_t n_offset, double* partials,
+                                     int64_t* out, const coda_xchg_t* x, uint32_t* flags, coda_stream_t stream);
+/* mp_entropy with mask_agreeing = (*n_disagree > 0) read on the device */
+int coda_b200_mp_entropy_dev(const uint16_t* hard, const float* posterior, int H, int64_t N, int C, double gamma,
+                             const uint8_t* labeled, const uint8_t* disagree, const int64_t* n_disagree, float* ent,
+                             coda_stream_t stream);
+/* One thread: this step's k (IID: the pre-drawn position; Uncertainty / ModelPicker: a Philox draw among best[1]
+ * ties, 0 for one tie) or u (AT / VMA: the pre-drawn u, after the stop checks on total[0] as fp32). */
+int coda_b200_bl_draw(const coda_bl_loop_t* a, coda_stream_t stream);
+/* One CTA: the step's item and q, its label, the labeled mark, the owner's hard row to every shard (record channel),
+ * the method's sums, the best model, the history slots, then the counters advance. */
+int coda_b200_bl_step(const coda_bl_loop_t* a, const coda_xchg_t* x, coda_stream_t stream);
 
 #ifdef __cplusplus
 }

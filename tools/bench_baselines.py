@@ -1,8 +1,13 @@
-"""Steps/s of one competing selector (coda_b200.baselines), one JSON line on stdout.
+"""Steps/s of one competing selector (coda_b200.baselines) or of CODA, one JSON line on stdout.
 
-    python tools/bench_baselines.py --method {iid,uncertainty,activetesting,vma,model_picker} [--steps 100] [--warmup 10]
-        [--shards S] [--gpus G] [--compact K]
+    python tools/bench_baselines.py --method {iid,uncertainty,activetesting,vma,model_picker,coda} [--steps 100] [--warmup 10]
+        [--shards S] [--gpus G] [--compact K] [--loop {api,device}]
     python -m torch.distributed.run --nproc-per-node 8 tools/bench_baselines.py --method model_picker --N 1000000
+
+--loop device times ``run_steps`` (one CUDA-graph replay per step and shard, the oracle's labels on the device) instead
+of the public API loop, and reports the final and cumulative regret of the timed steps from ``best_history()`` and the
+true accuracy losses of the models (Oracle.true_losses).  Not under torchrun.  --method coda runs CODA with its default
+arguments; its device loop is ``run_steps(..., record_best=True)``, the graph that also records each step's best model.
 
 --shards / --gpus split the task over in-process N-range shards (shards may share a GPU); under torchrun every rank
 holds its own N-range and rank 0 prints the line.  --compact K generates the task directly as a top-K compact slab
@@ -24,7 +29,7 @@ import time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 METHODS = {"iid": "IID", "uncertainty": "Uncertainty", "activetesting": "ActiveTesting", "vma": "VMA",
-           "model_picker": "ModelPicker"}
+           "model_picker": "ModelPicker", "coda": "CODA"}
 
 
 def main():
@@ -40,6 +45,7 @@ def main():
     ap.add_argument("--shards", type=int, default=None, help="in-process N-range shards (default: one)")
     ap.add_argument("--gpus", type=int, default=None, help="GPUs the in-process shards are spread over")
     ap.add_argument("--compact", type=int, default=0, metavar="K", help="top-K compact slab instead of a dense one")
+    ap.add_argument("--loop", choices=["api", "device"], default="api", help="public API loop or run_steps")
     args = ap.parse_args()
     if args.steps + args.warmup >= args.N:
         raise SystemExit("bench_baselines: steps + warmup must stay below the number of items")
@@ -69,7 +75,7 @@ def main():
     cls = getattr(coda_b200, METHODS[args.method])
     kw = dict(shards=args.shards, gpus=args.gpus)
     t = time.time()
-    sel = cls(ds, **kw) if args.method == "model_picker" else cls(ds, LOSS_FNS["acc"], **kw)
+    sel = cls(ds, **kw) if args.method in ("model_picker", "coda") else cls(ds, LOSS_FNS["acc"], **kw)
     torch.cuda.synchronize()
     t_init = time.time() - t
 
@@ -78,25 +84,50 @@ def main():
         sel.add_label(idx, int(labels[idx]), q)
         return int(sel.get_best_model_prediction())
 
-    for _ in range(args.warmup):
-        step()
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    for _ in range(args.steps):
-        step()
-    torch.cuda.synchronize()
-    ms = (time.perf_counter() - t) * 1e3 / args.steps
+    regret = None
+    if args.loop == "device":
+        labels_dev = ds.labels_host.to(dev)
+        loop_kw = dict(record_best=True) if args.method == "coda" else dict(seed=args.seed)
+        sel.run_steps(args.warmup, labels_dev, **loop_kw)
+        torch.cuda.synchronize()
+        t = time.perf_counter()
+        sel.run_steps(args.steps, labels_dev, **loop_kw)
+        torch.cuda.synchronize()
+        ms = (time.perf_counter() - t) * 1e3 / args.steps
+        best, _ties = sel.best_history()
+        # [N][H] arg-max class of every model (the slab scan)
+        hard = sel._cat("hard") if args.method == "coda" else sel.hard
+        true_losses = torch.zeros(H, dtype=torch.float64, device=dev)
+        for lo in range(0, hard.shape[0], 65536):         # accuracy loss of every model over all items
+            h = hard[lo:lo + 65536].to(torch.int64) & 0xFFFF
+            true_losses += (h != labels_dev[lo:lo + 65536, None]).sum(0).double()
+        true_losses = (true_losses / hard.shape[0]).cpu().numpy()
+        r = true_losses[best[args.warmup:]] - true_losses.min()
+        regret = {"final": float(r[-1]), "cumulative": float(r.sum())}
+    else:
+        for _ in range(args.warmup):
+            step()
+        torch.cuda.synchronize()
+        t = time.perf_counter()
+        for _ in range(args.steps):
+            step()
+        torch.cuda.synchronize()
+        ms = (time.perf_counter() - t) * 1e3 / args.steps
     try:
         power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
                                capture_output=True, text=True, timeout=30).stdout.strip() or None
     except Exception:
         power = None
+    shards = getattr(sel, "states", None) or sel.engines
     line = {"metric": "baseline acquisition steps/sec", "method": args.method, "value": 1e3 / ms, "unit": "steps/s",
             "ms_per_step": ms, "steps": args.steps, "warmup": args.warmup, "init_s": t_init,
             "workload": dict(H=H, N=N, C=C, dense=bool(args.dense), compact_k=args.compact, seed=args.seed),
-            "shards": len(sel.states) * world, "processes": world, "gpus": len({st.dev for st in sel.states}) * world,
+            "shards": len(shards) * world, "processes": world, "gpus": len({st.dev for st in shards}) * world,
             "device": torch.cuda.get_device_name(dev), "power_limit": power,
             "loop": "public API, host oracle (main.py:91-94)"}
+    if args.loop == "device":
+        line["loop"] = "device: run_steps, one CUDA-graph replay per step and shard"
+        line["regret"] = regret
     if args.method == "model_picker":
         nbytes = 2 * H * N + 2 * N + 4 * N          # hard rows + labeled / disagree masks + entropies, per step
         line["bytes_per_step"] = nbytes

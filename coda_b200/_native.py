@@ -29,6 +29,7 @@ FLAG_XCHG_TIMEOUT = 0x80
 FLAG_NEGATIVE_PROB = 0x100
 FLAG_ROWSUM_WARN = 0x200
 FLAG_PIPELINE_TIMEOUT = 0x400
+FLAG_PREDRAW_MISMATCH = 0x800
 SLAB_F32, SLAB_F16, SLAB_BF16 = 0, 1, 2
 
 
@@ -154,6 +155,12 @@ SIGNATURES = {
     "coda_b200_mp_entropy_dev": (i32, [p, p, i32, i64, i32, f64, p, p, p, p, p]),
     "coda_b200_bl_draw": (i32, [PL, p]),
     "coda_b200_bl_step": (i32, [PL, PX, p]),
+    "coda_b200_static_records": (i32, [p, p, p, i64, i64, i32, p, p]),
+    "coda_b200_abl_draw": (i32, [p, i32, p, p]),
+    "coda_b200_abl_commit": (i32, [PS, p, p, p, i32, p, p]),
+    "coda_b200_prefilter_blocks": (i32, [i32]),
+    "coda_b200_prefilter_pick": (i32, [p, p, p, i64, i64, p, p, p, i32, i32, p, p, p]),
+    "coda_b200_prefilter_commit": (i32, [PS, p, i32, p, p, i32, p, PX, p]),
 }
 
 

@@ -1015,3 +1015,246 @@ extern "C" int coda_b200_bl_step(const coda_bl_loop_t* a, const coda_xchg_t* x, 
   CODA_LAUNCH_OK("k_bl_step");
   return CODA_B200_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------------------
+// CODA's other acquisitions in its host-free loop (include/coda_b200.h, "CODA ablations"): q='uncertainty' and
+// q='iid' (coda.py:287-295) and the --prefilter-n subsample (coda.py:215-224).  The candidates are the unlabeled
+// items some model disagrees on, all unlabeled items when there are none (coda.py:239): the exact maximum ties of the
+// disagreement bits as floats (`cand`) under select_extreme_xchg(want_max = 1).  `pre` holds the host's pre-draws,
+// one row of `width` words per step: {n_s the host predicted, then the iid k or the prefilter's sample positions};
+// lw[0] is this step's row.
+// ---------------------------------------------------------------------------------------------------------------
+#define AB_KEY_SHIFT 40                                    // prefilter record key: sample position << 40 | global item
+
+// per-block CODA records from a static score vector, in the layout of the EIG assembly's block records
+__global__ void __launch_bounds__(BL_THREADS) k_static_records(const float* __restrict__ score,
+                                                              const uint8_t* __restrict__ labeled,
+                                                              const uint8_t* __restrict__ disagree, long long N,
+                                                              long long n_offset, long long* __restrict__ partials) {
+  __shared__ float sv[2][BL_THREADS / 32], sv2[2][BL_THREADS / 32];
+  __shared__ long long si[2][BL_THREADS / 32], sc[BL_THREADS / 32];
+  Best2 A = best2_empty(), B = best2_empty();
+  long long cn = 0;
+  for (long long n = (long long)blockIdx.x * BL_THREADS + threadIdx.x; n < N; n += (long long)gridDim.x * BL_THREADS) {
+    if (labeled[n]) continue;
+    const float v = score[n];
+    best2_add(B, v, n_offset + n);
+    if (disagree[n]) {
+      best2_add(A, v, n_offset + n);
+      ++cn;
+    }
+  }
+  best2_warp(A);
+  best2_warp(B);
+  cn = warp_sum(cn);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
+    sv[0][warp] = A.v; si[0][warp] = A.i; sv2[0][warp] = A.v2;
+    sv[1][warp] = B.v; si[1][warp] = B.i; sv2[1][warp] = B.v2;
+    sc[warp] = cn;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    Best2 fa = best2_empty(), fb = best2_empty();
+    long long c = 0;
+    for (int w = 0; w < BL_THREADS / 32; ++w) {
+      best2_merge(fa, Best2{sv[0][w], si[0][w], sv2[0][w]});
+      best2_merge(fb, Best2{sv[1][w], si[1][w], sv2[1][w]});
+      c += sc[w];
+    }
+    rec_store(partials + (size_t)blockIdx.x * REC_W, fa, c, fb);
+  }
+}
+
+// the step's pick -> sel, the history slots and the counters (what step_select writes after its arg-max)
+__device__ void abl_commit(const coda_step_t& a, long long g, float q, int tie, long long* lw) {
+  const long long k = *a.step_ctr;
+  long long loc = -1;
+  int t = 0;
+  if (g >= 0 && g < (1LL << AB_KEY_SHIFT)) {
+    t = (int)a.labels_global[g];                                       // oracle(idx), coda/oracle.py:23-24
+    if (t < 0 || t >= a.C) t = 0;
+    loc = g - a.n_offset;
+    if (loc < 0 || loc >= a.N) loc = -1;
+  } else {
+    g = -1;
+    atomicOr(a.flags, CODA_B200_FLAG_NO_CANDIDATE);
+  }
+  a.sel[0] = loc;
+  a.sel[1] = t;
+  if (a.hist_idx && a.hist_cap > 0) {
+    const long long slot = k % a.hist_cap;
+    a.hist_idx[slot] = g;
+    if (a.hist_q) a.hist_q[slot] = q;
+    if (a.hist_tie) a.hist_tie[slot] = tie;
+  }
+  *a.step_ctr = k + 1;
+  lw[0] += 1;
+}
+
+__global__ void k_abl_draw(const long long* __restrict__ pre, int width, long long* __restrict__ lw) {
+  lw[1] = pre[lw[0] * width + 1];
+}
+
+// iid: the pick is the k-th candidate (random.choice over the ascending list), q = fp32(1 / n_s)
+__global__ void k_abl_commit(const coda_step_t a, const long long* __restrict__ best, const long long* __restrict__ pick,
+                             const long long* __restrict__ pre, int width, long long* __restrict__ lw) {
+  const long long n = best[1];
+  if (n != pre[lw[0] * width]) atomicOr(a.flags, CODA_B200_FLAG_PREDRAW_MISMATCH);
+  abl_commit(a, n > 0 ? pick[0] : -1, n > 0 ? (float)(1.0 / (double)n) : 0.f, n > 1 ? 1 : 0, lw);
+}
+
+// prefilter: one warp per sample position j.  The position counts the candidates of all shards in ascending index
+// order; the shard whose candidates cover it finds the selection chunk from the select_extreme_xchg partials (as
+// kth_in_chunks does), then the item inside the chunk with ballots.  Block record {bits(v), key, bits(v2), 0} over
+// the block's samples, key = j << 40 | global item: equal values go to the earliest sample position.
+__global__ void __launch_bounds__(BL_THREADS) k_prefilter_pick(const float* __restrict__ eig, const float* __restrict__ cand,
+                                                              const uint8_t* __restrict__ labeled, long long N,
+                                                              long long n_offset, const long long* __restrict__ xp,
+                                                              int nxb, const long long* __restrict__ best,
+                                                              const long long* __restrict__ pre, int width, int m,
+                                                              const long long* __restrict__ lw,
+                                                              long long* __restrict__ recs) {
+  __shared__ float sv[BL_THREADS / 32], sv2[BL_THREADS / 32];
+  __shared__ long long si[BL_THREADS / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long j = (long long)blockIdx.x * (BL_THREADS / 32) + warp;
+  const float bv = __uint_as_float((unsigned)best[0]);
+  Best2 b = best2_empty();
+  const long long p = j < m ? pre[lw[0] * width + 1 + j] - best[2] : -1;
+  if (p >= 0 && p < best[3]) {                                         // warp-uniform
+    long long base = 0;
+    int blk = -1;
+    for (int b0 = 0; b0 < nxb && blk < 0; b0 += 32) {
+      const int bb = b0 + lane;
+      long long n = 0;
+      if (bb < nxb && xp[2 * bb + 1] > 0 && __uint_as_float((unsigned)xp[2 * bb]) == bv) n = xp[2 * bb + 1];
+      const long long incl = warp_incl_scan(n, lane);
+      const unsigned hit = __ballot_sync(CODA_FULL, base + incl > p);
+      if (hit) {
+        const int l = __ffs(hit) - 1;
+        blk = b0 + l;
+        base += __shfl_sync(CODA_FULL, incl - n, l);
+      } else {
+        base += __shfl_sync(CODA_FULL, incl, 31);
+      }
+    }
+    long long r = p - base, item = -1;
+    if (blk >= 0) {
+      const long long lo = (long long)blk * BL_CHUNK, hi = min(N, lo + BL_CHUNK);
+      for (long long i0 = lo; i0 < hi; i0 += 32) {
+        const long long i = i0 + lane;
+        const unsigned bal = __ballot_sync(CODA_FULL, i < hi && !labeled[i] && cand[i] == bv);
+        const int pc = __popc(bal);
+        if (r < pc) {
+          unsigned w = bal;
+          for (long long t = 0; t < r; ++t) w &= w - 1;
+          item = i0 + __ffs(w) - 1;
+          break;
+        }
+        r -= pc;
+      }
+    }
+    if (item >= 0) best2_add(b, eig[item], (j << AB_KEY_SHIFT) | (n_offset + item));
+  }
+  if (lane == 0) { sv[warp] = b.v; si[warp] = b.i; sv2[warp] = b.v2; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    Best2 f = best2_empty();
+    for (int w = 0; w < BL_THREADS / 32; ++w) best2_merge(f, Best2{sv[w], si[w], sv2[w]});
+    long long* r = recs + (size_t)blockIdx.x * 4;
+    r[0] = (long long)__float_as_int(f.v); r[1] = f.i; r[2] = (long long)__float_as_int(f.v2); r[3] = 0;
+  }
+}
+
+// one CTA: merge the block records, exchange them (record channel), the global winner -> abl_commit.  The isclose test
+// of coda.py:307 over the sample needs only the runner-up value v2.
+__global__ void __launch_bounds__(BL_THREADS) k_prefilter_commit(const coda_step_t a, const long long* __restrict__ recs,
+                                                                int nrec, const long long* __restrict__ best,
+                                                                const long long* __restrict__ pre, int width,
+                                                                long long* __restrict__ lw, XchgView x) {
+  __shared__ __align__(16) long long stage[4];
+  if (threadIdx.x == 0) {
+    Best2 f = best2_empty();
+    for (int r = 0; r < nrec; ++r)
+      best2_merge(f, Best2{__int_as_float((int)recs[4 * r]), recs[4 * r + 1], __int_as_float((int)recs[4 * r + 2])});
+    stage[0] = (long long)__float_as_int(f.v); stage[1] = f.i; stage[2] = (long long)__float_as_int(f.v2); stage[3] = 0;
+  }
+  __syncthreads();
+  const unsigned long long ep = bl_exchange(x, bl_epoch(x), stage, 32, a.flags);
+  if (threadIdx.x == 0) {
+    Best2 g = best2_empty();
+    for (int s = 0; s < x.world; ++s) {
+      const long long* r = reinterpret_cast<const long long*>(bl_rec(x, ep, s, stage));
+      best2_merge(g, Best2{__int_as_float((int)r[0]), r[1], __int_as_float((int)r[2])});
+    }
+    if (best[1] != pre[lw[0] * width]) atomicOr(a.flags, CODA_B200_FLAG_PREDRAW_MISMATCH);
+    const bool valid = g.i != IDX_NONE;
+    abl_commit(a, valid ? (g.i & ((1LL << AB_KEY_SHIFT) - 1)) : -1, valid ? g.v : 0.f,
+               (valid && isclose_best(g.v2, g.v)) ? 1 : 0, lw);
+  }
+  bl_exchange_done(x, ep);
+}
+
+static int abl_step_ok(const coda_step_t* st, const char* what) {
+  CODA_CHECK_ARG(st && st->flags && st->sel && st->step_ctr && st->labels_global && st->N >= 1 && st->C >= 1,
+                 "%s: bad step struct", what);
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_static_records(const float* score, const uint8_t* labeled, const uint8_t* disagree, int64_t N,
+                                        int64_t n_offset, int nblocks, int64_t* partials, coda_stream_t stream) {
+  CODA_CHECK_ARG(score && labeled && disagree && partials, "static_records: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << AB_KEY_SHIFT) && n_offset >= 0 && nblocks >= 1, "static_records: bad N=%lld",
+                 (long long)N);
+  k_static_records<<<nblocks, BL_THREADS, 0, as_stream(stream)>>>(score, labeled, disagree, N, n_offset,
+                                                                  (long long*)partials);
+  CODA_LAUNCH_OK("k_static_records");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_abl_draw(const int64_t* pre, int width, int64_t* lw, coda_stream_t stream) {
+  CODA_CHECK_ARG(pre && lw && width >= 2, "abl_draw: bad arguments");
+  k_abl_draw<<<1, 1, 0, as_stream(stream)>>>((const long long*)pre, width, (long long*)lw);
+  CODA_LAUNCH_OK("k_abl_draw");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_abl_commit(const coda_step_t* st, const int64_t* best, const int64_t* pick, const int64_t* pre,
+                                    int width, int64_t* lw, coda_stream_t stream) {
+  if (int rc = abl_step_ok(st, "abl_commit")) return rc;
+  CODA_CHECK_ARG(best && pick && pre && lw && width >= 1, "abl_commit: bad arguments");
+  k_abl_commit<<<1, 1, 0, as_stream(stream)>>>(*st, (const long long*)best, (const long long*)pick,
+                                               (const long long*)pre, width, (long long*)lw);
+  CODA_LAUNCH_OK("k_abl_commit");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_prefilter_blocks(int m) { return (m + BL_THREADS / 32 - 1) / (BL_THREADS / 32); }
+
+extern "C" int coda_b200_prefilter_pick(const float* eig, const float* cand, const uint8_t* labeled, int64_t N,
+                                        int64_t n_offset, const int64_t* partials, const int64_t* best,
+                                        const int64_t* pre, int width, int m, const int64_t* lw, int64_t* recs,
+                                        coda_stream_t stream) {
+  CODA_CHECK_ARG(eig && cand && labeled && partials && best && pre && lw && recs, "prefilter_pick: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << AB_KEY_SHIFT) && n_offset >= 0 && m >= 1 && m < (1 << 23) && width == m + 1,
+                 "prefilter_pick: bad N=%lld m=%d width=%d", (long long)N, m, width);
+  k_prefilter_pick<<<coda_b200_prefilter_blocks(m), BL_THREADS, 0, as_stream(stream)>>>(
+      eig, cand, labeled, N, n_offset, (const long long*)partials, coda_b200_select_blocks(N), (const long long*)best,
+      (const long long*)pre, width, m, (const long long*)lw, (long long*)recs);
+  CODA_LAUNCH_OK("k_prefilter_pick");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_prefilter_commit(const coda_step_t* st, const int64_t* recs, int nrec, const int64_t* best,
+                                          const int64_t* pre, int width, int64_t* lw, const coda_xchg_t* x,
+                                          coda_stream_t stream) {
+  if (int rc = abl_step_ok(st, "prefilter_commit")) return rc;
+  CODA_CHECK_ARG(recs && nrec >= 1 && best && pre && lw && width >= 2, "prefilter_commit: bad arguments");
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 32, "prefilter_commit")) return rc;
+  k_prefilter_commit<<<1, BL_THREADS, 0, as_stream(stream)>>>(*st, (const long long*)recs, nrec, (const long long*)best,
+                                                              (const long long*)pre, width, (long long*)lw, xv);
+  CODA_LAUNCH_OK("k_prefilter_commit");
+  return CODA_B200_OK;
+}

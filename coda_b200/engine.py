@@ -679,6 +679,8 @@ class Engine:
             self._labels_keep = labels_dev
             self.graphs.pop("loop", None)
             self.graphs.pop("loop_best", None)
+            for key in [k for k in self.graphs if isinstance(k, tuple) and k[0] == "abl"]:
+                del self.graphs[key]
 
     def _loop_body(self):
         """select -> posterior update -> scoring pass for the next selection (one graph)."""
@@ -776,6 +778,114 @@ class Engine:
             k -= 1
             self.loop_capture(record_best)
         self.loop_replay(k, record_best)
+
+    # ---- the loop of CODA's other acquisitions (CODA.run_steps with q='uncertainty' / 'iid' or prefilter_n) ----------
+    # kind "uncertainty": block records from the static scores -> step_select (no scoring pass);
+    # kind "iid":         candidate ties -> k-th of them (pre-drawn k) -> commit -> step_label (no scoring pass);
+    # kind "prefilter":   candidate ties -> sampled positions resolved and reduced -> commit -> step_label, then the
+    #                     scoring pass for the next step.  Steps the reference takes the plain arg-max for run the
+    #                     "loop" graph above.
+    # The pre-draws of iid / prefilter (one row of `width` int64 per step, include/coda_b200.h) are replayed from a
+    # device buffer of `rows` rows that the caller refills chunk by chunk (abl_load).
+    def abl_bind(self, kind, score=None, width=0, rows=0):
+        with self._on():
+            if kind == "uncertainty":
+                if getattr(self, "abl_score", None) is None:
+                    self.abl_score = score.to(self.dev, torch.float32).contiguous()
+                return
+            if getattr(self, "abl_cand", None) is None:
+                self.abl_cand = self.disagree.to(torch.float32)
+                self.abl_xp = self._z((2 * int(self.lib.coda_b200_select_blocks(self.N)),), torch.int64)
+                self.abl_best = self._z((4,), torch.int64)
+                self.abl_pick = self._z((1,), torch.int64)
+                self.abl_lw = self._z((8,), torch.int64)
+                self.abl_pre, self.abl_width, self.abl_recs, self.abl_nrec = None, 0, None, 0
+            if self.abl_pre is None or self.abl_width != width or self.abl_pre.numel() != rows * width:
+                self.abl_pre = self._z((rows * width,), torch.int64)
+                self.abl_width = width
+                if kind == "prefilter":
+                    self.abl_nrec = int(self.lib.coda_b200_prefilter_blocks(width - 1))
+                    self.abl_recs = self._z((4 * self.abl_nrec,), torch.int64)
+                for key in [k for k in self.graphs if isinstance(k, tuple) and k[0] == "abl" and k[1] != "uncertainty"]:
+                    del self.graphs[key]
+
+    def abl_load(self, pre_host):
+        """Pre-draw rows (pinned int64, row-major) -> the device buffer; the next step reads row 0."""
+        with self._on():
+            self.abl_pre[: pre_host.numel()].copy_(pre_host, non_blocking=True)
+            self.abl_lw[0:1].zero_()
+
+    def _abl_body(self, kind, record_best):
+        s, x = self._s(), self._x()
+        if kind == "uncertainty":
+            self._call("coda_b200_static_records", _ptr(self.abl_score), _ptr(self.labeled), _ptr(self.disagree), self.N,
+                       self.n_offset, self.nblocks, _ptr(self.partials), s)
+            self._call("coda_b200_step_select", self.st, x, s)
+        else:
+            lw, pre, w = self.abl_lw, self.abl_pre, self.abl_width
+            self._call("coda_b200_select_extreme_xchg", _ptr(self.abl_cand), _ptr(self.labeled), self.N, 1,
+                       _ptr(self.abl_xp), _ptr(self.abl_best), x, _ptr(self.flags), s, n=2)
+            if kind == "iid":
+                self._call("coda_b200_abl_draw", _ptr(pre), w, _ptr(lw), s)
+                self._call("coda_b200_select_kth_xchg_dev", _ptr(self.abl_cand), _ptr(self.labeled), self.N,
+                           _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(lw[1:]), _ptr(lw[2:]), self.n_offset,
+                           _ptr(self.abl_pick), x, _ptr(self.flags), s)
+                self._call("coda_b200_abl_commit", self.st, _ptr(self.abl_best), _ptr(self.abl_pick), _ptr(pre), w,
+                           _ptr(lw), s)
+            else:
+                self._call("coda_b200_prefilter_pick", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
+                           self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw),
+                           _ptr(self.abl_recs), s)
+                self._call("coda_b200_prefilter_commit", self.st, _ptr(self.abl_recs), self.abl_nrec,
+                           _ptr(self.abl_best), _ptr(pre), w, _ptr(lw), x, s)
+            self._call("coda_b200_step_label", self.st, x, s)
+        self._post_label()
+        if kind == "prefilter":
+            self._score()
+        if record_best:
+            self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
+                       HIST_CAP, s)
+
+    # the same phases as loop_prepare / loop_ready / loop_eager / loop_capture / loop_replay
+    def abl_prepare(self, labels_dev, kind, record_best=False):
+        with self._on():
+            self._bind_labels(labels_dev)
+            if record_best and getattr(self, "hist_best", None) is None:
+                self.hist_best = torch.full((HIST_CAP,), -1, dtype=torch.int32, device=self.dev)
+            if kind == "prefilter":
+                self._score()
+
+    def abl_ready(self, kind, record_best=False) -> bool:
+        return (not self.use_graph) or self.graphs.get(("abl", kind, bool(record_best))) is not None
+
+    def abl_eager(self, kind, record_best=False):
+        with self._on():
+            self._abl_body(kind, record_best)
+
+    def abl_capture(self, kind, record_best=False):
+        key = ("abl", kind, bool(record_best))
+        with self._on():
+            _g, n = self._try_capture(key, lambda: self._abl_body(kind, record_best))
+            self.abl_launches = getattr(self, "abl_launches", {})
+            self.abl_launches[key] = n
+
+    def abl_replay(self, kind, k=1, record_best=False):
+        key = ("abl", kind, bool(record_best))
+        with self._on():
+            g = self.graphs.get(key)
+            for _ in range(k):
+                if g is None:
+                    self._abl_body(kind, record_best)
+                else:
+                    g.replay()
+            if g is not None:
+                self.counters["launches"] += k * self.abl_launches[key]
+
+    def candidate_counts(self):
+        """(unlabeled items some model disagrees on, unlabeled items) of this shard; synchronises."""
+        with self._on():
+            un = self.labeled == 0
+            return int((un & (self.disagree != 0)).sum()), int(un.sum())
 
     def _capture(self, body):
         torch.cuda.synchronize(self.dev)
@@ -913,6 +1023,9 @@ class Engine:
             raise RuntimeError("coda_b200: a shard did not arrive at an exchange within 2 s (peer crashed or not launched)")
         if flags & nat.FLAG_NO_CANDIDATE:
             raise RuntimeError("no unlabeled items left to select from")
+        if flags & nat.FLAG_PREDRAW_MISMATCH:
+            raise RuntimeError("coda_b200: a device-loop step found a candidate count other than the one its "
+                               "pre-drawn random numbers were made for; the run does not follow the API path")
         if flags & nat.FLAG_NEGATIVE_PROB:
             raise RuntimeError("Pbest(beta) normalized has negatives")                 # util.py:33-35
         if flags & nat.FLAG_RANGE_INPUT and not flags & nat.FLAG_NONFINITE_INPUT:

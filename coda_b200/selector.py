@@ -55,6 +55,26 @@ class _Unlabeled:
         return list(self)[k]
 
 
+ABL_CHUNK_WORDS = 1 << 22      # int64 words of one shard's pre-draw buffer (q='iid' / prefilter_n device loop)
+
+
+def candidate_counts(d0: int, u0: int, k: int):
+    """The candidate count n_s of each of ``k`` steps from ``d0`` unlabeled items some model disagrees on and ``u0``
+    unlabeled items: every pick removes one candidate, so n_s = d0 - s while that is > 0, then u0 - s (coda.py:239)."""
+    return [d0 - s if d0 - s > 0 else u0 - s for s in range(k)]
+
+
+def ablation_draw(kind: str, n: int, m: int = 0):
+    """The Python ``random`` draws of one step with ``n`` candidates, made with the calls of the API path, as a pre-draw
+    row: ``kind='iid'`` -> [n, k], k = ``random.choice`` over the n candidates (no draw for one candidate: the arg-max
+    of coda.py:309); ``'prefilter'`` -> [n, positions...], ``random.sample`` of ``m`` positions into the ascending
+    candidate list (called only when n > m).  ``random.choice(range(n))`` and ``random.sample(range(n), m)`` consume
+    what the same calls on an n-item list consume and return its positions."""
+    if kind == "iid":
+        return [n, random.choice(range(n)) if n > 1 else 0]
+    return [n] + random.sample(range(n), m)
+
+
 def _auto_gpus(preds) -> int:
     env = os.environ.get("CODA_B200_GPUS")
     if env:
@@ -302,13 +322,35 @@ class CODA(ModelSelector):
         return out
 
     # -- host-free loop (SURVEY.md 8f rank 2) ----------------------------------------------------
+    def _loop_refusals(self):
+        """What the device loop does not offer, raised before anything is launched."""
+        q = self.q
+        if q not in ("eig", "iid", "uncertainty"):
+            raise NotImplementedError(q)                    # coda.py:297
+        if q == "eig" and not self.prefilter_n:
+            return
+        if q != "eig" and self.prefilter_n:
+            raise NotImplementedError(f"q={q!r} together with prefilter_n")
+        if self.group.world > 1 and len(self.engines) == 1:
+            raise NotImplementedError("run_steps with q='iid' / 'uncertainty' or prefilter_n needs all items in one "
+                                      "process: build CODA with gpus=... (one process driving all GPUs) instead of one "
+                                      "process per GPU")
+        if q == "uncertainty" and self.engine.ens is None:
+            raise RuntimeError("q='uncertainty' needs the ensemble sums (CODA_B200_ENS=0 disables them)")
+
     def run_steps(self, k, labels, *, record_best=False):
         """``k`` acquisition steps with the oracle's labels resident on the device(s): main.py:89-94 without a host
         round trip (arg-max pick, first index on equal values; a step where the reference would have drawn from
         ``random.choice`` because of an isclose tie is flagged in ``history()``).  ``labels``: int64 tensor of all N
         labels.  ``record_best``: replay a graph that also records every step's best model (``best_history()``, the
         regret curve of main.py:94-103); the default graph does not.  Returns nothing; read ``history()`` /
-        ``get_pbest()`` afterwards."""
+        ``get_pbest()`` afterwards.
+
+        Runs the acquisition the selector was built with: ``q='uncertainty'`` and ``q='iid'`` (coda.py:287-295) and
+        ``prefilter_n`` (coda.py:215-224) as well as EIG.  Their Python ``random`` draws (iid's ``random.choice``, the
+        prefilter's ``random.sample``) do not depend on the data and are made on the host before the steps run, with
+        the API path's own calls (DESIGN.md §4)."""
+        self._loop_refusals()
         cache = getattr(self, "_labels_dev", None)
         if cache is None or cache[0] is not labels:
             per_dev = {}
@@ -321,6 +363,12 @@ class CODA(ModelSelector):
         per_dev = cache[1]
         if k <= 0:
             return
+        if self.q != "eig" or self.prefilter_n:
+            self._run_ablation(k, per_dev, record_best)
+            return
+        self._run_eig(k, per_dev, record_best)
+
+    def _run_eig(self, k, per_dev, record_best):
         self._loop_dirty = True
         # phases in lock-step over the shards: nobody waits on the host for a peer that has not been enqueued
         for e in self.engines:
@@ -334,6 +382,61 @@ class CODA(ModelSelector):
         for _ in range(k):
             for e in self.engines:
                 e.loop_replay(1, record_best)
+
+    def _run_ablation(self, k, per_dev, record_best):
+        """run_steps for q='uncertainty' / 'iid' / prefilter_n (engine.py, "the loop of CODA's other acquisitions")."""
+        d0 = u0 = 0
+        for e in self.engines:                              # the candidate counts once; every step removes a candidate
+            d, u = e.candidate_counts()
+            d0, u0 = d0 + d, u0 + u
+        if k > u0:
+            raise RuntimeError("no unlabeled items left to select from")
+        kind = "prefilter" if self.q == "eig" else self.q
+        if kind == "uncertainty":
+            if getattr(self, "_ens_entropy", None) is None:  # the API path's vector (see _select_ablation)
+                from .baselines import ensemble_entropy
+                self._ens_entropy = ensemble_entropy(self._cat("ens"), self.H)
+            base = self.engines[0].n_offset
+            for e in self.engines:
+                e.abl_bind(kind, score=self._ens_entropy[e.n_offset - base: e.n_offset - base + e.N])
+            self._loop_dirty = True
+            self._abl_steps(kind, k, per_dev, record_best)
+            return
+        m = int(self.prefilter_n)
+        counts = candidate_counts(d0, u0, k)
+        # iid: every step; prefilter: the steps with more disagreeing candidates than the sample (a prefix: their count
+        # falls by one per step), the rest -- the all-unlabeled fallback included -- are the plain arg-max of the EIG loop
+        drawn = k if kind == "iid" else max(0, min(k, d0 - m))
+        width = 2 if kind == "iid" else m + 1
+        rows = max(1, ABL_CHUNK_WORDS // width)
+        if drawn:
+            for e in self.engines:
+                e.abl_bind(kind, width=width, rows=rows)
+            self._loop_dirty = True
+            for s0 in range(0, drawn, rows):
+                c = min(rows, drawn - s0)
+                pre = torch.tensor([ablation_draw(kind, counts[s0 + i], m) for i in range(c)], dtype=torch.int64)
+                pre = pre.reshape(-1).pin_memory()
+                for e in self.engines:
+                    e.abl_load(pre)
+                self._abl_steps(kind, c, per_dev, record_best)
+            if kind == "prefilter" or any(n > 1 for n in counts):
+                self.stochastic = True                      # coda.py:223 / 311
+        if k > drawn:
+            self._run_eig(k - drawn, per_dev, record_best)
+
+    def _abl_steps(self, kind, k, per_dev, record_best):
+        for e in self.engines:
+            e.abl_prepare(per_dev[e.dev], kind, record_best)
+        if not all(e.abl_ready(kind, record_best) for e in self.engines):
+            for e in self.engines:
+                e.abl_eager(kind, record_best)
+            k -= 1
+            for e in self.engines:
+                e.abl_capture(kind, record_best)
+        for _ in range(k):
+            for e in self.engines:
+                e.abl_replay(kind, 1, record_best)
 
     def history(self):
         """(idx, q, tie) arrays of the device-loop steps so far (the last HIST_CAP of them); also mirrors them into the

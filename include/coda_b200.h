@@ -53,6 +53,7 @@ extern "C" {
 #define CODA_B200_FLAG_NEGATIVE_PROB 0x100u  /* util._check_prob: probability < -1e-12 (util.py:33-35) */
 #define CODA_B200_FLAG_ROWSUM_WARN 0x200u    /* util._check_prob: |row sum - 1| > 1e-4 (util.py:37-39), a warning */
 #define CODA_B200_FLAG_PIPELINE_TIMEOUT 0x400u /* a TMA / tensor-core pipeline stopped (pi_full_tc); the result is invalid */
+#define CODA_B200_FLAG_PREDRAW_MISMATCH 0x800u /* a CODA ablation step found a candidate count the host did not predict */
 
 typedef void* coda_stream_t;
 
@@ -481,6 +482,37 @@ int coda_b200_bl_draw(const coda_bl_loop_t* a, coda_stream_t stream);
 /* One CTA: the step's item and q, its label, the labeled mark, the owner's hard row to every shard (record channel),
  * the method's sums, the best model, the history slots, then the counters advance. */
 int coda_b200_bl_step(const coda_bl_loop_t* a, const coda_xchg_t* x, coda_stream_t stream);
+
+/* ---- CODA's other acquisitions in its host-free loop (q='uncertainty', q='iid', prefilter_n; coda.py:215-224, 287-295)
+ * Candidates: the unlabeled items some model disagrees on, all unlabeled items when there are none (coda.py:239); as
+ * the exact maximum ties of `cand` (the disagreement bits as 1.0f / 0.0f) under select_extreme_xchg(want_max = 1).
+ * `pre` [rows][width] int64: per step {the candidate count n_s the host predicted, then the iid position k (width 2) or
+ * the prefilter's m sample positions into the ascending candidate list (width m + 1)}; `lw` [8] int64 loop words:
+ * lw[0] this step's row of pre (advanced by the commit), lw[1] the iid k, lw[2] 0 (the stop word of
+ * select_kth_xchg_dev).  A commit whose global candidate count differs from pre's sets CODA_B200_FLAG_PREDRAW_MISMATCH.
+ * Every commit writes what step_select writes after its arg-max: sel = {local index or -1, labels_global[item]},
+ * hist_idx / hist_q / hist_tie at *step_ctr % hist_cap, then *step_ctr += 1; step_label follows. */
+/* q='uncertainty': this shard's block records (the layout of the EIG assembly's, nblocks = st->nblocks of them) from a
+ * static score vector; step_select then picks as for EIG. */
+int coda_b200_static_records(const float* score, const uint8_t* labeled, const uint8_t* disagree, int64_t N,
+                             int64_t n_offset, int nblocks, int64_t* partials, coda_stream_t stream);
+/* q='iid', one thread: lw[1] = pre[lw[0]][1] (the k of select_kth_xchg_dev). */
+int coda_b200_abl_draw(const int64_t* pre, int width, int64_t* lw, coda_stream_t stream);
+/* q='iid', one thread: item pick[0], q = fp32(1 / best[1]), hist_tie = best[1] > 1 (the reference's random.choice). */
+int coda_b200_abl_commit(const coda_step_t* st, const int64_t* best /*[4]*/, const int64_t* pick /*[1]*/,
+                         const int64_t* pre, int width, int64_t* lw, coda_stream_t stream);
+/* number of block records of prefilter_pick for m samples */
+int coda_b200_prefilter_blocks(int m);
+/* prefilter_n = m (width m + 1): each sample position -> its item on the shard that holds it (from the partials and out
+ * `best` of select_extreme_xchg over cand), eig[item]; per block a record {bits(v), j << 40 | global item, bits(v2), 0}
+ * over its samples j (the earliest sample position wins equal values, v2 = the best of the others). */
+int coda_b200_prefilter_pick(const float* eig, const float* cand, const uint8_t* labeled, int64_t N, int64_t n_offset,
+                             const int64_t* partials, const int64_t* best, const int64_t* pre, int width, int m,
+                             const int64_t* lw, int64_t* recs, coda_stream_t stream);
+/* One CTA: merge the block records, exchange them (record channel), commit the winner with q = its EIG and hist_tie =
+ * isclose(v2, v) (coda.py:307 over the sample). */
+int coda_b200_prefilter_commit(const coda_step_t* st, const int64_t* recs, int nrec, const int64_t* best,
+                               const int64_t* pre, int width, int64_t* lw, const coda_xchg_t* x, coda_stream_t stream);
 
 #ifdef __cplusplus
 }

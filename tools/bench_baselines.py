@@ -1,13 +1,14 @@
 """Steps/s of one competing selector (coda_b200.baselines) or of CODA, one JSON line on stdout.
 
     python tools/bench_baselines.py --method {iid,uncertainty,activetesting,vma,model_picker,coda} [--steps 100] [--warmup 10]
-        [--shards S] [--gpus G] [--compact K] [--loop {api,device}]
+        [--shards S] [--gpus G] [--compact K] [--loop {api,device}] [--q {eig,iid,uncertainty}] [--prefilter-n K]
     python -m torch.distributed.run --nproc-per-node 8 tools/bench_baselines.py --method model_picker --N 1000000
 
 --loop device times ``run_steps`` (one CUDA-graph replay per step and shard, the oracle's labels on the device) instead
 of the public API loop, and reports the final and cumulative regret of the timed steps from ``best_history()`` and the
 true accuracy losses of the models (Oracle.true_losses).  Not under torchrun.  --method coda runs CODA with its default
-arguments; its device loop is ``run_steps(..., record_best=True)``, the graph that also records each step's best model.
+arguments unless --q / --prefilter-n name its other acquisitions (coda.py:215-224, 287-295); its device loop is
+``run_steps(..., record_best=True)``, the graph that also records each step's best model.
 
 --shards / --gpus split the task over in-process N-range shards (shards may share a GPU); under torchrun every rank
 holds its own N-range and rank 0 prints the line.  --compact K generates the task directly as a top-K compact slab
@@ -46,7 +47,11 @@ def main():
     ap.add_argument("--gpus", type=int, default=None, help="GPUs the in-process shards are spread over")
     ap.add_argument("--compact", type=int, default=0, metavar="K", help="top-K compact slab instead of a dense one")
     ap.add_argument("--loop", choices=["api", "device"], default="api", help="public API loop or run_steps")
+    ap.add_argument("--q", choices=["eig", "iid", "uncertainty"], default="eig", help="CODA's acquisition (--method coda)")
+    ap.add_argument("--prefilter-n", type=int, default=0, help="CODA's random subsample of the candidates (--method coda)")
     args = ap.parse_args()
+    if args.method != "coda" and (args.q != "eig" or args.prefilter_n):
+        raise SystemExit("bench_baselines: --q and --prefilter-n are options of --method coda")
     if args.steps + args.warmup >= args.N:
         raise SystemExit("bench_baselines: steps + warmup must stay below the number of items")
     # stdout carries exactly one JSON line
@@ -74,6 +79,8 @@ def main():
     torch.manual_seed(0)
     cls = getattr(coda_b200, METHODS[args.method])
     kw = dict(shards=args.shards, gpus=args.gpus)
+    if args.q != "eig" or args.prefilter_n:
+        kw.update(q=args.q, prefilter_n=args.prefilter_n)
     t = time.time()
     sel = cls(ds, **kw) if args.method in ("model_picker", "coda") else cls(ds, LOSS_FNS["acc"], **kw)
     torch.cuda.synchronize()
@@ -125,6 +132,8 @@ def main():
             "shards": len(shards) * world, "processes": world, "gpus": len({st.dev for st in shards}) * world,
             "device": torch.cuda.get_device_name(dev), "power_limit": power,
             "loop": "public API, host oracle (main.py:91-94)"}
+    if "q" in kw:
+        line["coda"] = dict(q=args.q, prefilter_n=args.prefilter_n)
     if args.loop == "device":
         line["loop"] = "device: run_steps, one CUDA-graph replay per step and shard"
         line["regret"] = regret

@@ -1030,4 +1030,7 @@ class ModelPicker(_Baseline):
         return ties[torch.randint(len(ties), (1,), device=self.device)].item()
 
 
-__all__ = ["IID", "Uncertainty", "ActiveTesting", "VMA", "ModelPicker", "ensemble_entropy"]
+from .eps_search import eps_search_run_key, modelpicker_eps_search  # noqa: E402  (uses _DeviceState above)
+
+__all__ = ["IID", "Uncertainty", "ActiveTesting", "VMA", "ModelPicker", "ensemble_entropy", "modelpicker_eps_search",
+           "eps_search_run_key"]

@@ -3,47 +3,14 @@
 // disagree [N], ens [N][C]); nothing touches the slab itself.  N-range shards exchange their selection records through
 // the mailboxes of xchg.cuh (record channel), so every shard ends a selection call with the same global answer.
 #include "xchg.cuh"
-
-#include <curand_philox4x32_x.h>
-#include <limits.h>
+#include "modelpicker.cuh"
 
 #define BL_THREADS 256
 #define BL_IPT 16                              // items per thread of a selection chunk (contiguous)
 #define BL_CHUNK (BL_THREADS * BL_IPT)         // items per block of the selection kernels
 
-__device__ __forceinline__ int warp_min_int(int v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_xor_sync(CODA_FULL, v, o));
-  return v;
-}
-
-// Walks the groups of models that predict the same class for one item, in the order of each group's lowest model
-// index (a relabelling of the classes keeps the groups and therefore the order and every rounding step).  `row` is the
-// item's hard row in shared memory; for each group `fn(c, lane_bits)` is called on every lane, lane_bits = the slots
-// (h = slot * 32 + lane) of this lane that belong to the group.
-template <typename Fn>
-__device__ __forceinline__ void for_each_group(const uint16_t* row, int H, int lane, Fn fn) {
-  const int nslots = (H + 31) >> 5;
-  unsigned rem = 0;
-  for (int s = 0; s < nslots; ++s)
-    if (s * 32 + lane < H) rem |= 1u << s;
-  while (true) {
-    const int hl = rem ? (__ffs(rem) - 1) * 32 + lane : INT_MAX;
-    const int hmin = warp_min_int(hl);
-    if (hmin == INT_MAX) break;
-    const uint16_t c = row[hmin];
-    unsigned mine = 0;
-    for (unsigned r = rem; r; r &= r - 1) {
-      const int s = __ffs(r) - 1;
-      if (row[s * 32 + lane] == c) mine |= 1u << s;
-    }
-    rem &= ~mine;
-    fn(c, mine);
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// ModelPicker acquisition (modelpicker.py:58-86) in closed form over the groups Z_c of an item (see the header).
+// ModelPicker acquisition (modelpicker.py:58-86) in closed form over the groups Z_c of an item (modelpicker.cuh).
 // Block prologue: p_h and p_h log2 p_h (0 log 0 = 0) in shared memory, S and B by every warp in the same order.
 // ---------------------------------------------------------------------------------------------------------------
 // DEV: the mask switch is *mask_dev > 0 (device loop) instead of mask_agreeing
@@ -61,18 +28,12 @@ __global__ void __launch_bounds__(BL_THREADS) k_mp_entropy(const uint16_t* __res
   const int Hp = (H + 31) & ~31;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint16_t* row = reinterpret_cast<uint16_t*>(spl + H) + (size_t)warp * Hp;
-  for (int h = threadIdx.x; h < H; h += blockDim.x) {
-    const double p = (double)post[h];
-    sp[h] = p;
-    spl[h] = p > 0.0 ? p * log2(p) : 0.0;
-  }
+  for (int h = threadIdx.x; h < H; h += blockDim.x) mp_post_terms(post[h], sp[h], spl[h]);
   __syncthreads();
-  double S = 0.0, B = 0.0;
-  for (int h = lane; h < H; h += 32) { S += sp[h]; B += spl[h]; }
-  S = warp_sum(S);
-  B = warp_sum(B);
+  double S, B;
+  mp_sums(sp, spl, H, lane, S, B);
   const double gm1 = gamma - 1.0, glg = gamma * log2(gamma);
-  const double h_none = log2(S) - B / S;               // a class no model predicts: the posterior is unchanged
+  const double h_none = mp_h_none(S, B);
   const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
   for (long long n = (long long)blockIdx.x * (blockDim.x >> 5) + warp; n < N; n += nw) {
     if (labeled[n] || (mask_agreeing && !disagree[n])) {   // warp-uniform
@@ -85,19 +46,10 @@ __global__ void __launch_bounds__(BL_THREADS) k_mp_entropy(const uint16_t* __res
     double acc = 0.0;
     int K = 0;
     for_each_group(row, H, lane, [&](uint16_t, unsigned mine) {
-      double a = 0.0, q = 0.0;
-      for (unsigned r = mine; r; r &= r - 1) {
-        const int h = (__ffs(r) - 1) * 32 + lane;
-        a += sp[h];
-        q += spl[h];
-      }
-      a = warp_sum(a);
-      q = warp_sum(q);
-      const double norm = S + gm1 * a;
-      acc += log2(norm) - (B + gm1 * q + glg * a) / norm;
+      acc += mp_group_term(sp, spl, mine, lane, S, B, gm1, glg);
       ++K;
     });
-    if (lane == 0) ent[n] = (float)((acc + (double)(C - K) * h_none) / (double)C);
+    if (lane == 0) ent[n] = mp_item_entropy(acc, K, C, h_none);
     __syncwarp();
   }
 }
@@ -780,17 +732,6 @@ extern "C" int coda_b200_mp_entropy_dev(const uint16_t* hard, const float* poste
                                                                                ent);
   CODA_LAUNCH_OK("k_mp_entropy");
   return CODA_B200_OK;
-}
-
-// r.x of Philox4x32-10 at key = the 64-bit seed, counter = {label count, purpose, 0, 0}
-__device__ __forceinline__ unsigned bl_philox(long long seed, long long count, unsigned purpose) {
-  const unsigned long long k = (unsigned long long)seed;
-  return curand_Philox4x32_10(make_uint4((unsigned)count, purpose, 0u, 0u), make_uint2((unsigned)k, (unsigned)(k >> 32))).x;
-}
-// (r * cnt) >> 32 in 96-bit arithmetic: the tie j in [0, cnt) in ascending index order
-__device__ __forceinline__ long long bl_tie_pick(unsigned r, long long cnt) {
-  const unsigned long long c = (unsigned long long)cnt, lo = (unsigned long long)r * (c & 0xffffffffull);
-  return (long long)(((unsigned long long)r * (c >> 32)) + (lo >> 32));
 }
 
 #define BL_STOP_VMA_UNIFORM 1

@@ -514,6 +514,24 @@ int coda_b200_prefilter_pick(const float* eig, const float* cand, const uint8_t*
 int coda_b200_prefilter_commit(const coda_step_t* st, const int64_t* recs, int nrec, const int64_t* best,
                                const int64_t* pre, int width, int64_t* lw, const coda_xchg_t* x, coda_stream_t stream);
 
+/* ---- ModelPicker's epsilon grid search (coda_b200/eps_search.py, DESIGN.md §5b) -------------------------------------
+ * A run (epsilon e, realisation r) is B steps of ModelPicker.run_steps(B, labels[pool[r]], seed = keys[e][r]) on the
+ * task restricted to the P items pool[r] (global item ids), bit for bit: picks[e][r][s] is the pool position labelled at
+ * step s, best[e][r][s] the best model after it, pick_tie / best_tie = 1 where either was drawn among > 1 exact ties.
+ * gammas[e] = fp32((1 - eps) / eps).  All arrays are on the current device; [E][R][B] outputs are row-major. */
+/* plan[5] = {runs per CTA, epsilon blocks, realisations per launch, dynamic shared bytes, scratch bytes} */
+int coda_b200_mp_runs_plan(int H, int E, int P, int64_t R, int B, int64_t* plan);
+/* every step of every run; one launch per `plan[2]` realisations; bit 1 of *flags: a step found no item (bad input) */
+int coda_b200_mp_runs(const uint16_t* hard, const int64_t* labels, const uint8_t* disagree, int H, int C,
+                      const int64_t* pool, int64_t R, int P, int B, const float* gammas, const int64_t* keys, int E,
+                      void* scratch, size_t scratch_bytes, int32_t* picks, int32_t* best, uint8_t* pick_tie,
+                      uint8_t* best_tie, uint32_t* flags, coda_stream_t stream);
+/* labels[n] = the class most models predict for item n, the smallest class id among equal counts */
+int coda_b200_majority(const uint16_t* hard, int H, int64_t N, int64_t* labels, coda_stream_t stream);
+/* acc[r][h] = number of pool positions p with hard[pool[r][p]][h] == labels[pool[r][p]] */
+int coda_b200_pool_accuracy(const uint16_t* hard, const int64_t* labels, int H, const int64_t* pool, int64_t R, int P,
+                            int32_t* acc, coda_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

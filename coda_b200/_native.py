@@ -161,6 +161,16 @@ SIGNATURES = {
     "coda_b200_prefilter_blocks": (i32, [i32]),
     "coda_b200_prefilter_pick": (i32, [p, p, p, i64, i64, p, p, p, i32, i32, p, p, p]),
     "coda_b200_prefilter_commit": (i32, [PS, p, i32, p, p, i32, p, PX, p]),
+    "coda_b200_step_select_defer": (i32, [PS, PX, p, p]),
+    "coda_b200_step_label_if": (i32, [PS, PX, p, p]),
+    "coda_b200_tie_band": (i32, [p, p, p, i64, p, p, p, p]),
+    "coda_b200_tie_draw": (i32, [PS, p, p, p, p, p, p, PX, p]),
+    "coda_b200_pf_sample": (i32, [p, p, i32, i64, p, p, p, p, p, p]),
+    "coda_b200_prefilter_commit_defer": (i32, [PS, p, i32, p, p, i32, p, p, PX, p]),
+    "coda_b200_pf_band": (i32, [p, p, p, i64, i64, p, p, p, i32, i32, p, p, p, p]),
+    "coda_b200_pf_tie_max_m": (i32, [i32]),
+    "coda_b200_pf_tie_draw": (i32, [PS, p, i32, p, p, p, p, PX, p]),
+    "coda_b200_pyrandom_run": (i32, [p, p, i32, p, p, p, p]),
     "coda_b200_mp_runs_plan": (i32, [i32, i32, i32, i64, i32, p]),
     "coda_b200_mp_runs": (i32, [p, p, p, i32, i32, p, i64, i32, i32, p, p, i32, p, sz, p, p, p, p, p, p]),
     "coda_b200_majority": (i32, [p, i32, i64, p, p]),

@@ -4,6 +4,7 @@
 // the mailboxes of xchg.cuh (record channel), so every shard ends a selection call with the same global answer.
 #include "xchg.cuh"
 #include "modelpicker.cuh"
+#include "pyrandom.cuh"
 
 #define BL_THREADS 256
 #define BL_IPT 16                              // items per thread of a selection chunk (contiguous)
@@ -312,11 +313,12 @@ __global__ void __launch_bounds__(BL_THREADS) k_extreme_blocks(const float* __re
   }
 }
 
-// One block: the k-th (ascending index) unlabeled item whose value equals best[0].  Only blocks whose partial value is
-// the best hold such items, so the partials locate the chunk without another pass over the vector.
+// One block: the k-th (ascending index) item i with in(i).  Only blocks whose partial is {bv, count > 0} hold such
+// items, so the partials locate the chunk without another pass over the vector.
 // Every thread of the block calls it; returns the item (to every thread), -1 if there is none.
-__device__ long long kth_in_chunks(const float* __restrict__ v, const uint8_t* __restrict__ labeled, long long N,
-                                   const long long* __restrict__ partials, int nblocks, float bv, long long k) {
+template <class Pred>
+__device__ long long kth_in_chunks_if(const Pred& in, long long N, const long long* __restrict__ partials, int nblocks,
+                                      float bv, long long k) {
   __shared__ long long shc[BL_THREADS / 32];
   __shared__ int s_blk;
   __shared__ long long s_k, s_out;
@@ -338,16 +340,28 @@ __device__ long long kth_in_chunks(const float* __restrict__ v, const uint8_t* _
   if (blk >= 0) {                                            // block-uniform
     const long long lo = min(N, (long long)blk * BL_CHUNK + (long long)threadIdx.x * BL_IPT), hi = min(N, lo + BL_IPT);
     long long cnt = 0;
-    for (long long i = lo; i < hi; ++i) cnt += (!labeled[i] && v[i] == bv);
+    for (long long i = lo; i < hi; ++i) cnt += in(i);
     long long tot;
     long long r = s_k - block_excl_scan(cnt, shc, tot);
     if (r >= 0 && r < cnt) {
       for (long long i = lo; i < hi; ++i)
-        if (!labeled[i] && v[i] == bv && r-- == 0) { s_out = i; break; }
+        if (in(i) && r-- == 0) { s_out = i; break; }
     }
   }
   __syncthreads();
   return s_out;
+}
+// the unlabeled items whose value equals bv: the chunks of k_extreme_blocks
+struct EqualTo {
+  const float* __restrict__ v;
+  const uint8_t* __restrict__ labeled;
+  float bv;
+  __device__ __forceinline__ bool operator()(long long i) const { return !labeled[i] && v[i] == bv; }
+};
+__device__ __forceinline__ long long kth_in_chunks(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
+                                                   long long N, const long long* __restrict__ partials, int nblocks,
+                                                   float bv, long long k) {
+  return kth_in_chunks_if(EqualTo{v, labeled, bv}, N, partials, nblocks, bv, k);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1045,24 +1059,14 @@ __global__ void k_abl_commit(const coda_step_t a, const long long* __restrict__ 
   abl_commit(a, n > 0 ? pick[0] : -1, n > 0 ? (float)(1.0 / (double)n) : 0.f, n > 1 ? 1 : 0, lw);
 }
 
-// prefilter: one warp per sample position j.  The position counts the candidates of all shards in ascending index
-// order; the shard whose candidates cover it finds the selection chunk from the select_extreme_xchg partials (as
-// kth_in_chunks does), then the item inside the chunk with ballots.  Block record {bits(v), key, bits(v2), 0} over
-// the block's samples, key = j << 40 | global item: equal values go to the earliest sample position.
-__global__ void __launch_bounds__(BL_THREADS) k_prefilter_pick(const float* __restrict__ eig, const float* __restrict__ cand,
-                                                              const uint8_t* __restrict__ labeled, long long N,
-                                                              long long n_offset, const long long* __restrict__ xp,
-                                                              int nxb, const long long* __restrict__ best,
-                                                              const long long* __restrict__ pre, int width, int m,
-                                                              const long long* __restrict__ lw,
-                                                              long long* __restrict__ recs) {
-  __shared__ float sv[BL_THREADS / 32], sv2[BL_THREADS / 32];
-  __shared__ long long si[BL_THREADS / 32];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long j = (long long)blockIdx.x * (BL_THREADS / 32) + warp;
+// one warp: the item (local index) of sample position j if this shard holds it, else -1 (warp-uniform)
+__device__ __forceinline__ long long pf_item(const float* __restrict__ cand, const uint8_t* __restrict__ labeled,
+                                             long long N, const long long* __restrict__ xp, int nxb,
+                                             const long long* __restrict__ best, const long long* __restrict__ pre,
+                                             int width, int m, const long long* __restrict__ lw, long long j, int lane) {
   const float bv = __uint_as_float((unsigned)best[0]);
-  Best2 b = best2_empty();
   const long long p = j < m ? pre[lw[0] * width + 1 + j] - best[2] : -1;
+  long long item = -1;
   if (p >= 0 && p < best[3]) {                                         // warp-uniform
     long long base = 0;
     int blk = -1;
@@ -1080,7 +1084,7 @@ __global__ void __launch_bounds__(BL_THREADS) k_prefilter_pick(const float* __re
         base += __shfl_sync(CODA_FULL, incl, 31);
       }
     }
-    long long r = p - base, item = -1;
+    long long r = p - base;
     if (blk >= 0) {
       const long long lo = (long long)blk * BL_CHUNK, hi = min(N, lo + BL_CHUNK);
       for (long long i0 = lo; i0 < hi; i0 += 32) {
@@ -1096,8 +1100,28 @@ __global__ void __launch_bounds__(BL_THREADS) k_prefilter_pick(const float* __re
         r -= pc;
       }
     }
-    if (item >= 0) best2_add(b, eig[item], (j << AB_KEY_SHIFT) | (n_offset + item));
   }
+  return item;
+}
+
+// prefilter: one warp per sample position j.  The position counts the candidates of all shards in ascending index
+// order; the shard whose candidates cover it finds the selection chunk from the select_extreme_xchg partials (as
+// kth_in_chunks does), then the item inside the chunk with ballots.  Block record {bits(v), key, bits(v2), 0} over
+// the block's samples, key = j << 40 | global item: equal values go to the earliest sample position.
+__global__ void __launch_bounds__(BL_THREADS) k_prefilter_pick(const float* __restrict__ eig, const float* __restrict__ cand,
+                                                              const uint8_t* __restrict__ labeled, long long N,
+                                                              long long n_offset, const long long* __restrict__ xp,
+                                                              int nxb, const long long* __restrict__ best,
+                                                              const long long* __restrict__ pre, int width, int m,
+                                                              const long long* __restrict__ lw,
+                                                              long long* __restrict__ recs) {
+  __shared__ float sv[BL_THREADS / 32], sv2[BL_THREADS / 32];
+  __shared__ long long si[BL_THREADS / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long j = (long long)blockIdx.x * (BL_THREADS / 32) + warp;
+  Best2 b = best2_empty();
+  const long long item = pf_item(cand, labeled, N, xp, nxb, best, pre, width, m, lw, j, lane);
+  if (item >= 0) best2_add(b, eig[item], (j << AB_KEY_SHIFT) | (n_offset + item));
   if (lane == 0) { sv[warp] = b.v; si[warp] = b.i; sv2[warp] = b.v2; }
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -1110,10 +1134,14 @@ __global__ void __launch_bounds__(BL_THREADS) k_prefilter_pick(const float* __re
 
 // one CTA: merge the block records, exchange them (record channel), the global winner -> abl_commit.  The isclose test
 // of coda.py:307 over the sample needs only the runner-up value v2.
+// DEFER (tie_rule="reference"): a winner with an isclose runner-up is not committed; *pending = 1 and lw[4] = bits(v)
+// instead (pf_band / pf_tie_draw finish the step); otherwise *pending = 0.
+template <bool DEFER>
 __global__ void __launch_bounds__(BL_THREADS) k_prefilter_commit(const coda_step_t a, const long long* __restrict__ recs,
                                                                 int nrec, const long long* __restrict__ best,
                                                                 const long long* __restrict__ pre, int width,
-                                                                long long* __restrict__ lw, XchgView x) {
+                                                                long long* __restrict__ lw, XchgView x,
+                                                                long long* __restrict__ pending) {
   __shared__ __align__(16) long long stage[4];
   if (threadIdx.x == 0) {
     Best2 f = best2_empty();
@@ -1131,8 +1159,12 @@ __global__ void __launch_bounds__(BL_THREADS) k_prefilter_commit(const coda_step
     }
     if (best[1] != pre[lw[0] * width]) atomicOr(a.flags, CODA_B200_FLAG_PREDRAW_MISMATCH);
     const bool valid = g.i != IDX_NONE;
-    abl_commit(a, valid ? (g.i & ((1LL << AB_KEY_SHIFT) - 1)) : -1, valid ? g.v : 0.f,
-               (valid && isclose_best(g.v2, g.v)) ? 1 : 0, lw);
+    const int tie = (valid && isclose_best(g.v2, g.v)) ? 1 : 0;
+    if constexpr (DEFER) {
+      *pending = tie;
+      lw[4] = (long long)__float_as_int(g.v);
+    }
+    if (!DEFER || !tie) abl_commit(a, valid ? (g.i & ((1LL << AB_KEY_SHIFT) - 1)) : -1, valid ? g.v : 0.f, tie, lw);
   }
   bl_exchange_done(x, ep);
 }
@@ -1194,8 +1226,350 @@ extern "C" int coda_b200_prefilter_commit(const coda_step_t* st, const int64_t* 
   CODA_CHECK_ARG(recs && nrec >= 1 && best && pre && lw && width >= 2, "prefilter_commit: bad arguments");
   XchgView xv;
   if (int rc = bl_view(x, &xv, 32, "prefilter_commit")) return rc;
-  k_prefilter_commit<<<1, BL_THREADS, 0, as_stream(stream)>>>(*st, (const long long*)recs, nrec, (const long long*)best,
-                                                              (const long long*)pre, width, (long long*)lw, xv);
+  k_prefilter_commit<false><<<1, BL_THREADS, 0, as_stream(stream)>>>(*st, (const long long*)recs, nrec,
+                                                                     (const long long*)best, (const long long*)pre,
+                                                                     width, (long long*)lw, xv, nullptr);
   CODA_LAUNCH_OK("k_prefilter_commit");
+  return CODA_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// tie_rule="reference" (include/coda_b200.h, "isclose ties from Python's random"): where the reference breaks an
+// isclose tie with random.choice (coda.py:306-311), the loop draws the same _randbelow from a device replica of the
+// Python generator (pyrandom.cuh) and takes that item.  The deferring select / prefilter commit leave such a step
+// pending (lw[3] for the prefilter, any word for the select); the kernels below exit at once on every other step.
+// ---------------------------------------------------------------------------------------------------------------
+// the isclose band of the global winner among the candidates (the predicate and `useA` fallback of k_ties)
+struct TieBand {
+  const float* __restrict__ v;
+  const uint8_t* __restrict__ labeled;
+  const uint8_t* __restrict__ disagree;
+  bool useA;
+  float bv;
+  __device__ __forceinline__ bool operator()(long long i) const {
+    return !labeled[i] && (!useA || disagree[i]) && isclose_best(v[i], bv);
+  }
+};
+__device__ __forceinline__ TieBand tie_band_of(const float* v, const uint8_t* labeled, const uint8_t* disagree,
+                                               const long long* bestrec) {
+  const bool useA = bestrec[2] > 0;                                   // coda.py:239 `or` fallback
+  return TieBand{v, labeled, disagree, useA, __int_as_float((int)(useA ? bestrec[0] : bestrec[3]))};
+}
+
+// per selection chunk {bits(bv), band items in it}: the partial layout of select_extreme_xchg
+__global__ void __launch_bounds__(BL_THREADS) k_tie_band(const float* __restrict__ v, const uint8_t* __restrict__ labeled,
+                                                        const uint8_t* __restrict__ disagree, long long N,
+                                                        const long long* __restrict__ bestrec,
+                                                        const long long* __restrict__ pending,
+                                                        long long* __restrict__ partials) {
+  if (!*pending) return;
+  __shared__ long long sh[BL_THREADS / 32];
+  const TieBand in = tie_band_of(v, labeled, disagree, bestrec);
+  const long long lo = chunk_lo(N), hi = min(N, lo + BL_IPT);
+  long long c = 0;
+  for (long long i = lo; i < hi; ++i) c += in(i);
+  c = warp_sum(c);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    long long t = 0;
+    for (int w = 0; w < BL_THREADS / 32; ++w) t += sh[w];
+    partials[2 * blockIdx.x] = (long long)__float_as_uint(in.bv);
+    partials[2 * blockIdx.x + 1] = t;
+  }
+}
+
+// one CTA: the shards' band counts (record channel) -> n; r = _randbelow(n) on every replica; the shard holding the
+// r-th band item in ascending global order finds it (kth_in_chunks_if); its index and value (second exchange) ->
+// abl_commit with hist_tie = 1
+__global__ void __launch_bounds__(BL_THREADS) k_tie_draw(const coda_step_t a, const float* __restrict__ v,
+                                                        const uint8_t* __restrict__ disagree,
+                                                        const long long* __restrict__ partials, int nblocks,
+                                                        const long long* __restrict__ pending, uint32_t* __restrict__ rng,
+                                                        long long* __restrict__ lw, XchgView x) {
+  if (!*pending) return;
+  __shared__ __align__(16) long long stage[2];
+  __shared__ long long sh[BL_THREADS / 32];
+  __shared__ uint32_t mt[PR_N];
+  __shared__ long long s_n, s_lower, s_r;
+  const TieBand in = tie_band_of(v, a.labeled, disagree, (const long long*)a.bestrec);
+  long long c = 0;
+  for (int b = threadIdx.x; b < nblocks; b += BL_THREADS) c += partials[2 * b + 1];
+  long long mine;
+  block_excl_scan(c, sh, mine);
+  if (threadIdx.x == 0) { stage[0] = mine; stage[1] = 0; }
+  __syncthreads();
+  const unsigned long long ep = bl_exchange(x, bl_epoch(x), stage, 16, a.flags);
+  if (threadIdx.x == 0) {
+    long long n = 0, lower = 0;
+    for (int s = 0; s < x.world; ++s) {
+      const long long r = reinterpret_cast<const long long*>(bl_rec(x, ep, s, stage))[0];
+      if (s < x.rank) lower += r;
+      n += r;
+    }
+    s_n = n;
+    s_lower = lower;
+  }
+  bl_exchange_done(x, ep);
+  const int pos = pr_load(rng, mt);
+  if (threadIdx.x < 32) {
+    PyRand g{mt, pos};
+    const long long r = s_n > 0 ? pr_randbelow(g, s_n) : -1;
+    if (threadIdx.x == 0) s_r = r;
+    pr_store(g, rng);
+  }
+  __syncthreads();
+  const long long k = s_r - s_lower;
+  long long i = -1;
+  if (s_r >= 0 && k >= 0 && k < mine) i = kth_in_chunks_if(in, a.N, partials, nblocks, in.bv, k);   // block-uniform
+  if (threadIdx.x == 0) {
+    stage[0] = i >= 0 ? a.n_offset + i : -1;
+    stage[1] = i >= 0 ? (long long)__float_as_int(v[i]) : 0;
+  }
+  __syncthreads();
+  const unsigned long long ep2 = bl_exchange(x, ep + 1, stage, 16, a.flags);
+  if (threadIdx.x == 0) {
+    long long g = -1;
+    float q = 0.f;
+    for (int s = 0; s < x.world; ++s) {
+      const long long* r = reinterpret_cast<const long long*>(bl_rec(x, ep2, s, stage));
+      if (r[0] >= 0) { g = r[0]; q = __int_as_float((int)r[1]); }
+    }
+    abl_commit(a, g, q, 1, lw);
+  }
+  bl_exchange_done(x, ep2);
+}
+
+// prefilter: this step's sample row {n_s, random.sample(range(n_s), m)} into pre row 0, lw[0] = 0 (then prefilter_pick
+// as with the host's rows).  n_s <= m means the host predicted a sampled step the device does not see: flagged.
+__global__ void __launch_bounds__(32) k_pf_sample(const long long* __restrict__ best, long long* __restrict__ pre, int m,
+                                                 long long setsize, uint32_t* __restrict__ rng, int* __restrict__ pool,
+                                                 uint32_t* __restrict__ seen, long long* __restrict__ lw,
+                                                 uint32_t* __restrict__ flags) {
+  __shared__ uint32_t mt[PR_N];
+  const long long n = best[1];
+  if (threadIdx.x == 0) { pre[0] = n; lw[0] = 0; }
+  if (n <= m) {
+    if (threadIdx.x == 0) atomicOr(flags, CODA_B200_FLAG_PREDRAW_MISMATCH);
+    return;
+  }
+  PyRand g{mt, pr_load(rng, mt)};
+  pr_sample(g, n, m, setsize, pre + 1, pool, seen);
+  pr_store(g, rng);
+}
+
+// prefilter, pending step: band_item[j] = the global item of sample position j if this shard holds it and its EIG is
+// isclose to the winner's (lw[4]), else -1
+__global__ void __launch_bounds__(BL_THREADS) k_pf_band(const float* __restrict__ eig, const float* __restrict__ cand,
+                                                       const uint8_t* __restrict__ labeled, long long N, long long n_offset,
+                                                       const long long* __restrict__ xp, int nxb,
+                                                       const long long* __restrict__ best,
+                                                       const long long* __restrict__ pre, int width, int m,
+                                                       const long long* __restrict__ lw,
+                                                       const long long* __restrict__ pending,
+                                                       long long* __restrict__ band_item) {
+  if (!*pending) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long j = (long long)blockIdx.x * (BL_THREADS / 32) + warp;
+  const long long item = pf_item(cand, labeled, N, xp, nxb, best, pre, width, m, lw, j, lane);
+  if (j < m && lane == 0)
+    band_item[j] = (item >= 0 && isclose_best(eig[item], __int_as_float((int)lw[4]))) ? n_offset + item : -1;
+}
+
+// prefilter, pending step, one CTA: the band as a bitmap over the sample positions, OR-ed over the shards (record
+// channel, one slot: m <= 8 * slot bytes), r = _randbelow(band size), the r-th band position in SAMPLE order (the
+// reference walks the sample, coda.py:306-311); its holder sends the item and its EIG -> abl_commit, hist_tie = 1
+__global__ void __launch_bounds__(BL_THREADS) k_pf_tie_draw(const coda_step_t a, const long long* __restrict__ band_item,
+                                                           int m, const long long* __restrict__ pending,
+                                                           uint32_t* __restrict__ rng, uint32_t* __restrict__ bits,
+                                                           long long* __restrict__ lw, XchgView x) {
+  if (!*pending) return;
+  __shared__ __align__(16) long long stage[2];
+  __shared__ long long sh[BL_THREADS / 32];
+  __shared__ uint32_t mt[PR_N];
+  __shared__ long long s_r, s_p;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int words = (m + 31) / 32;
+  for (int w = warp; w < words; w += BL_THREADS / 32) {
+    const int j = w * 32 + lane;
+    const unsigned bal = __ballot_sync(CODA_FULL, j < m && band_item[j] >= 0);
+    if (lane == 0) bits[w] = bal;
+  }
+  __syncthreads();
+  const unsigned long long ep = bl_epoch(x);
+  if (x.world > 1) {
+    bl_exchange(x, ep, bits, xch_align16((uint32_t)words * 4u), a.flags);
+    for (int w = threadIdx.x; w < words; w += BL_THREADS) {
+      uint32_t u = 0;
+      for (int s = 0; s < x.world; ++s) u |= reinterpret_cast<const uint32_t*>(xch_data(x, XCH_REC, ep, s))[w];
+      bits[w] = u;
+    }
+    bl_exchange_done(x, ep);
+  }
+  const int per = (words + BL_THREADS - 1) / BL_THREADS;
+  const int w0 = min(words, (int)threadIdx.x * per), w1 = min(words, w0 + per);
+  long long c = 0;
+  for (int w = w0; w < w1; ++w) c += __popc(bits[w]);
+  long long n;
+  const long long before = block_excl_scan(c, sh, n);
+  const int pos = pr_load(rng, mt);
+  if (threadIdx.x < 32) {
+    PyRand g{mt, pos};
+    const long long r = n > 0 ? pr_randbelow(g, n) : -1;
+    if (threadIdx.x == 0) { s_r = r; s_p = -1; }
+    pr_store(g, rng);
+  }
+  __syncthreads();
+  long long r = s_r - before;
+  if (s_r >= 0 && r >= 0 && r < c) {
+    for (int w = w0; w < w1; ++w) {
+      unsigned u = bits[w];
+      const int pc = __popc(u);
+      if (r < pc) {
+        for (long long t = 0; t < r; ++t) u &= u - 1;
+        s_p = (long long)w * 32 + __ffs(u) - 1;
+        break;
+      }
+      r -= pc;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const long long g = s_p >= 0 ? band_item[s_p] : -1;
+    stage[0] = g;
+    stage[1] = g >= 0 ? (long long)__float_as_int(a.eig[g - a.n_offset]) : 0;
+  }
+  __syncthreads();
+  const unsigned long long ep2 = x.world > 1 ? ep + 1 : 0;
+  bl_exchange(x, ep2, stage, 16, a.flags);
+  if (threadIdx.x == 0) {
+    long long g = -1;
+    float q = 0.f;
+    for (int s = 0; s < x.world; ++s) {
+      const long long* rr = reinterpret_cast<const long long*>(bl_rec(x, ep2, s, stage));
+      if (rr[0] >= 0) { g = rr[0]; q = __int_as_float((int)rr[1]); }
+    }
+    abl_commit(a, g, q, 1, lw);
+  }
+  bl_exchange_done(x, ep2);
+}
+
+// the kernel-level check of pyrandom.cuh: ops [nops][4] = {0, n, -, -}: _randbelow(n) -> 1 output;
+// {1, n, m, setsize}: random.sample(range(n), m) -> m outputs; outputs back to back
+__global__ void __launch_bounds__(32) k_pyrandom_run(uint32_t* __restrict__ state, const long long* __restrict__ ops,
+                                                    int nops, long long* __restrict__ out, int* __restrict__ pool,
+                                                    uint32_t* __restrict__ seen) {
+  __shared__ uint32_t mt[PR_N];
+  PyRand g{mt, pr_load(state, mt)};
+  long long o = 0;
+  for (int k = 0; k < nops; ++k) {
+    const long long* op = ops + 4 * k;
+    if (op[0] == 0) {
+      const long long r = pr_randbelow(g, op[1]);
+      if (threadIdx.x == 0) out[o] = r;
+      ++o;
+    } else {
+      pr_sample(g, op[1], (int)op[2], op[3], out + o, pool, seen);
+      o += op[2];
+    }
+  }
+  pr_store(g, state);
+}
+
+static int ref_step_ok(const coda_step_t* st, const char* what) {
+  if (int rc = abl_step_ok(st, what)) return rc;
+  CODA_CHECK_ARG(st->labeled && st->bestrec && st->eig && st->N < (1LL << AB_KEY_SHIFT), "%s: bad step struct", what);
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_tie_band(const float* v, const uint8_t* labeled, const uint8_t* disagree, int64_t N,
+                                  const int64_t* bestrec, const int64_t* pending, int64_t* partials,
+                                  coda_stream_t stream) {
+  CODA_CHECK_ARG(v && labeled && disagree && bestrec && pending && partials, "tie_band: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << AB_KEY_SHIFT), "tie_band: bad N=%lld", (long long)N);
+  k_tie_band<<<coda_b200_select_blocks(N), BL_THREADS, 0, as_stream(stream)>>>(
+      v, labeled, disagree, N, (const long long*)bestrec, (const long long*)pending, (long long*)partials);
+  CODA_LAUNCH_OK("k_tie_band");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_tie_draw(const coda_step_t* st, const float* v, const uint8_t* disagree,
+                                  const int64_t* partials, const int64_t* pending, uint32_t* rng, int64_t* lw,
+                                  const coda_xchg_t* x, coda_stream_t stream) {
+  if (int rc = ref_step_ok(st, "tie_draw")) return rc;
+  CODA_CHECK_ARG(v && disagree && partials && pending && rng && lw, "tie_draw: null pointer");
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 16, "tie_draw")) return rc;
+  k_tie_draw<<<1, BL_THREADS, 0, as_stream(stream)>>>(*st, v, disagree, (const long long*)partials,
+                                                      coda_b200_select_blocks(st->N), (const long long*)pending, rng,
+                                                      (long long*)lw, xv);
+  CODA_LAUNCH_OK("k_tie_draw");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_pf_sample(const int64_t* best, int64_t* pre, int m, int64_t setsize, uint32_t* rng,
+                                   int32_t* pool, uint32_t* seen, int64_t* lw, uint32_t* flags, coda_stream_t stream) {
+  CODA_CHECK_ARG(best && pre && rng && pool && seen && lw && flags, "pf_sample: null pointer");
+  CODA_CHECK_ARG(m >= 1 && m < (1 << 23) && setsize >= 21, "pf_sample: bad m=%d setsize=%lld", m, (long long)setsize);
+  k_pf_sample<<<1, 32, 0, as_stream(stream)>>>((const long long*)best, (long long*)pre, m, setsize, rng, pool, seen,
+                                                (long long*)lw, flags);
+  CODA_LAUNCH_OK("k_pf_sample");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_prefilter_commit_defer(const coda_step_t* st, const int64_t* recs, int nrec,
+                                                const int64_t* best, const int64_t* pre, int width, int64_t* lw,
+                                                int64_t* pending, const coda_xchg_t* x, coda_stream_t stream) {
+  if (int rc = abl_step_ok(st, "prefilter_commit_defer")) return rc;
+  CODA_CHECK_ARG(recs && nrec >= 1 && best && pre && lw && pending && width >= 2, "prefilter_commit_defer: bad arguments");
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 32, "prefilter_commit_defer")) return rc;
+  k_prefilter_commit<true><<<1, BL_THREADS, 0, as_stream(stream)>>>(*st, (const long long*)recs, nrec,
+                                                                    (const long long*)best, (const long long*)pre,
+                                                                    width, (long long*)lw, xv, (long long*)pending);
+  CODA_LAUNCH_OK("k_prefilter_commit_defer");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_pf_band(const float* eig, const float* cand, const uint8_t* labeled, int64_t N,
+                                 int64_t n_offset, const int64_t* partials, const int64_t* best, const int64_t* pre,
+                                 int width, int m, const int64_t* lw, const int64_t* pending, int64_t* band_item,
+                                 coda_stream_t stream) {
+  CODA_CHECK_ARG(eig && cand && labeled && partials && best && pre && lw && pending && band_item, "pf_band: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << AB_KEY_SHIFT) && n_offset >= 0 && m >= 1 && m < (1 << 23) && width == m + 1,
+                 "pf_band: bad N=%lld m=%d width=%d", (long long)N, m, width);
+  k_pf_band<<<coda_b200_prefilter_blocks(m), BL_THREADS, 0, as_stream(stream)>>>(
+      eig, cand, labeled, N, n_offset, (const long long*)partials, coda_b200_select_blocks(N), (const long long*)best,
+      (const long long*)pre, width, m, (const long long*)lw, (const long long*)pending, (long long*)band_item);
+  CODA_LAUNCH_OK("k_pf_band");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_pf_tie_max_m(int H) {
+  return 8 * (64 + 2 * (int)xch_align16((uint32_t)H * 2));   // the record slot (xchg_layout) as a bitmap
+}
+
+extern "C" int coda_b200_pf_tie_draw(const coda_step_t* st, const int64_t* band_item, int m, const int64_t* pending,
+                                     uint32_t* rng, uint32_t* bits, int64_t* lw, const coda_xchg_t* x,
+                                     coda_stream_t stream) {
+  if (int rc = ref_step_ok(st, "pf_tie_draw")) return rc;
+  CODA_CHECK_ARG(band_item && pending && rng && bits && lw && m >= 1 && m < (1 << 23), "pf_tie_draw: bad arguments");
+  CODA_CHECK_ARG((reinterpret_cast<uintptr_t>(bits) & 15) == 0, "pf_tie_draw: bits must be 16-byte aligned");
+  XchgView xv;
+  if (int rc = bl_view(x, &xv, 16, "pf_tie_draw")) return rc;
+  CODA_CHECK_ARG(xv.world == 1 || m <= coda_b200_pf_tie_max_m(st->H),
+                 "pf_tie_draw: prefilter_n=%d above %d, the bitmap one record slot holds at H=%d", m,
+                 coda_b200_pf_tie_max_m(st->H), st->H);
+  k_pf_tie_draw<<<1, BL_THREADS, 0, as_stream(stream)>>>(*st, (const long long*)band_item, m, (const long long*)pending,
+                                                         rng, bits, (long long*)lw, xv);
+  CODA_LAUNCH_OK("k_pf_tie_draw");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_pyrandom_run(uint32_t* state, const int64_t* ops, int nops, int64_t* out, int32_t* pool,
+                                      uint32_t* seen, coda_stream_t stream) {
+  CODA_CHECK_ARG(state && ops && out && pool && seen && nops >= 0, "pyrandom_run: bad arguments");
+  k_pyrandom_run<<<1, 32, 0, as_stream(stream)>>>(state, (const long long*)ops, nops, (long long*)out, pool, seen);
+  CODA_LAUNCH_OK("k_pyrandom_run");
   return CODA_B200_OK;
 }

@@ -677,8 +677,8 @@ class Engine:
             self.st.labels_global = labels_dev.data_ptr()
             self.labels_ptr = labels_dev.data_ptr()
             self._labels_keep = labels_dev
-            self.graphs.pop("loop", None)
-            self.graphs.pop("loop_best", None)
+            for key in ("loop", "loop_best", "loop_ref", "loop_ref_best"):
+                self.graphs.pop(key, None)
             for key in [k for k in self.graphs if isinstance(k, tuple) and k[0] == "abl"]:
                 del self.graphs[key]
 
@@ -694,7 +694,29 @@ class Engine:
         self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
                    HIST_CAP, self._s())
 
-    def _loop_key(self, record_best):
+    def _loop_body_ref(self, record_best):
+        """tie_rule="reference": the deferring select; a step it leaves pending draws its pick from the Python
+        generator's replica (_ref_tie); then the rest of the loop body."""
+        self._call("coda_b200_step_select_defer", self.st, self._x(), _ptr(self.ref_lw[3:]), self._s())
+        self._ref_tie(self.eig)
+        self._post_label()
+        self._score()
+        if record_best:
+            self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
+                       HIST_CAP, self._s())
+
+    def _ref_tie(self, v):
+        """A pending step's band of isclose candidates over score ``v`` -> _randbelow draw -> commit -> label."""
+        s, x, pend = self._s(), self._x(), _ptr(self.ref_lw[3:])
+        self._call("coda_b200_tie_band", _ptr(v), _ptr(self.labeled), _ptr(self.disagree), self.N, _ptr(self.bestrec),
+                   pend, _ptr(self.ref_xp), s)
+        self._call("coda_b200_tie_draw", self.st, _ptr(v), _ptr(self.disagree), _ptr(self.ref_xp), pend,
+                   _ptr(self.pyrng), _ptr(self.ref_lw), x, s)
+        self._call("coda_b200_step_label_if", self.st, x, pend, s)
+
+    def _loop_key(self, record_best, rule="first"):
+        if rule == "reference":
+            return ("loop_ref_best" if record_best else "loop_ref"), (lambda: self._loop_body_ref(record_best))
         return ("loop_best", self._loop_body_best) if record_best else ("loop", self._loop_body)
 
     def device_step(self, labels_dev: torch.Tensor, step: int | None = None, hist_idx=None, hist_q=None):
@@ -724,12 +746,12 @@ class Engine:
                 self.hist_best = torch.full((HIST_CAP,), -1, dtype=torch.int32, device=self.dev)
             self._score()
 
-    def loop_ready(self, record_best: bool = False) -> bool:
-        return (not self.use_graph) or self.graphs.get(self._loop_key(record_best)[0]) is not None
+    def loop_ready(self, record_best: bool = False, rule: str = "first") -> bool:
+        return (not self.use_graph) or self.graphs.get(self._loop_key(record_best, rule)[0]) is not None
 
-    def loop_eager(self, record_best: bool = False):
+    def loop_eager(self, record_best: bool = False, rule: str = "first"):
         with self._on():
-            self._loop_key(record_best)[1]()
+            self._loop_key(record_best, rule)[1]()
 
     def _try_capture(self, key, body):
         """Capture `body` as graph `key`; a failed capture (driver / allocator state) falls back to eager launches."""
@@ -745,17 +767,20 @@ class Engine:
         self.graphs[key] = g
         return g, n
 
-    def loop_capture(self, record_best: bool = False):
-        key, body = self._loop_key(record_best)
+    def loop_capture(self, record_best: bool = False, rule: str = "first"):
+        key, body = self._loop_key(record_best, rule)
         with self._on():
             _g, n = self._try_capture(key, body)
-            if record_best:
+            if rule != "first":
+                self.ref_launches = getattr(self, "ref_launches", {})
+                self.ref_launches[key] = n
+            elif record_best:
                 self.launches_per_step_best = n
             else:
                 self.launches_per_step = n
 
-    def loop_replay(self, k: int = 1, record_best: bool = False):
-        key, body = self._loop_key(record_best)
+    def loop_replay(self, k: int = 1, record_best: bool = False, rule: str = "first"):
+        key, body = self._loop_key(record_best, rule)
         with self._on():
             g = self.graphs.get(key)
             for _ in range(k):
@@ -764,7 +789,10 @@ class Engine:
                 else:
                     g.replay()
             if g is not None:
-                self.counters["launches"] += k * (self.launches_per_step_best if record_best else self.launches_per_step)
+                if rule != "first":
+                    self.counters["launches"] += k * self.ref_launches[key]
+                else:
+                    self.counters["launches"] += k * (self.launches_per_step_best if record_best else self.launches_per_step)
 
     def run_steps(self, k: int, labels_dev: torch.Tensor, record_best: bool = False):
         """``k`` acquisition steps as ``k`` replays of one captured CUDA graph (SURVEY.md 8f rank 2; replaces the
@@ -815,12 +843,33 @@ class Engine:
             self.abl_pre[: pre_host.numel()].copy_(pre_host, non_blocking=True)
             self.abl_lw[0:1].zero_()
 
-    def _abl_body(self, kind, record_best):
+    def _abl_body(self, kind, record_best, rule="first"):
         s, x = self._s(), self._x()
         if kind == "uncertainty":
             self._call("coda_b200_static_records", _ptr(self.abl_score), _ptr(self.labeled), _ptr(self.disagree), self.N,
                        self.n_offset, self.nblocks, _ptr(self.partials), s)
-            self._call("coda_b200_step_select", self.st, x, s)
+            if rule == "reference":
+                self._call("coda_b200_step_select_defer", self.st, x, _ptr(self.ref_lw[3:]), s)
+                self._ref_tie(self.abl_score)
+            else:
+                self._call("coda_b200_step_select", self.st, x, s)
+        elif rule == "reference":         # prefilter: the sample drawn on the device, ties from the same generator
+            lw, pre, w, pend = self.ref_lw, self.abl_pre, self.abl_width, _ptr(self.ref_lw[3:])
+            self._call("coda_b200_select_extreme_xchg", _ptr(self.abl_cand), _ptr(self.labeled), self.N, 1,
+                       _ptr(self.abl_xp), _ptr(self.abl_best), x, _ptr(self.flags), s, n=2)
+            self._call("coda_b200_pf_sample", _ptr(self.abl_best), _ptr(pre), w - 1, self.ref_setsize, _ptr(self.pyrng),
+                       _ptr(self.ref_pool), _ptr(self.ref_seen), _ptr(lw), _ptr(self.flags), s)
+            self._call("coda_b200_prefilter_pick", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
+                       self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw),
+                       _ptr(self.abl_recs), s)
+            self._call("coda_b200_prefilter_commit_defer", self.st, _ptr(self.abl_recs), self.abl_nrec,
+                       _ptr(self.abl_best), _ptr(pre), w, _ptr(lw), pend, x, s)
+            self._call("coda_b200_pf_band", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
+                       self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw), pend,
+                       _ptr(self.ref_band), s)
+            self._call("coda_b200_pf_tie_draw", self.st, _ptr(self.ref_band), w - 1, pend, _ptr(self.pyrng),
+                       _ptr(self.ref_bits), _ptr(lw), x, s)
+            self._call("coda_b200_step_label", self.st, x, s)
         else:
             lw, pre, w = self.abl_lw, self.abl_pre, self.abl_width
             self._call("coda_b200_select_extreme_xchg", _ptr(self.abl_cand), _ptr(self.labeled), self.N, 1,
@@ -855,31 +904,64 @@ class Engine:
             if kind == "prefilter":
                 self._score()
 
-    def abl_ready(self, kind, record_best=False) -> bool:
-        return (not self.use_graph) or self.graphs.get(("abl", kind, bool(record_best))) is not None
+    @staticmethod
+    def _abl_key(kind, record_best, rule):
+        return ("abl", kind, bool(record_best)) + (() if rule == "first" else (rule,))
 
-    def abl_eager(self, kind, record_best=False):
-        with self._on():
-            self._abl_body(kind, record_best)
+    def abl_ready(self, kind, record_best=False, rule="first") -> bool:
+        return (not self.use_graph) or self.graphs.get(self._abl_key(kind, record_best, rule)) is not None
 
-    def abl_capture(self, kind, record_best=False):
-        key = ("abl", kind, bool(record_best))
+    def abl_eager(self, kind, record_best=False, rule="first"):
         with self._on():
-            _g, n = self._try_capture(key, lambda: self._abl_body(kind, record_best))
+            self._abl_body(kind, record_best, rule)
+
+    def abl_capture(self, kind, record_best=False, rule="first"):
+        key = self._abl_key(kind, record_best, rule)
+        with self._on():
+            _g, n = self._try_capture(key, lambda: self._abl_body(kind, record_best, rule))
             self.abl_launches = getattr(self, "abl_launches", {})
             self.abl_launches[key] = n
 
-    def abl_replay(self, kind, k=1, record_best=False):
-        key = ("abl", kind, bool(record_best))
+    def abl_replay(self, kind, k=1, record_best=False, rule="first"):
+        key = self._abl_key(kind, record_best, rule)
         with self._on():
             g = self.graphs.get(key)
             for _ in range(k):
                 if g is None:
-                    self._abl_body(kind, record_best)
+                    self._abl_body(kind, record_best, rule)
                 else:
                     g.replay()
             if g is not None:
                 self.counters["launches"] += k * self.abl_launches[key]
+
+    # ---- tie_rule="reference": a replica of Python's generator on this shard (csrc/pyrandom.cuh) --------------------
+    # pyrng [625] int32 (the uint32 words of random.getstate()[1]); ref_lw [8] int64 loop words of the reference-mode
+    # kernels: [0] pre row, [3] the pending word, [4] the prefilter winner's EIG bits; ref_xp: tie_band's partials.
+    def ref_bind(self):
+        with self._on():
+            if getattr(self, "pyrng", None) is None:
+                self.pyrng = self._z((625,), torch.int32)
+                self.ref_lw = self._z((8,), torch.int64)
+                self.ref_xp = self._z((2 * int(self.lib.coda_b200_select_blocks(self.N)),), torch.int64)
+
+    def ref_bind_prefilter(self, m, setsize):
+        """Scratch of the device sampler and of the prefilter's tie draw for prefilter_n = m (abl_bind first)."""
+        with self._on():
+            if getattr(self, "ref_m", None) != (m, setsize):
+                self.ref_m, self.ref_setsize = (m, setsize), int(setsize)
+                self.ref_pool = self._z((min(int(setsize), self.n_global) + 1,), torch.int32)
+                self.ref_seen = self._z(((self.n_global + 31) // 32 + 1,), torch.int32)
+                self.ref_band = self._z((m,), torch.int64)
+                self.ref_bits = self._z(((m + 127) // 128 * 4,), torch.int32)
+
+    def rng_upload(self, words):
+        """words: CPU int32 [625] -> this shard's replica (ordered on its stream)."""
+        with self._on():
+            self.pyrng.copy_(words)
+
+    def rng_download(self):
+        with self._on():
+            return self.pyrng.cpu()
 
     def candidate_counts(self):
         """(unlabeled items some model disagrees on, unlabeled items) of this shard; synchronises."""

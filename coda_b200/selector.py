@@ -14,6 +14,7 @@ Sharding (SURVEY.md 8e), chosen at construction:
 """
 from __future__ import annotations
 
+import math
 import os
 import random
 
@@ -22,7 +23,7 @@ import torch
 
 from .base import ModelSelector
 from .dist import InProcessGroup, ProcessGroup, SoloGroup, choose_among_ties, default_comm, split_slab
-from .engine import TIE_CAP, build_engines
+from .engine import HIST_CAP, TIE_CAP, build_engines
 
 
 class _Unlabeled:
@@ -73,6 +74,25 @@ def ablation_draw(kind: str, n: int, m: int = 0):
     if kind == "iid":
         return [n, random.choice(range(n)) if n > 1 else 0]
     return [n] + random.sample(range(n), m)
+
+
+def sample_setsize(m: int) -> int:
+    """Lib/random.py's ``setsize`` of ``random.sample(population, m)``: a population of at most this many items is
+    sampled from a list (pool branch), a larger one by rejecting repeats (set branch)."""
+    setsize = 21
+    if m > 5:
+        setsize += 4 ** math.ceil(math.log(m * 3, 4))
+    return setsize
+
+
+def rng_words(state) -> torch.Tensor:
+    """random.getstate() -> the device replica's int32 [625]: the 624 MT19937 words (as uint32 bits), the position."""
+    return torch.from_numpy(np.array(state[1], dtype=np.uint32).view(np.int32).copy())
+
+
+def rng_state(words: torch.Tensor, gauss_next):
+    """The inverse of ``rng_words``: a state for random.setstate, with ``gauss_next`` as given."""
+    return (3, tuple(int(w) for w in words.numpy().view(np.uint32)), gauss_next)
 
 
 def _auto_gpus(preds) -> int:
@@ -338,7 +358,28 @@ class CODA(ModelSelector):
         if q == "uncertainty" and self.engine.ens is None:
             raise RuntimeError("q='uncertainty' needs the ensemble sums (CODA_B200_ENS=0 disables them)")
 
-    def run_steps(self, k, labels, *, record_best=False):
+    def _reference_refusals(self):
+        """What tie_rule="reference" does not offer, raised before anything is launched."""
+        if self.group.world > 1 and len(self.engines) == 1:
+            raise NotImplementedError("run_steps(tie_rule='reference') needs all items in one process: build CODA with "
+                                      "gpus=... (one process driving all GPUs) instead of one process per GPU")
+        inst = getattr(random, "_inst", None)
+        if type(inst) is not random.Random:
+            raise RuntimeError("tie_rule='reference' follows the random module's own generator, which has been "
+                               f"replaced by a {type(inst).__name__}")
+        if random.Random._randbelow is not random.Random._randbelow_with_getrandbits:
+            raise RuntimeError("tie_rule='reference' needs random.Random._randbelow to be _randbelow_with_getrandbits")
+        if self.N >= 2 ** 32:
+            raise NotImplementedError("tie_rule='reference' draws _randbelow over candidate counts below 2**32")
+        m = int(self.prefilter_n or 0)
+        if m and len(self.engines) > 1:
+            bound = int(self.engine.lib.coda_b200_pf_tie_max_m(self.H))
+            if m > bound:
+                raise NotImplementedError(f"tie_rule='reference' with {len(self.engines)} shards takes prefilter_n <= "
+                                          f"{bound} at H={self.H} (the tie draw's sample bitmap travels in one record "
+                                          f"slot); got {m}")
+
+    def run_steps(self, k, labels, *, record_best=False, tie_rule="first"):
         """``k`` acquisition steps with the oracle's labels resident on the device(s): main.py:89-94 without a host
         round trip (arg-max pick, first index on equal values; a step where the reference would have drawn from
         ``random.choice`` because of an isclose tie is flagged in ``history()``).  ``labels``: int64 tensor of all N
@@ -349,8 +390,19 @@ class CODA(ModelSelector):
         Runs the acquisition the selector was built with: ``q='uncertainty'`` and ``q='iid'`` (coda.py:287-295) and
         ``prefilter_n`` (coda.py:215-224) as well as EIG.  Their Python ``random`` draws (iid's ``random.choice``, the
         prefilter's ``random.sample``) do not depend on the data and are made on the host before the steps run, with
-        the API path's own calls (DESIGN.md §4)."""
+        the API path's own calls (DESIGN.md §4).
+
+        ``tie_rule``: which random stream the picks follow.  ``"first"`` (the default) takes the first maximum of an
+        isclose tie and only flags the step.  ``"reference"`` breaks it as coda.py:306-311 does, with ``random.choice``'s
+        draw made on the device from a replica of Python's generator; the prefilter's samples come from the same
+        replica.  Then the picks, q values, ``stochastic``, the posterior and the final ``random.getstate()`` are those
+        of ``k`` API steps.  q='iid' draws before the loop either way."""
+        if tie_rule not in ("first", "reference"):
+            raise ValueError(f"tie_rule must be 'first' or 'reference', got {tie_rule!r}")
         self._loop_refusals()
+        rule = "reference" if tie_rule == "reference" and self.q != "iid" else "first"
+        if rule == "reference":
+            self._reference_refusals()
         cache = getattr(self, "_labels_dev", None)
         if cache is None or cache[0] is not labels:
             per_dev = {}
@@ -363,27 +415,53 @@ class CODA(ModelSelector):
         per_dev = cache[1]
         if k <= 0:
             return
+        if rule == "reference":
+            self._run_reference(k, per_dev, record_best)
+            return
         if self.q != "eig" or self.prefilter_n:
             self._run_ablation(k, per_dev, record_best)
             return
         self._run_eig(k, per_dev, record_best)
 
-    def _run_eig(self, k, per_dev, record_best):
+    def _run_reference(self, k, per_dev, record_best):
+        """run_steps(tie_rule="reference"): Python's state goes to every shard's replica before the steps and comes
+        back from it after them."""
+        e0 = self.engine
+        with e0._on():
+            ctr0 = int(e0.step_ctr.item())
+        words = rng_words(random.getstate())
+        for e in self.engines:
+            e.ref_bind()
+            e.rng_upload(words)
+        if self.q == "eig" and not self.prefilter_n:
+            self._run_eig(k, per_dev, record_best, "reference")
+        else:
+            self._run_ablation(k, per_dev, record_best, "reference")
+        states = [e.rng_download() for e in self.engines]
+        if any(not torch.equal(s, states[0]) for s in states[1:]):
+            raise RuntimeError("the shards' replicas of Python's generator differ after run_steps")
+        random.setstate(rng_state(states[0], random.getstate()[2]))
+        with e0._on():
+            slots = torch.arange(ctr0, int(e0.step_ctr.item()), device=e0.dev) % HIST_CAP
+            if bool(e0.hist_tie[slots].any()):
+                self.stochastic = True                      # coda.py:311
+
+    def _run_eig(self, k, per_dev, record_best, rule="first"):
         self._loop_dirty = True
         # phases in lock-step over the shards: nobody waits on the host for a peer that has not been enqueued
         for e in self.engines:
             e.loop_prepare(per_dev[e.dev], record_best)
-        if not all(e.loop_ready(record_best) for e in self.engines):
+        if not all(e.loop_ready(record_best, rule) for e in self.engines):
             for e in self.engines:
-                e.loop_eager(record_best)
+                e.loop_eager(record_best, rule)
             k -= 1
             for e in self.engines:
-                e.loop_capture(record_best)
+                e.loop_capture(record_best, rule)
         for _ in range(k):
             for e in self.engines:
-                e.loop_replay(1, record_best)
+                e.loop_replay(1, record_best, rule)
 
-    def _run_ablation(self, k, per_dev, record_best):
+    def _run_ablation(self, k, per_dev, record_best, rule="first"):
         """run_steps for q='uncertainty' / 'iid' / prefilter_n (engine.py, "the loop of CODA's other acquisitions")."""
         d0 = u0 = 0
         for e in self.engines:                              # the candidate counts once; every step removes a candidate
@@ -400,7 +478,7 @@ class CODA(ModelSelector):
             for e in self.engines:
                 e.abl_bind(kind, score=self._ens_entropy[e.n_offset - base: e.n_offset - base + e.N])
             self._loop_dirty = True
-            self._abl_steps(kind, k, per_dev, record_best)
+            self._abl_steps(kind, k, per_dev, record_best, rule)
             return
         m = int(self.prefilter_n)
         counts = candidate_counts(d0, u0, k)
@@ -409,7 +487,14 @@ class CODA(ModelSelector):
         drawn = k if kind == "iid" else max(0, min(k, d0 - m))
         width = 2 if kind == "iid" else m + 1
         rows = max(1, ABL_CHUNK_WORDS // width)
-        if drawn:
+        if drawn and rule == "reference":                   # the device samples each step's row itself
+            for e in self.engines:
+                e.abl_bind(kind, width=width, rows=1)
+                e.ref_bind_prefilter(m, sample_setsize(m))
+            self._loop_dirty = True
+            self._abl_steps(kind, drawn, per_dev, record_best, rule)
+            self.stochastic = True                          # coda.py:223
+        elif drawn:
             for e in self.engines:
                 e.abl_bind(kind, width=width, rows=rows)
             self._loop_dirty = True
@@ -423,20 +508,20 @@ class CODA(ModelSelector):
             if kind == "prefilter" or any(n > 1 for n in counts):
                 self.stochastic = True                      # coda.py:223 / 311
         if k > drawn:
-            self._run_eig(k - drawn, per_dev, record_best)
+            self._run_eig(k - drawn, per_dev, record_best, rule)
 
-    def _abl_steps(self, kind, k, per_dev, record_best):
+    def _abl_steps(self, kind, k, per_dev, record_best, rule="first"):
         for e in self.engines:
             e.abl_prepare(per_dev[e.dev], kind, record_best)
-        if not all(e.abl_ready(kind, record_best) for e in self.engines):
+        if not all(e.abl_ready(kind, record_best, rule) for e in self.engines):
             for e in self.engines:
-                e.abl_eager(kind, record_best)
+                e.abl_eager(kind, record_best, rule)
             k -= 1
             for e in self.engines:
-                e.abl_capture(kind, record_best)
+                e.abl_capture(kind, record_best, rule)
         for _ in range(k):
             for e in self.engines:
-                e.abl_replay(kind, 1, record_best)
+                e.abl_replay(kind, 1, record_best, rule)
 
     def history(self):
         """(idx, q, tie) arrays of the device-loop steps so far (the last HIST_CAP of them); also mirrors them into the

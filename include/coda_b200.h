@@ -514,6 +514,50 @@ int coda_b200_prefilter_pick(const float* eig, const float* cand, const uint8_t*
 int coda_b200_prefilter_commit(const coda_step_t* st, const int64_t* recs, int nrec, const int64_t* best,
                                const int64_t* pre, int width, int64_t* lw, const coda_xchg_t* x, coda_stream_t stream);
 
+/* ---- isclose ties from Python's random (CODA.run_steps(..., tie_rule="reference"); coda.py:306-311) -----------------
+ * `rng` [625] uint32 on every shard: a replica of Python's generator as random.getstate()[1] holds it (624 MT19937 words,
+ * then the position); every shard advances its replica identically.  `pending` is one int64 word set by the deferring
+ * select / prefilter commit: 1 on a step whose winner has an isclose runner-up, which then commits nothing; tie_band,
+ * tie_draw, step_label_if, pf_band and pf_tie_draw return at once unless it is 1.  A tie draw commits as abl_commit
+ * does, with q = the drawn item's value and hist_tie = 1.  Candidate counts must be < 2^32 (the caller checks). */
+/* step_select (pick = 1), except that a step with an isclose tie commits nothing and sets *pending = 1 (else 0) */
+int coda_b200_step_select_defer(const coda_step_t* st, const coda_xchg_t* x, int64_t* pending, coda_stream_t stream);
+/* step_label on a pending step only */
+int coda_b200_step_label_if(const coda_step_t* st, const coda_xchg_t* x, const int64_t* pending, coda_stream_t stream);
+/* per selection chunk {bits(best), candidates isclose to bestrec's winner} (select_extreme_xchg's partial layout) over
+ * score v (the EIG vector, or q='uncertainty''s static score) */
+int coda_b200_tie_band(const float* v, const uint8_t* labeled, const uint8_t* disagree, int64_t N,
+                       const int64_t* bestrec, const int64_t* pending, int64_t* partials, coda_stream_t stream);
+/* One CTA: n = the band's global size (record channel), r = _randbelow(n), commit the r-th band item in ascending
+ * global index order */
+int coda_b200_tie_draw(const coda_step_t* st, const float* v, const uint8_t* disagree, const int64_t* partials,
+                       const int64_t* pending, uint32_t* rng, int64_t* lw, const coda_xchg_t* x, coda_stream_t stream);
+/* prefilter_n = m: pre row 0 = {n_s = best[1], random.sample(range(n_s), m)} and lw[0] = 0.  setsize: Lib/random.py's
+ * (21, plus 4 ** ceil(log(3 m, 4)) when m > 5); pool >= min(setsize, n_s) int32, seen >= ceil(n_s / 32) zero words
+ * (left zero).  n_s <= m sets CODA_B200_FLAG_PREDRAW_MISMATCH. */
+int coda_b200_pf_sample(const int64_t* best, int64_t* pre, int m, int64_t setsize, uint32_t* rng, int32_t* pool,
+                        uint32_t* seen, int64_t* lw, uint32_t* flags, coda_stream_t stream);
+/* prefilter_commit, except that a winner with an isclose runner-up is not committed: *pending = 1 (else 0), and
+ * lw[4] = bits(winner's EIG) */
+int coda_b200_prefilter_commit_defer(const coda_step_t* st, const int64_t* recs, int nrec, const int64_t* best,
+                                     const int64_t* pre, int width, int64_t* lw, int64_t* pending,
+                                     const coda_xchg_t* x, coda_stream_t stream);
+/* band_item[j] (m entries) = the global item of sample position j if this shard holds it and its EIG is isclose to
+ * lw[4], else -1 */
+int coda_b200_pf_band(const float* eig, const float* cand, const uint8_t* labeled, int64_t N, int64_t n_offset,
+                      const int64_t* partials, const int64_t* best, const int64_t* pre, int width, int m,
+                      const int64_t* lw, const int64_t* pending, int64_t* band_item, coda_stream_t stream);
+/* the largest m pf_tie_draw takes with several shards at H models: its band bitmap travels in one record slot */
+int coda_b200_pf_tie_max_m(int H);
+/* One CTA: the band bitmap over the sample positions (OR over the shards), r = _randbelow(its size), commit the r-th
+ * band position in sample order.  bits: >= ceil(m / 32) words rounded up to 16 bytes, 16-byte aligned. */
+int coda_b200_pf_tie_draw(const coda_step_t* st, const int64_t* band_item, int m, const int64_t* pending,
+                          uint32_t* rng, uint32_t* bits, int64_t* lw, const coda_xchg_t* x, coda_stream_t stream);
+/* One warp runs ops [nops][4] on the generator `state` [625] in order: {0, n, 0, 0} -> _randbelow(n) (1 <= n < 2^32),
+ * one output; {1, n, m, setsize} -> random.sample(range(n), m), m outputs.  pool / seen as for pf_sample. */
+int coda_b200_pyrandom_run(uint32_t* state, const int64_t* ops, int nops, int64_t* out, int32_t* pool, uint32_t* seen,
+                           coda_stream_t stream);
+
 /* ---- ModelPicker's epsilon grid search (coda_b200/eps_search.py, DESIGN.md §5b) -------------------------------------
  * A run (epsilon e, realisation r) is B steps of ModelPicker.run_steps(B, labels[pool[r]], seed = keys[e][r]) on the
  * task restricted to the P items pool[r] (global item ids), bit for bit: picks[e][r][s] is the pool position labelled at

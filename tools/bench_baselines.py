@@ -2,6 +2,7 @@
 
     python tools/bench_baselines.py --method {iid,uncertainty,activetesting,vma,model_picker,coda} [--steps 100] [--warmup 10]
         [--shards S] [--gpus G] [--compact K] [--loop {api,device}] [--q {eig,iid,uncertainty}] [--prefilter-n K]
+        [--tie-rule {first,reference}]
     python -m torch.distributed.run --nproc-per-node 8 tools/bench_baselines.py --method model_picker --N 1000000
 
 --loop device times ``run_steps`` (one CUDA-graph replay per step and shard, the oracle's labels on the device) instead
@@ -49,9 +50,13 @@ def main():
     ap.add_argument("--loop", choices=["api", "device"], default="api", help="public API loop or run_steps")
     ap.add_argument("--q", choices=["eig", "iid", "uncertainty"], default="eig", help="CODA's acquisition (--method coda)")
     ap.add_argument("--prefilter-n", type=int, default=0, help="CODA's random subsample of the candidates (--method coda)")
+    ap.add_argument("--tie-rule", choices=["first", "reference"], default="first",
+                    help="CODA's run_steps tie rule (--method coda --loop device)")
     args = ap.parse_args()
     if args.method != "coda" and (args.q != "eig" or args.prefilter_n):
         raise SystemExit("bench_baselines: --q and --prefilter-n are options of --method coda")
+    if args.tie_rule != "first" and (args.method != "coda" or args.loop != "device"):
+        raise SystemExit("bench_baselines: --tie-rule is an option of --method coda --loop device")
     if args.steps + args.warmup >= args.N:
         raise SystemExit("bench_baselines: steps + warmup must stay below the number of items")
     # stdout carries exactly one JSON line
@@ -94,7 +99,7 @@ def main():
     regret = None
     if args.loop == "device":
         labels_dev = ds.labels_host.to(dev)
-        loop_kw = dict(record_best=True) if args.method == "coda" else dict(seed=args.seed)
+        loop_kw = dict(record_best=True, tie_rule=args.tie_rule) if args.method == "coda" else dict(seed=args.seed)
         sel.run_steps(args.warmup, labels_dev, **loop_kw)
         torch.cuda.synchronize()
         t = time.perf_counter()
@@ -137,6 +142,9 @@ def main():
     if args.loop == "device":
         line["loop"] = "device: run_steps, one CUDA-graph replay per step and shard"
         line["regret"] = regret
+        if args.method == "coda":
+            line["tie_rule"] = args.tie_rule
+            line["tie_steps"] = int(sel.history()[2][args.warmup:].sum())
     if args.method == "model_picker":
         nbytes = 2 * H * N + 2 * N + 4 * N          # hard rows + labeled / disagree masks + entropies, per step
         line["bytes_per_step"] = nbytes

@@ -1132,6 +1132,20 @@ __global__ void __launch_bounds__(BL_THREADS) k_prefilter_pick(const float* __re
   }
 }
 
+// prefilter with sample scoring: one warp per sample position, its local item on this shard (or -1), resolved as
+// k_prefilter_pick resolves it
+__global__ void __launch_bounds__(BL_THREADS) k_pf_resolve(const float* __restrict__ cand,
+                                                          const uint8_t* __restrict__ labeled, long long N,
+                                                          const long long* __restrict__ xp, int nxb,
+                                                          const long long* __restrict__ best,
+                                                          const long long* __restrict__ pre, int width, int m,
+                                                          const long long* __restrict__ lw, int32_t* __restrict__ items) {
+  const int lane = threadIdx.x & 31;
+  const long long j = (long long)blockIdx.x * (BL_THREADS / 32) + (threadIdx.x >> 5);
+  const long long item = pf_item(cand, labeled, N, xp, nxb, best, pre, width, m, lw, j, lane);
+  if (lane == 0 && j < m) items[j] = (int32_t)item;
+}
+
 // one CTA: merge the block records, exchange them (record channel), the global winner -> abl_commit.  The isclose test
 // of coda.py:307 over the sample needs only the runner-up value v2.
 // DEFER (tie_rule="reference"): a winner with an isclose runner-up is not committed; *pending = 1 and lw[4] = bits(v)
@@ -1216,6 +1230,19 @@ extern "C" int coda_b200_prefilter_pick(const float* eig, const float* cand, con
       eig, cand, labeled, N, n_offset, (const long long*)partials, coda_b200_select_blocks(N), (const long long*)best,
       (const long long*)pre, width, m, (const long long*)lw, (long long*)recs);
   CODA_LAUNCH_OK("k_prefilter_pick");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_pf_resolve(const float* cand, const uint8_t* labeled, int64_t N, const int64_t* partials,
+                                    const int64_t* best, const int64_t* pre, int width, int m, const int64_t* lw,
+                                    int32_t* items, coda_stream_t stream) {
+  CODA_CHECK_ARG(cand && labeled && partials && best && pre && lw && items, "pf_resolve: null pointer");
+  CODA_CHECK_ARG(N >= 1 && N < (1LL << 31) && m >= 1 && m < (1 << 23) && width == m + 1,
+                 "pf_resolve: bad N=%lld m=%d width=%d", (long long)N, m, width);
+  k_pf_resolve<<<coda_b200_prefilter_blocks(m), BL_THREADS, 0, as_stream(stream)>>>(
+      cand, labeled, N, (const long long*)partials, coda_b200_select_blocks(N), (const long long*)best,
+      (const long long*)pre, width, m, (const long long*)lw, items);
+  CODA_LAUNCH_OK("k_pf_resolve");
   return CODA_B200_OK;
 }
 
@@ -1356,6 +1383,20 @@ __global__ void __launch_bounds__(32) k_pf_sample(const long long* __restrict__ 
   PyRand g{mt, pr_load(rng, mt)};
   pr_sample(g, n, m, setsize, pre + 1, pool, seen);
   pr_store(g, rng);
+}
+
+// prefilter with sample scoring, a step with n_s <= m candidates (the reference takes them all, coda.py:221-223, and
+// draws nothing): pre row 0 = {n_s, 0, 1, ..., n_s - 1, -1, ...} (every candidate, ascending), lw[0] = 0.  No word of
+// the generator is used.  n_s > m sets CODA_B200_FLAG_PREDRAW_MISMATCH (the host predicted a step without a sample).
+__global__ void __launch_bounds__(BL_THREADS) k_pf_identity(const long long* __restrict__ best, long long* __restrict__ pre,
+                                                           int m, long long* __restrict__ lw, uint32_t* __restrict__ flags) {
+  const long long n = best[1];
+  if (threadIdx.x == 0) {
+    pre[0] = n;
+    lw[0] = 0;
+    if (n > m) atomicOr(flags, CODA_B200_FLAG_PREDRAW_MISMATCH);
+  }
+  for (int j = threadIdx.x; j < m; j += BL_THREADS) pre[1 + j] = j < n ? j : -1;
 }
 
 // prefilter, pending step: band_item[j] = the global item of sample position j if this shard holds it and its EIG is
@@ -1514,6 +1555,15 @@ extern "C" int coda_b200_pf_sample(const int64_t* best, int64_t* pre, int m, int
   k_pf_sample<<<1, 32, 0, as_stream(stream)>>>((const long long*)best, (long long*)pre, m, setsize, rng, pool, seen,
                                                 (long long*)lw, flags);
   CODA_LAUNCH_OK("k_pf_sample");
+  return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_pf_identity(const int64_t* best, int64_t* pre, int m, int64_t* lw, uint32_t* flags,
+                                     coda_stream_t stream) {
+  CODA_CHECK_ARG(best && pre && lw && flags && m >= 1, "pf_identity: bad arguments");
+  k_pf_identity<<<1, BL_THREADS, 0, as_stream(stream)>>>((const long long*)best, (long long*)pre, m, (long long*)lw,
+                                                         flags);
+  CODA_LAUNCH_OK("k_pf_identity");
   return CODA_B200_OK;
 }
 

@@ -8,6 +8,8 @@
 // the item.  The gains of all rows come from row_gains (cached rows) or pair_rows (no cache); the assembly looks
 // them up.  An item's entries and its U row are contiguous in HBM: a warp that walks items in order streams them.
 // Candidate filter (coda.py:215-219, 239) and the arg-max with runner-up (coda.py:306-309) ride along.
+// The per-item arithmetic of k_gain_eig / k_eig_assemble_g8 and the per-row arithmetic of k_row_gains are restated
+// for the sampled scoring pass (eig_item.cuh, sample.cu); a change to one order of operations must be made to both.
 #include "common.cuh"
 
 #define GE_THREADS 384

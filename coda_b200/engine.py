@@ -54,6 +54,12 @@ REP_WORDS = 12 + TIE_CAP + TIE_CAP // 2     # [flags | record (8) | tie hdr (2) 
 MODES = ("incremental", "recompute", "recompute_all")
 TABLE_BATCH_BYTES = 512 << 20
 HIST_CAP = 1 << 16
+# With prefilter_n = m the engine scores only the sample when m * PREFILTER_ROW_COST_RATIO <= N.  Fitted by
+# tools/bench_prefilter.py on an H100 80GB HBM3 at 700 W, cfg3 (256 x 5e5 x 100): the sampled pass takes
+# 0.116 ms + 0.032 us per item (m = 1 000 ... 125 000), the full pass 0.885 ms, so they cross at m = 24 050 = N / 20.8
+# (BASELINE.md §6b).
+PREFILTER_ROW_COST_RATIO = 20.8
+PREFILTER_SCORING = ("auto", "sample", "full")
 
 
 def _ptr(t):
@@ -78,7 +84,8 @@ class Engine:
 
     def __init__(self, preds: torch.Tensor, *, alpha: float, learning_rate: float, multiplier: float,
                  uniform_prior: bool, hyp_w: float = 1.0, mode: str = "incremental", n_offset: int = 0,
-                 n_global: int | None = None, world: int = 1, own_stream: bool = False):
+                 n_global: int | None = None, world: int = 1, own_stream: bool = False, prefilter_n: int = 0,
+                 q: str = "eig"):
         from .datasets import CompactSlab
         if mode not in MODES:
             raise ValueError(f"mode must be one of {MODES}")
@@ -138,6 +145,14 @@ class Engine:
         # CODA_B200_OVERLAP=0: class-t table / row refresh on the main stream instead of a side stream
         self.overlap = os.environ.get("CODA_B200_OVERLAP", "1") != "0"
         self.use_graph = os.environ.get("CODA_B200_GRAPH", "1") != "0"
+        # prefilter_n: score only the sampled items each step (see _choose_sample_scoring)
+        self.pf_m = int(prefilter_n or 0) if q == "eig" else 0
+        self.pf_scoring = os.environ.get("CODA_B200_PREFILTER_SCORING", "auto")
+        if self.pf_scoring not in PREFILTER_SCORING:
+            raise ValueError(f"CODA_B200_PREFILTER_SCORING must be one of {PREFILTER_SCORING}, got {self.pf_scoring!r}")
+        if self.pf_scoring == "sample" and self.pf_m and mode != "incremental":
+            raise ValueError("CODA_B200_PREFILTER_SCORING=sample needs mode='incremental' (the template rows are cached)")
+        self.sample_scoring, self.sw = False, None
         self.profile, self.profile_only = None, None
         self.xchg = None                                      # set by the group (dist.py) before the first exchange
         self._mailbox = None
@@ -243,7 +258,7 @@ class Engine:
         self.m0 = self._z((Hp,), torch.float32)
         self.hb = self._z((1,), torch.float32)
         self.best_model = self._z((1,), torch.int64)
-        self.eig = self._e((N,), torch.float32)
+        self.eig = self._z((N,), torch.float32)
         self.nblocks = int(self.lib.coda_b200_eig_blocks(N, H, C))
         self.partials = self._z((self.nblocks, nat.REC_WORDS), torch.int64)
         # report block: one D2H copy per API step.  [flags | record (8) | tie hdr (2) | pad | tie idx | tie val]
@@ -461,7 +476,7 @@ class Engine:
         self.cls_base_host = cls_base
         self.cls_base = torch.from_numpy(cls_base).to(self.dev)
         # tiles of <= 32 (SIMT) or <= 128 (wgmma) same-class work-list positions
-        def make_tiles(width):
+        def make_tiles(width, per_cls=per_cls):
             nt = (per_cls + width - 1) // width
             tile_off = np.zeros(C + 1, dtype=np.int64)
             np.cumsum(nt, out=tile_off[1:])
@@ -472,10 +487,13 @@ class Engine:
             tiles = np.stack([cls_of_tile, start, cnt, np.zeros_like(cnt)], axis=1).astype(np.int32)
             return tile_off, int(nt.max()), torch.from_numpy(tiles).to(self.dev)
         width = 128 if self.use_tc else 32
-        tile_off, self.max_cls_tiles, self.tiles = make_tiles(width)
-        self.tile_off_host = tile_off
-        self.tile_off = torch.from_numpy(tile_off).to(self.dev)
-        self.ntiles = int(tile_off[-1])
+
+        def set_tiles(tiles):
+            tile_off, self.max_cls_tiles, self.tiles = tiles
+            self.tile_off_host = tile_off
+            self.tile_off = torch.from_numpy(tile_off).to(self.dev)
+            self.ntiles = int(tile_off[-1])
+        set_tiles(make_tiles(width))
         self.ent_row = self._e((max(1, n_ent),), torch.int32)
         self.ent_cls = self._e((max(1, n_ent),), torch.int16)
         self.zmask = self._e((self.npairs, W), torch.int32)
@@ -493,10 +511,13 @@ class Engine:
             self.ell_cls = self._e((N, self.ell_k), torch.int16)
             self._call("coda_b200_ell_build", _ptr(self.ent_off), _ptr(self.ent_row), _ptr(self.ent_cls), N, self.ell_k,
                        _ptr(self.ell_row), _ptr(self.ell_cls), s)
-        self.gain = self._z((self.npairs,), torch.float32)      # information gain of every row (templates first)
+        # sample scoring caches the T template rows only; the sample's heavy rows go to a scratch of `cap` rows
+        sample = self._choose_sample_scoring()
+        cap = self._sample_capacity() if sample else 0
+        self.gain = None if sample else self._z((self.npairs,), torch.float32)   # every row's gain (templates first)
         self.ph_cache = None
         if self.mode == "incremental":
-            need = self.npairs * self.Hp * 4
+            need = (self.T * self.Hp * 4 + self._sample_bytes(cap)) if sample else self.npairs * self.Hp * 4
             free, _total = torch.cuda.mem_get_info(self.dev)
             if need + (2 << 30) > free + torch.cuda.memory_reserved(self.dev) - torch.cuda.memory_allocated(self.dev):
                 # the row cache does not fit next to the slab: fall back to recomputing the rows every step
@@ -504,8 +525,50 @@ class Engine:
                 warnings.warn(f"coda_b200: row cache of {need / 2 ** 30:.1f} GiB does not fit "
                               f"({free / 2 ** 30:.1f} GiB free); falling back to mode='recompute'")
                 self.mode = "recompute"
+                if sample:
+                    self.gain = self._z((self.npairs,), torch.float32)
+                sample = False
             else:
-                self.ph_cache = self._e((self.npairs, self.Hp), torch.float32)
+                self.ph_cache = self._e((self.T if sample else self.npairs, self.Hp), torch.float32)
+        self.sample_scoring = sample
+        if sample:
+            # the tile lists cover the template positions only: the cache fill and the class-t refresh touch no
+            # heavy row (row ids < T, so they land in the T cached rows)
+            set_tiles(make_tiles(width, np.full(C, 1 + H, dtype=np.int64)))
+            self._alloc_sample(cap)
+
+    def _choose_sample_scoring(self) -> bool:
+        """prefilter_n = m: score only the m sampled items (sample.cu) instead of every item.  Chosen when the
+        sample's heavy rows cost less to integrate than all cached rows cost to stream (m * R <= N), in incremental
+        mode only: the sampled scoring reads the cached template rows.  CODA_B200_PREFILTER_SCORING forces a side."""
+        if self.pf_m <= 0 or self.pf_scoring == "full" or self.mode != "incremental":
+            return False
+        return self.pf_scoring == "sample" or self.pf_m * PREFILTER_ROW_COST_RATIO <= self.n_global
+
+    def _sample_capacity(self) -> int:
+        """Heavy rows of the m items that have the most: the most one sample (or one chunk of m items) can hold."""
+        heavy = self.heavy_off[1:] - self.heavy_off[:-1]
+        return max(1, int(torch.topk(heavy, min(self.pf_m, self.N)).values.sum()) if self.n_heavy else 0)
+
+    def _sample_bytes(self, cap) -> int:
+        """Device bytes of the sampled pass's scratch (see _alloc_sample)."""
+        width = 128 if self.use_tc else 32
+        m, C = self.pf_m, self.C
+        return cap * (self.Hp * 4 + self.W * 4 + 4 + 2 + 4) + self.T * 4 + (cap // width + C + 1) * 16 + 8 * m + 4 * C
+
+    def _alloc_sample(self, cap):
+        """Scratch of the sampled scoring pass, sized for the m items with the most heavy rows."""
+        H, C, W, Hp, T, m = self.H, self.C, self.W, self.Hp, self.T, self.pf_m
+        width = 128 if self.use_tc else 32
+        maxtiles = cap // width + C + 1
+        self.sw = dict(cap=cap, width=width, maxtiles=maxtiles,
+                       items=self._z((m,), torch.int32), hoff=self._z((m + 1,), torch.int32),
+                       cursor=self._z((C,), torch.int32), tiles=self._z((maxtiles, 4), torch.int32),
+                       tile_off=self._z((2,), torch.int64), sel=self._z((2,), torch.int64),
+                       nheavy=self._z((1,), torch.int64), zmask=self._z((cap, W), torch.int32),
+                       row_of=self._z((cap,), torch.int32), row_cls=self._z((cap,), torch.int16),
+                       rows=self._e((cap, Hp), torch.float32), gain=self._z((T + cap,), torch.float32),
+                       all_items=None)
 
     def shadow_reserve(self) -> int:
         """Device bytes this shard leaves free when it sizes its shadow: what it still allocates after construction
@@ -597,6 +660,9 @@ class Engine:
         """coda.py:235-281 + the per-block arg-max of coda.py:306/309 -> ``partials``."""
         if self.scored:
             return
+        if self.sample_scoring:
+            raise RuntimeError("coda_b200: this engine scores only prefilter samples (no heavy-row cache); the full "
+                               "scoring pass is not available (CODA_B200_PREFILTER_SCORING=full keeps it)")
         if self.mode == "incremental":
             if not self.cache_valid:
                 self._pair_rows(0, self.ntiles, gains=False)    # fill the row cache once
@@ -617,6 +683,78 @@ class Engine:
                    self.max_entries, _ptr(self.ell_row), _ptr(self.ell_cls), self.ell_k, _ptr(self.eig),
                    _ptr(self.partials), _ptr(self.flags), self._s())
         self.scored = True
+
+    def _score_sample(self):
+        """eig of the items in ``sw['items']`` only (sample.cu): their heavy rows as a work list, integrated into the
+        scratch by the row kernel in its device-``sel`` form, the gains of the template rows and the scratch, then the
+        assembly.  Every other entry of ``eig`` keeps its value."""
+        H, C, s, sw, m = self.H, self.C, self._s(), self.sw, self.pf_m
+        if not self.cache_valid:
+            self._pair_rows(0, self.ntiles, gains=False)    # the template rows (the cache is filled once)
+            self.cache_valid = True
+        common = (_ptr(self.ent_off), _ptr(self.ent_row), _ptr(self.ent_cls), _ptr(self.heavy_off))
+        self._call("coda_b200_sample_plan", _ptr(sw["items"]), m, *common, H, C, sw["width"], _ptr(sw["hoff"]),
+                   _ptr(sw["cursor"]), _ptr(sw["tiles"]), _ptr(sw["tile_off"]), _ptr(sw["nheavy"]), s)
+        self._call("coda_b200_sample_fill", _ptr(sw["items"]), m, _ptr(self.hard), H, C, *common, _ptr(sw["hoff"]),
+                   _ptr(sw["cursor"]), _ptr(sw["zmask"]), _ptr(sw["row_of"]), _ptr(sw["row_cls"]), s)
+        tail = (_ptr(self.PB), None, None, H, _ptr(sw["rows"]), None, _ptr(sw["sel"]), _ptr(sw["tile_off"]),
+                _ptr(self.flags), s)
+        if self.use_tc:
+            self._call("coda_b200_pair_rows_tc", _ptr(sw["tiles"]), 0, sw["maxtiles"], _ptr(sw["zmask"]),
+                       _ptr(sw["row_of"]), _ptr(self.dLb), _ptr(self.Gb), *tail)
+        else:
+            self._call("coda_b200_pair_rows", _ptr(sw["tiles"]), 0, sw["maxtiles"], _ptr(sw["zmask"]),
+                       _ptr(sw["row_of"]), _ptr(self.dL), _ptr(self.G0T), _ptr(self.G1T), *tail)
+        if self.pending:
+            self._cur().wait_event(self.ev_join)            # the class-t template rows of the side stream
+            self.pending = False
+        self._call("coda_b200_sample_gains", _ptr(self.ph_cache), _ptr(sw["rows"]), _ptr(sw["row_cls"]), sw["cap"],
+                   _ptr(sw["nheavy"]), H, C, _ptr(self.PB), _ptr(self.m0), _ptr(self.pi_hat), _ptr(sw["gain"]), s)
+        self._call("coda_b200_sample_eig", _ptr(sw["items"]), m, _ptr(sw["hoff"]), _ptr(self.U), C, H, *common,
+                   _ptr(sw["gain"]), self.max_entries, _ptr(self.eig), _ptr(self.flags), s)
+
+    def score_items(self, local_ids):
+        """Sample scoring: eig of the local items ``local_ids`` (a CPU or device integer tensor; None = every item of
+        the shard), in chunks of the scratch capacity (prefilter_n items).  One upload, then device copies; enqueue
+        only."""
+        m, items = self.pf_m, self.sw["items"]
+        with self._on():
+            if local_ids is None:
+                if self.sw["all_items"] is None:
+                    self.sw["all_items"] = torch.arange(self.N, dtype=torch.int32, device=self.dev)
+                ids = self.sw["all_items"]
+            elif local_ids.device == self.dev:
+                ids = local_ids.to(torch.int32)
+            else:
+                ids = local_ids.to(torch.int32).pin_memory().to(self.dev, non_blocking=True)
+            for c0 in range(0, ids.numel(), m):
+                chunk = ids[c0:c0 + m]
+                if chunk.numel() < m:
+                    items.fill_(-1)
+                items[: chunk.numel()].copy_(chunk)
+                self._score_sample()
+
+    def pf_fallback_score(self):
+        """run_steps, all-unlabeled fallback with more candidates than the sample holds (coda.py:239: every unlabeled
+        item is scored): eig of every item in chunks, then the block records of the EIG pass from it."""
+        with self._on():
+            self.score_items(None)
+            self._call("coda_b200_static_records", _ptr(self.eig), _ptr(self.labeled), _ptr(self.disagree), self.N,
+                       self.n_offset, self.nblocks, _ptr(self.partials), self._s())
+
+    def pf_fallback_commit(self, rule, record_best):
+        """The EIG loop's selection over those records (its tie rule), the label and the posterior update."""
+        with self._on():
+            s, x = self._s(), self._x()
+            if rule == "reference":
+                self._call("coda_b200_step_select_defer", self.st, x, _ptr(self.ref_lw[3:]), s)
+                self._ref_tie(self.eig)
+            else:
+                self._call("coda_b200_step_select", self.st, x, s)
+            self._post_label()
+            if record_best:
+                self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
+                           HIST_CAP, s)
 
     def _post_label(self):
         """coda.py:317-319 after ``sel`` / ``jvec`` / D / the gather list are in place (step_select or step_label):
@@ -857,8 +995,12 @@ class Engine:
             lw, pre, w, pend = self.ref_lw, self.abl_pre, self.abl_width, _ptr(self.ref_lw[3:])
             self._call("coda_b200_select_extreme_xchg", _ptr(self.abl_cand), _ptr(self.labeled), self.N, 1,
                        _ptr(self.abl_xp), _ptr(self.abl_best), x, _ptr(self.flags), s, n=2)
-            self._call("coda_b200_pf_sample", _ptr(self.abl_best), _ptr(pre), w - 1, self.ref_setsize, _ptr(self.pyrng),
-                       _ptr(self.ref_pool), _ptr(self.ref_seen), _ptr(lw), _ptr(self.flags), s)
+            if kind == "prefilter_id":
+                self._call("coda_b200_pf_identity", _ptr(self.abl_best), _ptr(pre), w - 1, _ptr(lw), _ptr(self.flags), s)
+            else:
+                self._call("coda_b200_pf_sample", _ptr(self.abl_best), _ptr(pre), w - 1, self.ref_setsize,
+                           _ptr(self.pyrng), _ptr(self.ref_pool), _ptr(self.ref_seen), _ptr(lw), _ptr(self.flags), s)
+            self._pf_score_sample(pre, w, lw)
             self._call("coda_b200_prefilter_pick", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
                        self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw),
                        _ptr(self.abl_recs), s)
@@ -882,6 +1024,10 @@ class Engine:
                 self._call("coda_b200_abl_commit", self.st, _ptr(self.abl_best), _ptr(self.abl_pick), _ptr(pre), w,
                            _ptr(lw), s)
             else:
+                if kind == "prefilter_id":
+                    self._call("coda_b200_pf_identity", _ptr(self.abl_best), _ptr(pre), w - 1, _ptr(lw),
+                               _ptr(self.flags), s)
+                self._pf_score_sample(pre, w, lw)
                 self._call("coda_b200_prefilter_pick", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
                            self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw),
                            _ptr(self.abl_recs), s)
@@ -889,11 +1035,19 @@ class Engine:
                            _ptr(self.abl_best), _ptr(pre), w, _ptr(lw), x, s)
             self._call("coda_b200_step_label", self.st, x, s)
         self._post_label()
-        if kind == "prefilter":
+        if kind == "prefilter" and not self.sample_scoring:
             self._score()
         if record_best:
             self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
                        HIST_CAP, s)
+
+    def _pf_score_sample(self, pre, w, lw):
+        """With sample scoring: this step's sample positions -> local items (as prefilter_pick resolves them) -> their
+        eig, which prefilter_pick then reads."""
+        if self.sample_scoring:
+            self._call("coda_b200_pf_resolve", _ptr(self.abl_cand), _ptr(self.labeled), self.N, _ptr(self.abl_xp),
+                       _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw), _ptr(self.sw["items"]), self._s())
+            self._score_sample()
 
     # the same phases as loop_prepare / loop_ready / loop_eager / loop_capture / loop_replay
     def abl_prepare(self, labels_dev, kind, record_best=False):
@@ -901,7 +1055,7 @@ class Engine:
             self._bind_labels(labels_dev)
             if record_best and getattr(self, "hist_best", None) is None:
                 self.hist_best = torch.full((HIST_CAP,), -1, dtype=torch.int32, device=self.dev)
-            if kind == "prefilter":
+            if kind == "prefilter" and not self.sample_scoring:
                 self._score()
 
     @staticmethod

@@ -120,7 +120,7 @@ class CODA(ModelSelector):
         n_offset = int(getattr(dataset, "n_offset", 0))
         n_global = int(getattr(dataset, "n_global", preds.shape[1]))
         kw = dict(alpha=alpha, learning_rate=learning_rate, multiplier=multiplier,
-                  uniform_prior=bool(disable_diag_prior), mode=mode, n_global=n_global)
+                  uniform_prior=bool(disable_diag_prior), mode=mode, n_global=n_global, prefilter_n=prefilter_n, q=q)
         if comm.world > 1:                                  # one process per GPU: this is one shard of the task
             self.group = ProcessGroup(comm)
             layout = [(preds, n_offset)]
@@ -200,7 +200,9 @@ class CODA(ModelSelector):
 
     @property
     def eig(self):
-        """Per-item expected information gain of the last scoring pass (this process's shards, item order)."""
+        """Per-item expected information gain of the last scoring pass (this process's shards, item order).  When the
+        engine scores only the ``prefilter_n`` sample (``sample_scoring``), an entry is current only for the items
+        scored last; the others keep the value they were last scored with (0 if never)."""
         self._sync()
         return self.engine.eig if len(self.engines) == 1 else torch.cat([self._home(e.eig) for e in self.engines], 0)
 
@@ -219,9 +221,9 @@ class CODA(ModelSelector):
             return self._select_ablation()                  # coda.py:287-295
         if self.q != "eig":
             raise NotImplementedError(self.q)               # coda.py:297
-        rep = self._fetch_report()
         if self.prefilter_n:
             return self._select_prefiltered()
+        rep = self._fetch_report()
         if rep["n_ties"] == 0:
             raise RuntimeError("no unlabeled items left to select from")
         if rep["n_ties"] > 1:                               # coda.py:308-311
@@ -283,7 +285,11 @@ class CODA(ModelSelector):
 
     def _select_prefiltered(self):
         """coda.py:221-223: random subsample of the candidates (``--prefilter-n``), then coda.py:306-313
-        on the subsample in sample order.  Cold ablation path; uses the EIG vector the kernels produced."""
+        on the subsample in sample order.  With sample scoring only the candidates the reference scores (the sample,
+        or the whole candidate list when it is not sampled) are scored; otherwise every item is."""
+        sample = self.engine.sample_scoring
+        if not sample:
+            self._fetch_report()
         labeled, disagree = self._cat("labeled"), self._cat("disagree")
         m = (labeled == 0) & (disagree != 0)
         ids = torch.nonzero(m, as_tuple=True)[0].tolist()
@@ -292,6 +298,14 @@ class CODA(ModelSelector):
             self.stochastic = True
         if not ids:
             ids = torch.nonzero(labeled == 0, as_tuple=True)[0].tolist()
+        if sample:
+            ids_t = torch.tensor(ids, dtype=torch.int64)
+            for e in self.engines:
+                lo, hi = e.n_offset, e.n_offset + e.N
+                e.score_items(ids_t[(ids_t >= lo) & (ids_t < hi)] - lo)
+            for e in self.engines:
+                e.sync()
+                e.check_flags(sync=True)
         qv = self._cat("eig")[torch.tensor(ids, device=self.device)]
         best = qv.max()
         ties = torch.isclose(qv, best, rtol=1e-8)
@@ -507,8 +521,38 @@ class CODA(ModelSelector):
                 self._abl_steps(kind, c, per_dev, record_best)
             if kind == "prefilter" or any(n > 1 for n in counts):
                 self.stochastic = True                      # coda.py:223 / 311
-        if k > drawn:
+        if k > drawn and kind == "prefilter" and self.engine.sample_scoring:
+            self._run_unsampled(counts, drawn, k, m, per_dev, record_best, rule)
+        elif k > drawn:
             self._run_eig(k - drawn, per_dev, record_best, rule)
+
+    def _run_unsampled(self, counts, s, k, m, per_dev, record_best, rule):
+        """Sample scoring, the prefilter steps without a sample (n_s <= prefilter_n, or the all-unlabeled fallback):
+        every candidate is scored.  Up to m candidates run the prefilter's graph with the identity sample
+        (k_pf_identity: all candidates in ascending order, no random draw, so the pick, q and tie flag of the EIG
+        loop); more, which only the fallback has, run eagerly with every item scored in chunks of m."""
+        width = m + 1
+        for e in self.engines:
+            e.abl_bind("prefilter", width=width, rows=max(1, ABL_CHUNK_WORDS // width) if rule == "first" else 1)
+            if rule == "reference":
+                e.ref_bind_prefilter(m, sample_setsize(m))
+        self._loop_dirty = True
+        while s < k:
+            big = counts[s] > m
+            t = s
+            while t < k and (counts[t] > m) == big:
+                t += 1
+            if big:
+                for e in self.engines:
+                    e.abl_prepare(per_dev[e.dev], "prefilter_id", record_best)   # labels and hist_best
+                for _ in range(t - s):
+                    for e in self.engines:
+                        e.pf_fallback_score()
+                    for e in self.engines:
+                        e.pf_fallback_commit(rule, record_best)
+            else:
+                self._abl_steps("prefilter_id", t - s, per_dev, record_best, rule)
+            s = t
 
     def _abl_steps(self, kind, k, per_dev, record_best, rule="first"):
         for e in self.engines:

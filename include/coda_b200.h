@@ -558,6 +558,39 @@ int coda_b200_pf_tie_draw(const coda_step_t* st, const int64_t* band_item, int m
 int coda_b200_pyrandom_run(uint32_t* state, const int64_t* ops, int nops, int64_t* out, int32_t* pool, uint32_t* seen,
                            coda_stream_t stream);
 
+/* ---- scoring only the prefilter_n sample (csrc/sample.cu) ---------------------------------------------------------
+ * items [m] int32: the local item of every sample position on this shard, -1 for none.  Every sampled item's eig is the
+ * bits the full scoring pass (row_gains + gain_eig) gives it from the same state; other entries of eig are untouched. */
+/* prefilter_pick's position -> local item resolution, written to items (-1: not on this shard / past n_s) */
+int coda_b200_pf_resolve(const float* cand, const uint8_t* labeled, int64_t N, const int64_t* partials,
+                         const int64_t* best, const int64_t* pre, int width, int m, const int64_t* lw, int32_t* items,
+                         coda_stream_t stream);
+/* a step with n_s = best[1] <= m candidates: pre row 0 = {n_s, 0 .. n_s - 1, -1 ...}, lw[0] = 0, no random draw
+ * (n_s > m sets CODA_B200_FLAG_PREDRAW_MISMATCH) */
+int coda_b200_pf_identity(const int64_t* best, int64_t* pre, int m, int64_t* lw, uint32_t* flags, coda_stream_t stream);
+/* One CTA: the sample's heavy rows as a class-major work list.  hoff [m+1]: slot of each position's first heavy row;
+ * cursor [C]: class bases (consumed by sample_fill); tiles [>= heavy/width + C][4] {class, first position, count, 0} of
+ * <= width (32 SIMT, 128 tensor-core) same-class positions; tile_off [2] = {0, tile count} (pair_rows' `sel` form with
+ * sel[1] = 0); nheavy [1] = the heavy-row count. */
+int coda_b200_sample_plan(const int32_t* items, int m, const int32_t* ent_off, const int32_t* ent_row,
+                          const uint16_t* ent_cls, const int32_t* heavy_off, int H, int C, int width, int32_t* hoff,
+                          int32_t* cursor, int32_t* tiles, int64_t* tile_off, int64_t* nheavy, coda_stream_t stream);
+/* masks (as pair_fill builds them), row_of (slot) and row_cls (class per slot) of the sample's heavy rows */
+int coda_b200_sample_fill(const int32_t* items, int m, const uint16_t* hard, int H, int C, const int32_t* ent_off,
+                          const int32_t* ent_row, const uint16_t* ent_cls, const int32_t* heavy_off, const int32_t* hoff,
+                          int32_t* cursor, uint32_t* zmask, int32_t* row_of, uint16_t* row_cls, coda_stream_t stream);
+/* gain [T + *nheavy]: the template rows' gains from tmpl [T][Hp], the sample rows' from scratch [cap][Hp] (row_gains'
+ * arithmetic) */
+int coda_b200_sample_gains(const float* tmpl, const float* scratch, const uint16_t* row_cls, int64_t cap,
+                           const int64_t* nheavy, int H, int C, const float* PB, const float* m0, const float* pi_hat,
+                           float* gain, coda_stream_t stream);
+/* eig[items[j]] for every position j with an item: the arithmetic gain_eig uses for this C and max_entries; sets
+ * CODA_B200_FLAG_NONFINITE_EIG */
+int coda_b200_sample_eig(const int32_t* items, int m, const int32_t* hoff, const float* U, int C, int H,
+                         const int32_t* ent_off, const int32_t* ent_row, const uint16_t* ent_cls,
+                         const int32_t* heavy_off, const float* gain, int max_entries, float* eig, uint32_t* flags,
+                         coda_stream_t stream);
+
 /* ---- ModelPicker's epsilon grid search (coda_b200/eps_search.py, DESIGN.md §5b) -------------------------------------
  * A run (epsilon e, realisation r) is B steps of ModelPicker.run_steps(B, labels[pool[r]], seed = keys[e][r]) on the
  * task restricted to the P items pool[r] (global item ids), bit for bit: picks[e][r][s] is the pool position labelled at

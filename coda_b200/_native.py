@@ -31,6 +31,7 @@ FLAG_ROWSUM_WARN = 0x200
 FLAG_PIPELINE_TIMEOUT = 0x400
 FLAG_PREDRAW_MISMATCH = 0x800
 SLAB_F32, SLAB_F16, SLAB_BF16 = 0, 1, 2
+RANDPERM32_MAX = 214748364          # CODA_B200_RANDPERM32_MAX: torch.randperm(n) draws 64-bit words from here
 
 
 def slab_format(dtype) -> int:
@@ -155,6 +156,9 @@ SIGNATURES = {
     "coda_b200_mp_entropy_dev": (i32, [p, p, i32, i64, i32, f64, p, p, p, p, p]),
     "coda_b200_bl_draw": (i32, [PL, p]),
     "coda_b200_bl_step": (i32, [PL, PX, p]),
+    "coda_b200_bl_draw_ref": (i32, [PL, p, p]),
+    "coda_b200_bl_best_ref": (i32, [PL, p, p, p]),
+    "coda_b200_torch_rng_run": (i32, [p, p, p, i32, p, p]),
     "coda_b200_static_records": (i32, [p, p, p, i64, i64, i32, p, p]),
     "coda_b200_abl_draw": (i32, [p, i32, p, p]),
     "coda_b200_abl_commit": (i32, [PS, p, p, p, i32, p, p]),

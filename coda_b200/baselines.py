@@ -21,8 +21,10 @@ Host-free loop: ``run_steps(k, labels, seed=...)`` runs ``k`` steps of main.py:9
 best model) as one CUDA-graph replay per step and shard, with one host sync at the end; ``history()`` /
 ``best_history()`` read back the picks and per-step best models and bring the host-side state up to date, so API calls
 and device loops can follow each other.  Draws whose consumption is known up front (IID's ``random.choice``, the
-``random.random()`` of ActiveTesting and VMA) are made on the host before the loop with the API's own calls; tie
-breaks are drawn on the device from a Philox4x32-10 stream (``include/coda_b200.h``, DESIGN.md §5b).
+``random.random()`` of ActiveTesting and VMA) are made on the host before the loop with the API's own calls.  The
+draws the reference makes from torch's generators (tie breaks, ModelPicker's draws) come from a Philox4x32-10 stream
+by default, or with ``tie_rule="reference"`` from device replicas of torch's CPU and CUDA generators, call for call
+(``include/coda_b200.h``, DESIGN.md §5b).
 """
 from __future__ import annotations
 
@@ -78,6 +80,43 @@ def rewind(state, kind, j, n0):
     """Python ``random`` as after the first ``j`` steps' draws from ``state`` (the state before ``predraw``)."""
     random.setstate(state)
     predraw(kind, j, n0)
+
+
+# torch.get_rng_state(): u64 seed, i32 left, i32 seeded, u64 next, then the 624 MT19937 words as u64 (low 32 bits),
+# then the normal samplers' cache (5056 bytes in all)
+_MT_WORDS = slice(24, 24 + 8 * 624)
+
+
+def torch_rng_words(state: torch.Tensor) -> torch.Tensor:
+    """torch.get_rng_state() -> the device replica's int32 [625]: the 624 words (as uint32 bits), then the position of
+    the next word, 625 - left (torch draws ``if (--left == 0) twist; y = state[next++]``)."""
+    b = state.numpy().tobytes()
+    left = int(np.frombuffer(b, "<i4", 1, 8)[0])
+    out = np.empty(625, np.uint32)
+    out[:624] = np.frombuffer(b[_MT_WORDS], "<u8")
+    out[624] = 625 - left
+    return torch.from_numpy(out.view(np.int32))
+
+
+def torch_rng_state(words: torch.Tensor, state0: torch.Tensor) -> torch.Tensor:
+    """The inverse of ``torch_rng_words``: ``state0`` with its words, ``left`` and ``next`` taken from the replica and
+    every other byte kept."""
+    b = state0.numpy().copy()
+    w = words.numpy().view(np.uint32)
+    pos = int(w[624])
+    b[8:12] = np.array([625 - pos], "<i4").view(np.uint8)
+    b[16:24] = np.array([pos], "<u8").view(np.uint8)
+    b[_MT_WORDS] = w[:624].astype("<u8").view(np.uint8)
+    return torch.from_numpy(b)
+
+
+def cuda_rng_words(state: torch.Tensor) -> torch.Tensor:
+    """torch.cuda.get_rng_state() (u64 seed, i64 offset) -> the device replica's int64 [2]."""
+    return torch.from_numpy(np.frombuffer(state.numpy().tobytes(), "<i8").copy())
+
+
+def cuda_rng_state(words: torch.Tensor) -> torch.Tensor:
+    return torch.from_numpy(words.numpy().astype("<i8").view(np.uint8).copy())
 
 
 def _synced(fn):
@@ -291,7 +330,10 @@ class _DeviceState:
             self.h_best = z(HIST_CAP, dt=torch.int32)
             self.h_btie = z(HIST_CAP, dt=torch.int32)
             self.h_loss = z(HIST_CAP, H, dt=torch.uint8) if lure else None
+            self.trng = z(625, dt=torch.int32)                # tie_rule="reference": torch's CPU generator
+            self.grng = z(2, dt=torch.int64)                  # and its CUDA generator (ModelPicker)
         self.lmethod, self.lgraph, self.lstruct = method, None, None
+        self.lrule = "philox"
         self.lgamma_f32 = float(np.float32(gamma))            # gamma enters modelpicker.py:78 as a float32 factor
         self.n_global = int(n_global)
         # the vector the arg-extreme selection runs over (IID: all zeros, so the k-th tie is the k-th unlabeled item)
@@ -323,10 +365,17 @@ class _DeviceState:
     def _lw(self, i):
         return self.ls.data_ptr() + 8 * i                     # address of loop word i
 
+    def loop_rule(self, rule):
+        """The tie rule of the next steps; the captured graph is of one rule."""
+        if rule != self.lrule:
+            self.lrule, self.lgraph = rule, None
+
     def loop_phase(self, phase):
-        """Enqueue phase 0-3 of one device-loop step: the selection pass, the draw, the pick, the step kernel."""
+        """Enqueue phase 0-3 of one device-loop step: the selection pass, the draw, the pick, the step kernel (with
+        tie_rule="reference": the draw from torch's CPU generator, and the best model's tie redrawn after the step)."""
         m, a = self.lmethod, ctypes.byref(self.lstruct)
         lure = m in (nat.BL_ACTIVETESTING, nat.BL_VMA)
+        ref = self.lrule == "reference"
         with self._on():
             if phase == 0:
                 if lure:
@@ -338,7 +387,10 @@ class _DeviceState:
                                self._s())
                 self.extreme(self.lvec, m != nat.BL_MODELPICKER)
             elif phase == 1:
-                self._call("coda_b200_bl_draw", a, self._s())
+                if ref and m in (nat.BL_UNCERTAINTY, nat.BL_MODELPICKER):
+                    self._call("coda_b200_bl_draw_ref", a, _ptr(self.trng), self._s())
+                else:
+                    self._call("coda_b200_bl_draw", a, self._s())
             elif phase == 2:
                 if lure:
                     self._call("coda_b200_weighted_draw_xchg_dev", _ptr(self.score), _ptr(self.labeled), self.N,
@@ -351,6 +403,8 @@ class _DeviceState:
                                _ptr(self.flags), self._s())
             else:
                 self._call("coda_b200_bl_step", a, self._x(), self._s())
+                if ref:
+                    self._call("coda_b200_bl_best_ref", a, _ptr(self.trng), _ptr(self.grng), self._s())
 
     def loop_body(self):
         for phase in range(4):
@@ -637,21 +691,80 @@ class _Baseline(ModelSelector):
                     getattr(st, name).copy_(v)
         self._dev_nlab = nlab
 
-    def run_steps(self, k, labels, *, seed=None):
+    def _reference_refusals(self):
+        if self._loop_method == nat.BL_UNCERTAINTY and self.N >= nat.RANDPERM32_MAX:
+            raise NotImplementedError(f"coda_b200.baselines: tie_rule='reference' mirrors torch.randperm's 32-bit "
+                                      f"branch, which takes fewer than {nat.RANDPERM32_MAX} items; got {self.N}")
+
+    def _rng_upload(self):
+        """tie_rule="reference": torch's CPU generator (and for ModelPicker the CUDA generator of the dataset's
+        device) -> every shard's replicas; returns what ``_rng_download`` needs."""
+        cpu = torch.get_rng_state()
+        if cpu.numel() != 5056:
+            raise RuntimeError(f"coda_b200.baselines: torch.get_rng_state() has {cpu.numel()} bytes, the replica "
+                               f"reads the layout of 5056")
+        gpu = torch.cuda.get_rng_state(self.device) if self._loop_method == nat.BL_MODELPICKER else None
+        if gpu is not None and gpu.numel() != 16:
+            raise RuntimeError(f"coda_b200.baselines: torch.cuda.get_rng_state() has {gpu.numel()} bytes, the replica "
+                               f"reads {{seed, offset}} (16)")
+        words = torch_rng_words(cpu)
+        gw = cuda_rng_words(gpu) if gpu is not None else None
+        for st in self.states:
+            st.enter()
+            with st._on():
+                st.trng.copy_(words)
+                if gw is not None:
+                    st.grng.copy_(gw)
+        return cpu, words, gw
+
+    def _rng_download(self, up):
+        """The replicas -> torch's generators (only the words and the position or offset change); raises if the
+        shards' replicas differ."""
+        cpu, words, gw = up
+        got = []
+        for st in self.states:
+            with st._on():
+                got.append((st.trng.cpu(), st.grng.cpu()))
+        t, g = got[0]
+        if any(not torch.equal(t2, t) or (gw is not None and not torch.equal(g2, g)) for t2, g2 in got[1:]):
+            raise RuntimeError("coda_b200.baselines: the shards' replicas of torch's generators differ after run_steps")
+        if not torch.equal(t, words):                  # untouched: keep torch's own bytes (e.g. left = 1, next = 0)
+            torch.set_rng_state(torch_rng_state(t, cpu))
+        if gw is not None and not torch.equal(g, gw):
+            torch.cuda.set_rng_state(cuda_rng_state(g), self.device)
+
+    def run_steps(self, k, labels, *, seed=None, tie_rule="philox"):
         """``k`` steps of main.py:91-94 (get_next_item_to_label, oracle, add_label, get_best_model_prediction) on the
         device: after a warm-up step, one CUDA-graph replay per step and shard (``CODA_B200_GRAPH=0``: the same
         kernels launched one by one), one host sync at the end.  ``labels``: int64 tensor of all N labels (cached per
-        device).  ``seed``: key of the Philox stream of the tie draws (``None``: one ``torch.randint`` on the CPU
-        generator).  Python ``random`` is consumed as by ``k`` API steps.  When a step needs what the device loop does
+        device).  Python ``random`` is consumed as by ``k`` API steps.  When a step needs what the device loop does
         not do (VMA's uniform fallback, ActiveTesting's zero total), the remaining steps run on the API path, with the
         API's result or error.  Returns the number of steps performed (``k``); read ``history()`` /
-        ``best_history()`` afterwards."""
+        ``best_history()`` afterwards.
+
+        ``tie_rule``: where the draws the reference makes from torch's generators come from (Uncertainty's item ties,
+        ModelPicker's item and best model, the best-model ties of the others).  ``"philox"`` (the default): a
+        Philox4x32-10 stream keyed by ``seed`` (``None``: one ``torch.randint`` on the CPU generator), the same
+        distribution as the reference's.  ``"reference"``: the same draws, from device replicas of torch's CPU
+        generator and of the CUDA generator of the dataset's device, written back afterwards, so the picks, best
+        models and ``torch.get_rng_state()`` / ``torch.cuda.get_rng_state()`` are those of ``k`` API steps.  It takes
+        no ``seed``."""
+        if tie_rule not in ("philox", "reference"):
+            raise ValueError(f"tie_rule must be 'philox' or 'reference', got {tie_rule!r}")
+        ref = tie_rule == "reference"
+        if ref and seed is not None:
+            raise ValueError("coda_b200.baselines: seed= keys the Philox stream of tie_rule='philox'; "
+                             "tie_rule='reference' draws from torch's generators")
         k = int(k)
         self._loop_check(k, labels)
+        if ref:
+            self._reference_refusals()
         if k == 0:
             return 0
         per_dev = self._loop_bind_labels(labels)
-        if seed is None:
+        if ref:
+            seed = 0
+        elif seed is None:
             seed = int(torch.randint(0, 1 << 62, (1,)).item())
         seed = int(seed) & ((1 << 64) - 1)
         seed = seed - (1 << 64) if seed >= 1 << 63 else seed
@@ -667,8 +780,10 @@ class _Baseline(ModelSelector):
         for st in self.states:
             st.enter()                                # after what the caller's stream enqueued (API-path state)
             st.loop_bind(per_dev[st.dev], k)
+            st.loop_rule(tie_rule)
         if not self._loop_dirty and self._dev_nlab != len(self.d_l_idxs):
             self._loop_upload(seed)
+        up = self._rng_upload() if ref else None
         for st in self.states:
             with st._on():
                 st.pre[:pre_host.numel()].copy_(pre_host, non_blocking=True)
@@ -706,6 +821,8 @@ class _Baseline(ModelSelector):
         self._dev_steps = done_before + done
         self._dev_nlab = len(self.d_l_idxs) + (self._dev_steps - self._hist_seen)
         self._loop_dirty = self._dev_steps > self._hist_seen
+        if ref:
+            self._rng_download(up)
         if done < k:                                   # the API path takes over where the device loop stopped
             self.history()
             rewind(state0, self._loop_draw, done, n0)

@@ -72,7 +72,7 @@ __device__ __forceinline__ long long pr_randbelow(PyRand& g, long long n) {
 
 // random.sample(range(n), m) -> out[0 .. m).  pool: >= n ints (used when n <= setsize); seen: ceil(n / 32) words,
 // zero on entry and on return (used otherwise).  setsize is Lib/random.py's, computed on the host (it depends on m only).
-__device__ void pr_sample(PyRand& g, long long n, int m, long long setsize, long long* out, int* pool, uint32_t* seen) {
+static __device__ void pr_sample(PyRand& g, long long n, int m, long long setsize, long long* out, int* pool, uint32_t* seen) {
   const int lane = threadIdx.x & 31;
   if (n <= setsize) {
     for (long long i = lane; i < n; i += 32) pool[i] = (int)i;

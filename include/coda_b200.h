@@ -483,6 +483,30 @@ int coda_b200_bl_draw(const coda_bl_loop_t* a, coda_stream_t stream);
  * the method's sums, the best model, the history slots, then the counters advance. */
 int coda_b200_bl_step(const coda_bl_loop_t* a, const coda_xchg_t* x, coda_stream_t stream);
 
+/* ---- torch's generators on the device (run_steps(..., tie_rule="reference") of the competing selectors) -----------
+ * The draws the reference makes from torch's generators, from replicas of them on every shard (csrc/bl_ref.cu):
+ *   cpu_rng [625] uint32: torch's CPU generator (MT19937), the 624 state words then the position of the next word,
+ *     pos = 625 - left of torch.get_rng_state() (pos = next after the first word of a twist).
+ *     randperm(n)[0] = word % n, then n - 2 words dropped (n < CODA_B200_RANDPERM32_MAX: torch's 32-bit branch);
+ *     randint(n) = word % n for n < 2^28, else ((word1 << 32) | word2) % n.
+ *   cuda_rng [2] int64: torch's CUDA generator {seed, offset}; randint(n) (n < 2^28) = curand4(curand_init(seed, 0,
+ *     offset)).x % n, then offset += 4.
+ * Per step: Uncertainty and ModelPicker run bl_draw_ref in place of bl_draw; every method runs bl_best_ref right after
+ * bl_step.  Every shard advances its replicas by the same global counts. */
+#define CODA_B200_RANDPERM32_MAX 214748364LL /* (2^32 - 1) / 20: from here torch.randperm draws 64-bit words */
+/* One warp, in place of bl_draw: this step's k (Uncertainty: randperm(best[1])[0] when best[1] > 1 items tie, else 0;
+ * ModelPicker: randint(best[1]), every step) from cpu_rng. */
+int coda_b200_bl_draw_ref(const coda_bl_loop_t* a, uint32_t* cpu_rng, coda_stream_t stream);
+/* One warp, after bl_step of a step that committed: the best model again from the sums bl_step left, with its tie drawn
+ * as the reference draws it -- randperm(ties)[0] from cpu_rng when several models tie (IID, Uncertainty, ActiveTesting,
+ * VMA), randint(ties) from cuda_rng every step (ModelPicker) -- into hist_best of the step.  The unused replica may be
+ * NULL. */
+int coda_b200_bl_best_ref(const coda_bl_loop_t* a, uint32_t* cpu_rng, int64_t* cuda_rng, coda_stream_t stream);
+/* One warp runs ops [nops][2] in order, one output each: {0, n} randperm(n)[0] (0 for n = 1) and {1, n} randint(n) from
+ * cpu_rng, {2, n} randint(n) from cuda_rng. */
+int coda_b200_torch_rng_run(uint32_t* cpu_rng, int64_t* cuda_rng, const int64_t* ops, int nops, int64_t* out,
+                            coda_stream_t stream);
+
 /* ---- CODA's other acquisitions in its host-free loop (q='uncertainty', q='iid', prefilter_n; coda.py:215-224, 287-295)
  * Candidates: the unlabeled items some model disagrees on, all unlabeled items when there are none (coda.py:239); as
  * the exact maximum ties of `cand` (the disagreement bits as 1.0f / 0.0f) under select_extreme_xchg(want_max = 1).

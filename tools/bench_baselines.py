@@ -2,14 +2,16 @@
 
     python tools/bench_baselines.py --method {iid,uncertainty,activetesting,vma,model_picker,coda} [--steps 100] [--warmup 10]
         [--shards S] [--gpus G] [--compact K] [--loop {api,device}] [--q {eig,iid,uncertainty}] [--prefilter-n K]
-        [--tie-rule {first,reference}]
+        [--tie-rule {first,philox,reference}]
     python -m torch.distributed.run --nproc-per-node 8 tools/bench_baselines.py --method model_picker --N 1000000
 
 --loop device times ``run_steps`` (one CUDA-graph replay per step and shard, the oracle's labels on the device) instead
 of the public API loop, and reports the final and cumulative regret of the timed steps from ``best_history()`` and the
 true accuracy losses of the models (Oracle.true_losses).  Not under torchrun.  --method coda runs CODA with its default
 arguments unless --q / --prefilter-n name its other acquisitions (coda.py:215-224, 287-295); its device loop is
-``run_steps(..., record_best=True)``, the graph that also records each step's best model.
+``run_steps(..., record_best=True)``, the graph that also records each step's best model.  --tie-rule picks run_steps'
+tie rule: ``first`` / ``reference`` for CODA, ``philox`` / ``reference`` (torch's own generators, mirrored on the
+device) for the five competing selectors; the default is each one's default.
 
 --shards / --gpus split the task over in-process N-range shards (shards may share a GPU); under torchrun every rank
 holds its own N-range and rank 0 prints the line.  --compact K generates the task directly as a top-K compact slab
@@ -50,13 +52,17 @@ def main():
     ap.add_argument("--loop", choices=["api", "device"], default="api", help="public API loop or run_steps")
     ap.add_argument("--q", choices=["eig", "iid", "uncertainty"], default="eig", help="CODA's acquisition (--method coda)")
     ap.add_argument("--prefilter-n", type=int, default=0, help="CODA's random subsample of the candidates (--method coda)")
-    ap.add_argument("--tie-rule", choices=["first", "reference"], default="first",
-                    help="CODA's run_steps tie rule (--method coda --loop device)")
+    ap.add_argument("--tie-rule", choices=["first", "philox", "reference"], default=None,
+                    help="run_steps' tie rule (--loop device): first | reference for coda, philox | reference otherwise")
     args = ap.parse_args()
     if args.method != "coda" and (args.q != "eig" or args.prefilter_n):
         raise SystemExit("bench_baselines: --q and --prefilter-n are options of --method coda")
-    if args.tie_rule != "first" and (args.method != "coda" or args.loop != "device"):
-        raise SystemExit("bench_baselines: --tie-rule is an option of --method coda --loop device")
+    if args.tie_rule is not None and args.loop != "device":
+        raise SystemExit("bench_baselines: --tie-rule is an option of --loop device")
+    rules = ("first", "reference") if args.method == "coda" else ("philox", "reference")
+    args.tie_rule = args.tie_rule or rules[0]
+    if args.tie_rule not in rules:
+        raise SystemExit(f"bench_baselines: --method {args.method} takes --tie-rule {' or '.join(rules)}")
     if args.steps + args.warmup >= args.N:
         raise SystemExit("bench_baselines: steps + warmup must stay below the number of items")
     # stdout carries exactly one JSON line
@@ -99,7 +105,12 @@ def main():
     regret = None
     if args.loop == "device":
         labels_dev = ds.labels_host.to(dev)
-        loop_kw = dict(record_best=True, tie_rule=args.tie_rule) if args.method == "coda" else dict(seed=args.seed)
+        if args.method == "coda":
+            loop_kw = dict(record_best=True, tie_rule=args.tie_rule)
+        elif args.tie_rule == "reference":
+            loop_kw = dict(tie_rule="reference")           # draws from torch's generators, seeded above
+        else:
+            loop_kw = dict(seed=args.seed)
         sel.run_steps(args.warmup, labels_dev, **loop_kw)
         torch.cuda.synchronize()
         t = time.perf_counter()
@@ -142,9 +153,10 @@ def main():
     if args.loop == "device":
         line["loop"] = "device: run_steps, one CUDA-graph replay per step and shard"
         line["regret"] = regret
-        if args.method == "coda":
-            line["tie_rule"] = args.tie_rule
-            line["tie_steps"] = int(sel.history()[2][args.warmup:].sum())
+        line["tie_rule"] = args.tie_rule
+        line["tie_steps"] = int(sel.history()[2][args.warmup:].sum())
+        if args.method != "coda":
+            line["best_tie_steps"] = int(sel.best_history()[1][args.warmup:].sum())
     if args.method == "model_picker":
         nbytes = 2 * H * N + 2 * N + 4 * N          # hard rows + labeled / disagree masks + entropies, per step
         line["bytes_per_step"] = nbytes

@@ -467,12 +467,15 @@ extern "C" int coda_b200_init_dirichlets(const int64_t* conf_fx, const int64_t* 
 
 // ---------------------------------------------------------------------------------------
 // pi_full: U[n][c] = sum_h sum_s D[h][c][s] * preds[h][n][s]   (fp32 SIMT GEMM, K = H*C)
-// CTA: 64 points x (up to 128 classes per pass); thread (pg, cg) owns 4 points x 8 classes.
+// CTA: 64 points x 128 classes (grid.y walks the class blocks); thread (pg, cg) owns 4 points x 8 classes.
+// COMP (C > 128, where no tensor-core pass exists): compensated (Kahan) accumulation.  There the diagonal term puts the
+// accumulator near 1 and the H*C off-diagonal terms are each about one ulp of it; a plain chain rounds every one of them
+// the same way and drifts by 1e-4 relative at C = 3200 (1e-3 at H = 128), the compensated chain stays at a few ulps.
 // ---------------------------------------------------------------------------------------
 #define PF_TN 64
 #define PF_TC 128
 #define PF_SK 32
-template <typename T>
+template <typename T, bool COMP>
 __global__ void __launch_bounds__(256) k_pi_full(const T* __restrict__ preds, long long ldh,
                                                  const float* __restrict__ D, int H, long long N, int C,
                                                  float* __restrict__ U) {
@@ -481,52 +484,60 @@ __global__ void __launch_bounds__(256) k_pi_full(const T* __restrict__ preds, lo
   const int tid = threadIdx.x;
   const int pg = tid >> 4, cg = tid & 15;
   const long long n0 = (long long)blockIdx.x * PF_TN;
-  for (int c0 = 0; c0 < C; c0 += PF_TC) {
-    float acc[4][8];
+  const int c0 = blockIdx.y * PF_TC;
+  float acc[4][8], cmp[4][8];
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
+  for (int i = 0; i < 4; ++i)
 #pragma unroll
-      for (int k = 0; k < 8; ++k) acc[i][k] = 0.f;
-    for (int h = 0; h < H; ++h) {
-      const T* Ah = preds + (size_t)h * ldh;
-      const float* Dh = D + ((size_t)h * C) * C;
-      for (int s0 = 0; s0 < C; s0 += PF_SK) {
-        __syncthreads();
-        for (int e = tid; e < PF_TN * PF_SK; e += 256) {
-          int r = e >> 5, col = e & 31;
-          long long n = n0 + r;
-          int s = s0 + col;
-          As[r][col] = (n < N && s < C) ? ldg_f(Ah + (size_t)n * C + s) : 0.f;
-        }
-        for (int e = tid; e < PF_TC * PF_SK; e += 256) {
-          int r = e >> 5, col = e & 31;
-          int c = c0 + r, s = s0 + col;
-          Bs[r][col] = (c < C && s < C) ? __ldg(Dh + (size_t)c * C + s) : 0.f;
-        }
-        __syncthreads();
+    for (int k = 0; k < 8; ++k) acc[i][k] = cmp[i][k] = 0.f;
+  for (int h = 0; h < H; ++h) {
+    const T* Ah = preds + (size_t)h * ldh;
+    const float* Dh = D + ((size_t)h * C) * C;
+    for (int s0 = 0; s0 < C; s0 += PF_SK) {
+      __syncthreads();
+      for (int e = tid; e < PF_TN * PF_SK; e += 256) {
+        int r = e >> 5, col = e & 31;
+        long long n = n0 + r;
+        int s = s0 + col;
+        As[r][col] = (n < N && s < C) ? ldg_f(Ah + (size_t)n * C + s) : 0.f;
+      }
+      for (int e = tid; e < PF_TC * PF_SK; e += 256) {
+        int r = e >> 5, col = e & 31;
+        int c = c0 + r, s = s0 + col;
+        Bs[r][col] = (c < C && s < C) ? __ldg(Dh + (size_t)c * C + s) : 0.f;
+      }
+      __syncthreads();
 #pragma unroll 8
-        for (int s = 0; s < PF_SK; ++s) {
-          float a[4], b[8];
+      for (int s = 0; s < PF_SK; ++s) {
+        float a[4], b[8];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) a[i] = As[pg * 4 + i][s];
+        for (int i = 0; i < 4; ++i) a[i] = As[pg * 4 + i][s];
 #pragma unroll
-          for (int k = 0; k < 8; ++k) b[k] = Bs[cg + 16 * k][s];
+        for (int k = 0; k < 8; ++k) b[k] = Bs[cg + 16 * k][s];
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 4; ++i)
 #pragma unroll
-            for (int k = 0; k < 8; ++k) acc[i][k] = fmaf(a[i], b[k], acc[i][k]);
-        }
+          for (int k = 0; k < 8; ++k) {
+            if (COMP) {
+              const float y = fmaf(a[i], b[k], -cmp[i][k]);
+              const float t = acc[i][k] + y;
+              cmp[i][k] = (t - acc[i][k]) - y;
+              acc[i][k] = t;
+            } else {
+              acc[i][k] = fmaf(a[i], b[k], acc[i][k]);
+            }
+          }
       }
     }
+  }
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      long long n = n0 + pg * 4 + i;
-      if (n >= N) continue;
+  for (int i = 0; i < 4; ++i) {
+    long long n = n0 + pg * 4 + i;
+    if (n >= N) continue;
 #pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        int c = c0 + cg + 16 * k;
-        if (c < C) U[(size_t)n * C + c] = acc[i][k];
-      }
+    for (int k = 0; k < 8; ++k) {
+      int c = c0 + cg + 16 * k;
+      if (c < C) U[(size_t)n * C + c] = acc[i][k];
     }
   }
 }
@@ -535,8 +546,11 @@ template <typename T>
 static int pi_full(const T* preds, int64_t model_stride, const float* D, int H, int64_t N, int C, float* U,
                    coda_stream_t stream) {
   CODA_CHECK_ARG(preds && D && U, "pi_full: null pointer");
-  long long grid = (N + PF_TN - 1) / PF_TN;
-  k_pi_full<T><<<(unsigned)grid, 256, 0, as_stream(stream)>>>(preds, (long long)model_stride, D, H, N, C, U);
+  dim3 grid((unsigned)((N + PF_TN - 1) / PF_TN), (unsigned)((C + PF_TC - 1) / PF_TC));
+  if (C > PF_TC)
+    k_pi_full<T, true><<<grid, 256, 0, as_stream(stream)>>>(preds, (long long)model_stride, D, H, N, C, U);
+  else
+    k_pi_full<T, false><<<grid, 256, 0, as_stream(stream)>>>(preds, (long long)model_stride, D, H, N, C, U);
   CODA_LAUNCH_OK("k_pi_full");
   return CODA_B200_OK;
 }
@@ -552,8 +566,10 @@ extern "C" int coda_b200_pi_full_x(const void* preds, int fmt, int64_t model_str
 }
 
 // ---------------------------------------------------------------------------------------
-// shared tail of pi_reduce / pi_rank1: one warp normalises one row of U and accumulates the
-// per-class column sums of pi_hat_xi (fixed point) into a warp-private shared-memory vector.
+// shared tail of pi_reduce / pi_rank1: one warp normalises one row of U and adds the per-class
+// column sums of pi_hat_xi (fixed point) into the block's shared-memory vector wacc[C] with 64-bit
+// shared atomics.  One [C] vector per block (not one per warp) keeps C = 4096 at 32 KB; the sums
+// are integers, so the order of the atomics does not change their bits.
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ void row_accumulate(float* __restrict__ urow, int C, int lane, float fxs, int t,
                                                float delta_t, float* __restrict__ xi_out,
@@ -576,7 +592,7 @@ __device__ __forceinline__ void row_accumulate(float* __restrict__ urow, int C, 
     float xi = row_quot(urow[c], den, rden);   // column t was rewritten above by this same lane
 
     if (xi_out) xi_out[c] = xi;
-    wacc[c] += to_fx(xi, fxs);
+    atomicAdd(reinterpret_cast<unsigned long long*>(wacc) + c, (unsigned long long)to_fx(xi, fxs));
   }
 }
 
@@ -585,18 +601,16 @@ __global__ void __launch_bounds__(256) k_pi_reduce(float* __restrict__ U, long l
                                                    unsigned long long* __restrict__ pisum_fx,
                                                    uint32_t* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  long long* wacc_all = reinterpret_cast<long long*>(smem_raw);       // [nwarp][C]
+  long long* wacc = reinterpret_cast<long long*>(smem_raw);           // [C] the block's column sums
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarp = blockDim.x >> 5;
-  long long* wacc = wacc_all + (size_t)warp * C;
-  for (int c = lane; c < C; c += 32) wacc[c] = 0;
-  __syncwarp();
+  for (int c = threadIdx.x; c < C; c += blockDim.x) wacc[c] = 0;
+  __syncthreads();
   uint32_t bad = 0;
   for (long long n = (long long)blockIdx.x * nwarp + warp; n < N; n += (long long)gridDim.x * nwarp)
     row_accumulate(U + (size_t)n * C, C, lane, fxs, -1, 0.f, xi_out ? xi_out + (size_t)n * C : nullptr, wacc, bad);
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    long long s = 0;
-    for (int w = 0; w < nwarp; ++w) s += wacc_all[(size_t)w * C + c];
+    const long long s = wacc[c];
     if (s) atomicAdd(pisum_fx + c, (unsigned long long)s);
   }
   if (bad) atomicOr(flags, bad);
@@ -605,7 +619,7 @@ __global__ void __launch_bounds__(256) k_pi_reduce(float* __restrict__ U, long l
 extern "C" int coda_b200_pi_reduce(float* U, int64_t N, int C, int fx_shift, float* xi_out, int64_t* pisum_fx,
                                    uint32_t* flags, coda_stream_t stream) {
   CODA_CHECK_ARG(U && pisum_fx && flags, "pi_reduce: null pointer");
-  size_t smem = (size_t)8 * C * 8;
+  size_t smem = (size_t)C * 8;
   CODA_CHECK_ARG(smem <= 200 * 1024, "pi_reduce: C=%d too large", C);
   CODA_CUDA_OK(cudaFuncSetAttribute(k_pi_reduce, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   long long want = (N + 7) / 8;
@@ -742,8 +756,9 @@ __global__ void __launch_bounds__(256, 4) k_pi_rank1(const T* __restrict__ preds
                                                   float* __restrict__ U, unsigned long long* __restrict__ pisum_fx,
                                                   uint32_t* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  long long* wacc_all = reinterpret_cast<long long*>(smem_raw);                 // [8][C]
-  R1Term* s_terms = reinterpret_cast<R1Term*>(wacc_all + (size_t)8 * C);        // [nt] gather list (broadcast reads)
+  constexpr int NACC = KC > 0 ? 8 : 1;                                           // KC > 0: one [C] per warp; KC == 0: one
+  long long* wacc_all = reinterpret_cast<long long*>(smem_raw);                 // [NACC][C]   for the block (row_accumulate)
+  R1Term* s_terms = reinterpret_cast<R1Term*>(wacc_all + (size_t)NACC * C);     // [nt] gather list (broadcast reads)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t = (int)sel[1];
   const int nt = hdr[0];
@@ -751,8 +766,11 @@ __global__ void __launch_bounds__(256, 4) k_pi_rank1(const T* __restrict__ preds
   if (!CONST_TERMS)
     for (int k = threadIdx.x; k < nt; k += blockDim.x) s_terms[k] = gterms[k];
   const R1Term* c_terms = CONST_TERMS ? (c_terms_bank + const_base) : s_terms;
-  long long* wacc = wacc_all + (size_t)warp * C;
-  for (int c = lane; c < C; c += 32) wacc[c] = 0;
+  long long* wacc = wacc_all + (size_t)(KC > 0 ? warp : 0) * C;
+  if (KC > 0)
+    for (int c = lane; c < C; c += 32) wacc[c] = 0;
+  else
+    for (int c = threadIdx.x; c < C; c += blockDim.x) wacc[c] = 0;
   long long racc[KC > 0 ? KC : 1];
 #pragma unroll
   for (int k = 0; k < (KC > 0 ? KC : 1); ++k) racc[k] = 0;
@@ -805,7 +823,7 @@ __global__ void __launch_bounds__(256, 4) k_pi_rank1(const T* __restrict__ preds
   __syncthreads();          // every warp's column sums are in shared memory
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     long long s2 = 0;
-    for (int w = 0; w < 8; ++w) s2 += wacc_all[(size_t)w * C + c];
+    for (int w = 0; w < NACC; ++w) s2 += wacc_all[(size_t)w * C + c];
     if (s2) atomicAdd(pisum_fx + c, (unsigned long long)s2);
   }
   if (bad) atomicOr(flags, bad);
@@ -821,7 +839,7 @@ static int pi_rank1(const T* preds, const float* ensb, int H, int64_t N, int C, 
   const int32_t* hdr = terms;                                                  // 2 ints
   const R1Term* tlist = reinterpret_cast<const R1Term*>(terms + 2);            // <= 2H x 16 bytes
   cudaStream_t st = as_stream(stream);
-  size_t smem = (size_t)8 * C * 8 + (size_t)2 * H * sizeof(R1Term);
+  size_t smem = (size_t)(C <= 128 ? 8 : 1) * C * 8 + (size_t)2 * H * sizeof(R1Term);   // NACC of the KC chosen below
   CODA_CHECK_ARG(smem <= 200 * 1024, "pi_rank1: C=%d too large", C);
   long long want = (N + R1_TN - 1) / R1_TN;
   if (ctas_per_sm < 1 || ctas_per_sm > 8) ctas_per_sm = 8;

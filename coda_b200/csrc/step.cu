@@ -184,7 +184,8 @@ extern "C" int coda_b200_step_mixture(const coda_step_t* st, const coda_xchg_t* 
   CODA_CHECK_ARG(st->pisum_fx && st->PB && st->pi_hat && st->m0 && st->h_before && st->best_model, "step_mixture: null pointer");
   XchgView v;
   if (int rc = xchg_view_from(x, &v)) return rc;
-  const size_t smem = (size_t)xch_align16((uint32_t)st->C * 8) + (size_t)st->C * 4;
+  const size_t smem = (size_t)xch_align16((uint32_t)st->C * 8) + (size_t)st->C * 4;   // 48 KB at C = 4096: over the default
+  CODA_CUDA_OK(cudaFuncSetAttribute(k_step_mixture, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_step_mixture<<<1, ST_THREADS, smem, as_stream(stream)>>>(*st, v);
   CODA_LAUNCH_OK("k_step_mixture");
   return CODA_B200_OK;

@@ -1,11 +1,19 @@
 import os
 
 from coda_b200.datasets import Dataset as _Dataset
+from coda_b200.datasets import shard_load_count
 
 
 class Dataset(_Dataset):
     """reference coda/datasets.py.  ``CODA_B200_KEEP_DTYPE=1`` keeps a stored fp16 / bf16 slab at its width (half the
-    device memory, the same results as the fp32 widening)."""
+    device memory, the same results as the fp32 widening).  ``CODA_B200_SHARD_LOAD=1``, or a slab larger than the
+    target device's free memory with more than one GPU visible, loads it as N-range pieces over the GPUs
+    (``coda_b200.datasets.ShardedSlab``; ``CODA_B200_GPUS`` pieces, else one per visible GPU)."""
 
     def __init__(self, filepath, device):
-        super().__init__(filepath, device, keep_dtype=os.environ.get("CODA_B200_KEEP_DTYPE", "0") == "1")
+        keep = os.environ.get("CODA_B200_KEEP_DTYPE", "0") == "1"
+        shards = shard_load_count(filepath, device, keep)
+        if shards:
+            super().__init__(filepath, device, keep_dtype=keep, shards=shards)
+        else:
+            super().__init__(filepath, device, keep_dtype=keep)

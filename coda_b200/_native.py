@@ -185,6 +185,8 @@ SIGNATURES = {
     "coda_b200_sample_fill": (i32, [p, i32, p, i32, i32, p, p, p, p, p, p, p, p, p, p]),
     "coda_b200_sample_gains": (i32, [p, p, p, i64, p, i32, i32, p, p, p, p, p]),
     "coda_b200_sample_eig": (i32, [p, i32, p, p, i32, i32, p, p, p, p, p, i32, p, p, p]),
+    "coda_b200_true_loss_counts": (i32, [p, i32, i64, i32, i64, i32, p, p, p]),
+    "coda_b200_preload_kernels": (i32, [p]),
 }
 
 

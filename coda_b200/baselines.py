@@ -40,7 +40,7 @@ import torch
 
 from . import _native as nat
 from .base import ModelSelector
-from .dist import InProcessGroup, ProcessGroup, SoloGroup, default_comm, split_slab
+from .dist import InProcessGroup, ProcessGroup, SoloGroup, default_comm, piece_layout, split_slab
 from .selector import _Unlabeled
 
 _NO_CPU = ("coda_b200.baselines: dataset.preds must be a CUDA tensor on an sm_90a device; there is no CPU path in this "
@@ -467,8 +467,13 @@ def _check_rank_ranges(preds, n_offset, N, n_global, comm):
 
 def _layout(dataset, gpus, shards, comm):
     """-> (group, [(shard slab, n_offset)] of this process)."""
-    from .datasets import CompactSlab
+    from .datasets import CompactSlab, ShardedSlab
     preds = getattr(dataset, "preds", None)
+    if isinstance(preds, ShardedSlab):                     # the pieces are the shards
+        layout = piece_layout(preds, gpus, shards, comm.world)
+        if not preds.is_cuda:
+            raise NotImplementedError(_NO_CPU)
+        return (SoloGroup() if len(layout) == 1 else InProcessGroup(len(layout))), layout
     if not ((isinstance(preds, torch.Tensor) or isinstance(preds, CompactSlab)) and preds.is_cuda):
         raise NotImplementedError(_NO_CPU)
     n_offset = int(getattr(dataset, "n_offset", 0))
@@ -1131,7 +1136,8 @@ class ModelPicker(_Baseline):
         elif self.state.compact is not None:
             preds = self.state.hard[int(chosen_idx)].to(torch.int64) & 0xFFFF
         else:
-            preds = self.dataset.preds[:, chosen_idx].argmax(dim=1)
+            st = self.state                                   # the one shard's slab (a ShardedSlab's only piece)
+            preds = st.preds[:, int(chosen_idx) - st.n_offset].argmax(dim=1)
         self.correct_counts += (preds == true_class).long()
         self.posterior = self.update_posterior(self.posterior, preds, true_class, self.gamma)
 

@@ -1623,3 +1623,5 @@ extern "C" int coda_b200_pyrandom_run(uint32_t* state, const int64_t* ops, int n
   CODA_LAUNCH_OK("k_pyrandom_run");
   return CODA_B200_OK;
 }
+
+CODA_MODULE_ANCHOR(baselines, k_static_scores)

@@ -193,3 +193,5 @@ extern "C" int coda_b200_torch_rng_run(uint32_t* cpu_rng, int64_t* cuda_rng, con
   CODA_LAUNCH_OK("k_torch_rng_run");
   return CODA_B200_OK;
 }
+
+CODA_MODULE_ANCHOR(bl_ref, k_bl_draw_ref)

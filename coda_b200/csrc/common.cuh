@@ -45,6 +45,11 @@ void coda_set_error(const char* fmt, ...);
 
 static inline cudaStream_t as_stream(coda_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 
+// One kernel of a translation unit (each unit is a module of its own): coda_b200_preload_kernels (preload.cu) finds the
+// unit's module through it and loads all of the unit's kernels.
+#define CODA_MODULE_ANCHOR(unit, kernel) \
+  extern "C" const void* coda_anchor_##unit(void) { return reinterpret_cast<const void*>(&kernel); }
+
 // ---- slab element types ----------------------------------------------------------------
 // The prediction slab may be stored as fp32, fp16 or bf16 (CODA_B200_SLAB_*).  Every kernel that reads it widens the
 // value to fp32 at the load and does the rest in fp32, so a 16-bit slab gives the bits of its exact fp32 widening.

@@ -691,3 +691,5 @@ extern "C" int coda_b200_pi_rank1_index(const int64_t* offsets, const void* entr
   CODA_LAUNCH_OK("k_r1i_rows");
   return CODA_B200_OK;
 }
+
+CODA_MODULE_ANCHOR(compact, k_transpose_D)

@@ -375,3 +375,5 @@ extern "C" int coda_b200_pool_accuracy(const uint16_t* hard, const int64_t* labe
   CODA_LAUNCH_OK("k_pool_accuracy");
   return CODA_B200_OK;
 }
+
+CODA_MODULE_ANCHOR(eps_search, k_mp_runs)

@@ -484,3 +484,5 @@ extern "C" int coda_b200_ell_build(const int32_t* ent_off, const int32_t* ent_ro
   CODA_LAUNCH_OK("k_ell_build");
   return CODA_B200_OK;
 }
+
+CODA_MODULE_ANCHOR(gain, k_ell_build)

@@ -398,3 +398,5 @@ extern "C" int coda_b200_pair_rows(const int32_t* tiles, int tile_lo, int tile_h
   return CODA_B200_OK;
 }
 
+
+CODA_MODULE_ANCHOR(pairs, k_pair_count)

@@ -373,3 +373,5 @@ extern "C" int coda_b200_pair_rows_tc(const int32_t* tiles128, int tile_lo, int 
   CODA_LAUNCH_OK("k_pair_rows_tc");
   return CODA_B200_OK;
 }
+
+CODA_MODULE_ANCHOR(pairs_tc, k_pair_rows_tc)

@@ -393,3 +393,5 @@ extern "C" int coda_b200_pi_full_tc_x(const void* preds, int fmt, int64_t model_
     return pi_full_tc(p, fmt, model_stride, D, H, N, C, U, scratch, flags, stream);
   });
 }
+
+CODA_MODULE_ANCHOR(pi_tc, k_pi_w_max)

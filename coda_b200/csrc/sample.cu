@@ -380,3 +380,5 @@ extern "C" int coda_b200_sample_eig(const int32_t* items, int m, const int32_t* 
   CODA_LAUNCH_OK("k_sample_eig_warp");
   return CODA_B200_OK;
 }
+
+CODA_MODULE_ANCHOR(sample, k_sample_plan)

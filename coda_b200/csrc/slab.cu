@@ -891,3 +891,5 @@ extern "C" int coda_b200_pi_rank1_x(const void* preds, int fmt, const float* ens
                     fx_shift, terms, U, pisum_fx, flags, ctas_per_sm, const_slot, stream);
   });
 }
+
+CODA_MODULE_ANCHOR(slab, k_init_dirichlets)

@@ -285,3 +285,5 @@ extern "C" int coda_b200_report_gather(const int64_t* rep, int rep_words, int64_
   CODA_LAUNCH_OK("k_report_gather");
   return CODA_B200_OK;
 }
+
+CODA_MODULE_ANCHOR(step, k_step_mixture)

@@ -7,3 +7,5 @@ extern "C" int coda_b200_step_select_defer(const coda_step_t* st, const coda_xch
   CODA_CHECK_ARG(pending, "step_select_defer: null pending word");
   return launch_select<true>(st, x, 1, stream, pending);
 }
+
+CODA_MODULE_ANCHOR(step_defer, k_step_select<true>)

@@ -254,3 +254,5 @@ extern "C" int coda_b200_beta_tables(const float* D, const float* grid_x, int H,
   return CODA_B200_OK;
 }
 
+
+CODA_MODULE_ANCHOR(tables, k_beta_nodes)

@@ -17,14 +17,198 @@ def _slab_dtype(t: torch.Tensor, keep_dtype: bool) -> torch.dtype:
     return t.dtype if keep_dtype and t.dtype in _KEPT_DTYPES else torch.float32
 
 
+class ShardedSlab:
+    """An (H, N, C) slab held as contiguous N-range pieces, one dense (H, N_i, C) tensor per piece, each on its own
+    device (consecutive pieces may share one).  The pieces ARE the shard layout: CODA and the competing selectors run
+    one shard per piece, in place.  Duck-types the tensor attributes the selectors and main.py read from
+    ``dataset.preds``; ``device`` is the first piece's."""
+
+    def __init__(self, pieces):
+        pieces = list(pieces)
+        if not pieces:
+            raise ValueError("ShardedSlab: at least one piece expected")
+        for p in pieces:
+            if isinstance(p, CompactSlab) or not isinstance(p, torch.Tensor):
+                raise TypeError("ShardedSlab: pieces must be dense (H, N_i, C) tensors; a compact ShardedSlab is not "
+                                "supported")
+            if p.dim() != 3 or p.dtype not in _KEPT_DTYPES:
+                raise TypeError(f"ShardedSlab: pieces must be float32, float16 or bfloat16 (H, N_i, C) tensors, got "
+                                f"{p.dtype} {tuple(p.shape)}")
+            if not p.is_contiguous() or p.shape[1] < 1:
+                raise ValueError("ShardedSlab: every piece must be a contiguous tensor with at least one item")
+        H, _, C = pieces[0].shape
+        if any(p.shape[0] != H or p.shape[2] != C or p.dtype != pieces[0].dtype for p in pieces):
+            raise TypeError("ShardedSlab: all pieces must share one dtype, H and C")
+        self.pieces = pieces
+        self.offsets = []
+        n = 0
+        for p in pieces:
+            self.offsets.append(n)
+            n += int(p.shape[1])
+        self.shape = torch.Size([int(H), n, int(C)])
+        self.device = pieces[0].device
+        self.dtype = pieces[0].dtype
+        self.is_cuda = pieces[0].is_cuda
+
+    def layout(self):
+        """[(piece, n_offset)]: the shard layout selectors build from."""
+        return list(zip(self.pieces, self.offsets))
+
+    def numel(self):
+        return self.shape[0] * self.shape[1] * self.shape[2]
+
+    def element_size(self):
+        return self.pieces[0].element_size()
+
+    def item_column(self, idx) -> torch.Tensor:
+        """The (H, C) float32 scores of item ``idx``, on the device of the piece that holds it."""
+        idx = int(idx)
+        if not 0 <= idx < self.shape[1]:
+            raise IndexError(f"ShardedSlab: item {idx} outside [0, {self.shape[1]})")
+        r = max(i for i, off in enumerate(self.offsets) if off <= idx)
+        return self.pieces[r][:, idx - self.offsets[r]].float()
+
+
+def piece_plan(N, nshards, ngpus, home, device_count):
+    """[(lo, hi, device index)] of ``nshards`` N-range pieces: the ranges ``shard_range(N, r, nshards)`` and the device
+    assignment of ``dist.split_slab`` -- the home device first, consecutive pieces sharing a device when there are more
+    pieces than GPUs."""
+    devs = [home] + [d for d in range(device_count) if d != home]
+    devs = devs[:max(1, ngpus)]
+    return [(*shard_range(N, r, nshards), devs[r * len(devs) // nshards]) for r in range(nshards)]
+
+
+def chunk_walk(lo, hi, C, esz, chunk_bytes):
+    """[(a, b)] element ranges of one model's items [lo, hi) (the elements [lo*C, hi*C) of that model), at most
+    ``chunk_bytes`` each (at least one element)."""
+    step = max(1, int(chunk_bytes) // int(esz))
+    a, end = lo * C, hi * C
+    out = []
+    while a < end:
+        out.append((a, min(end, a + step)))
+        a = out[-1][1]
+    return out
+
+
+DEFAULT_CHUNK_BYTES = 64 << 20
+
+
+def _open_mmap(filepath):
+    import zipfile
+    if not zipfile.is_zipfile(filepath):
+        raise ValueError(f"{filepath}: a sharded load memory-maps the file, which needs torch.save's zip format; this "
+                         f"file is in the legacy format -- re-save it with torch.save(torch.load(path), path)")
+    full = torch.load(filepath, map_location="cpu", mmap=True, weights_only=True)
+    if not isinstance(full, torch.Tensor) or full.dim() != 3:
+        raise ValueError(f"{filepath}: expected an (H, N, C) tensor")
+    if not full.is_contiguous():
+        raise ValueError(f"{filepath}: the saved (H, N, C) tensor is not contiguous, so a model's items are not one "
+                         f"contiguous range of the file; re-save it with torch.save(t.contiguous(), path)")
+    return full
+
+
+def _fill_device(full, todo, dtype, chunk_bytes):
+    """Fill the pieces ``todo`` = [(piece, lo, hi)] of one device model by model: each model's range is one contiguous
+    read of the file, staged through two pinned chunks; a 16-bit file read into fp32 pieces is widened on the device."""
+    dev = todo[0][0].device
+    H, _, C = full.shape
+    src_t = full.dtype
+    esz = full.element_size()
+    step = max(1, int(chunk_bytes) // esz)
+    pins = [torch.empty(step, dtype=src_t, pin_memory=True) for _ in range(2)]
+    done = [None, None]
+    with torch.cuda.device(dev):
+        stream = torch.cuda.Stream(device=dev)
+        stage = torch.empty(step, dtype=src_t, device=dev) if src_t != dtype else None
+        flat = full.view(H, -1)
+        k = 0
+        with torch.cuda.stream(stream):
+            for piece, lo, hi in todo:
+                dst = piece.view(H, -1)
+                for h in range(H):
+                    for a, b in chunk_walk(lo, hi, C, esz, chunk_bytes):
+                        j = k % 2
+                        if done[j] is not None:
+                            done[j].synchronize()             # the copy that last read this pinned chunk is over
+                        n = b - a
+                        pins[j][:n].copy_(flat[h, a:b])
+                        out = dst[h, a - lo * C:b - lo * C]
+                        if stage is None:
+                            out.copy_(pins[j][:n], non_blocking=True)
+                        else:
+                            stage[:n].copy_(pins[j][:n], non_blocking=True)
+                            out.copy_(stage[:n])                # fp16 / bf16 -> fp32 is exact
+                        done[j] = torch.cuda.Event()
+                        done[j].record(stream)
+                        k += 1
+        stream.synchronize()
+        del stage
+
+
+def load_sharded(filepath, device, keep_dtype=False, shards=None, gpus=None, chunk_bytes=DEFAULT_CHUNK_BYTES):
+    """``filepath``'s (H, N, C) slab as a ``ShardedSlab`` of ``shards`` pieces over ``gpus`` devices, read through a
+    memory map: no device ever holds more than its pieces plus one staging chunk, and host memory holds two pinned
+    chunks per device.  Every piece equals ``torch.load(filepath)[:, lo:hi]`` at the slab dtype (see ``Dataset``)."""
+    import concurrent.futures as cf
+    full = _open_mmap(filepath)
+    H, N, C = (int(s) for s in full.shape)
+    dtype = _slab_dtype(full, keep_dtype)
+    nshards = int(shards) if shards else int(gpus)
+    ngpus = int(gpus) if gpus else min(nshards, max(1, torch.cuda.device_count()))
+    nshards = max(1, min(nshards, N))
+    dev = torch.device(device)
+    home = dev.index if dev.index is not None else torch.cuda.current_device()
+    plan = piece_plan(N, nshards, ngpus, home, torch.cuda.device_count())
+    pieces, by_dev = [], {}
+    for lo, hi, d in plan:
+        p = torch.empty((H, hi - lo, C), dtype=dtype, device=torch.device("cuda", d))
+        pieces.append(p)
+        by_dev.setdefault(d, []).append((p, lo, hi))
+    with cf.ThreadPoolExecutor(max_workers=len(by_dev)) as ex:     # one host thread per device
+        for f in [ex.submit(_fill_device, full, todo, dtype, chunk_bytes) for todo in by_dev.values()]:
+            f.result()
+    return ShardedSlab(pieces)
+
+
+def _free_bytes(index):
+    return torch.cuda.mem_get_info(index)[0]
+
+
+def shard_load_count(filepath, device, keep_dtype=False, env=None):
+    """How many pieces ``coda.datasets.Dataset`` loads ``filepath`` into: 0 for a plain load.  Sharded when
+    ``CODA_B200_SHARD_LOAD=1``, or when the slab (at the width it would be held) exceeds the free memory of the target
+    device and more than one GPU is visible.  The count is ``CODA_B200_GPUS`` if set, else the visible GPUs."""
+    env = os.environ if env is None else env
+    ngpus = torch.cuda.device_count()
+    count = max(1, int(env["CODA_B200_GPUS"])) if env.get("CODA_B200_GPUS") else max(1, ngpus)
+    if env.get("CODA_B200_SHARD_LOAD", "0") == "1":
+        return count
+    dev = torch.device(device)
+    if dev.type != "cuda" or ngpus < 2:
+        return 0
+    try:
+        full = _open_mmap(filepath)
+    except Exception:                                              # legacy format: keep the plain load
+        return 0
+    nbytes = full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep_dtype)).element_size()
+    index = dev.index if dev.index is not None else torch.cuda.current_device()
+    return count if nbytes > _free_bytes(index) else 0
+
+
 class Dataset:
     """(H, N, C) post-softmax scores from ``filepath`` (+ optional ``*_labels.pt``), forced to fp32
-    (coda/datasets.py:12-23).  ``keep_dtype=True`` keeps a stored fp16 or bf16 slab at its width."""
+    (coda/datasets.py:12-23).  ``keep_dtype=True`` keeps a stored fp16 or bf16 slab at its width.
 
-    def __init__(self, filepath, device, keep_dtype=False):
+    With ``shards=`` / ``gpus=`` the slab is loaded as a ``ShardedSlab`` of N-range pieces over the GPUs
+    (``load_sharded``) and never held whole on one device; ``chunk_bytes`` bounds its staging chunks."""
+
+    def __init__(self, filepath, device, keep_dtype=False, *, shards=None, gpus=None, chunk_bytes=DEFAULT_CHUNK_BYTES):
         self.device = device
-        preds = torch.load(filepath, map_location=device)
-        self.preds = preds.to(_slab_dtype(preds, keep_dtype)).contiguous()
+        if shards or gpus:
+            self.preds = load_sharded(filepath, device, keep_dtype, shards=shards, gpus=gpus, chunk_bytes=chunk_bytes)
+        else:
+            preds = torch.load(filepath, map_location=device)
+            self.preds = preds.to(_slab_dtype(preds, keep_dtype)).contiguous()
         print("Loaded preds of shape", self.preds.shape)
         self.labels = None
         label_p = filepath.replace(".pt", "_labels.pt")

@@ -73,6 +73,19 @@ class TorchComm:
         self.dist.barrier(group=self.group)
 
 
+def preload_kernels() -> int:
+    """Load every kernel of the library into the current device's context (once per device and process)."""
+    d = torch.cuda.current_device()
+    if d not in _PRELOADED:
+        n = ct.c_int64(0)
+        nat.check(nat.load().coda_b200_preload_kernels(ct.byref(n)), "preload_kernels")
+        _PRELOADED[d] = int(n.value)
+    return _PRELOADED[d]
+
+
+_PRELOADED = {}
+
+
 def default_comm():
     import torch.distributed as dist
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
@@ -134,6 +147,24 @@ class Mailbox:
                     self.ptr = 0
         except Exception:
             pass
+
+
+def piece_layout(slab, gpus, shards, world):
+    """A ``ShardedSlab`` is its own shard layout: [(piece, n_offset)], used in place (no peer copy, no re-split, and
+    ``CODA_B200_GPUS`` is not consulted).  ``shards=`` (or ``gpus=`` alone) must equal the piece count, ``gpus=`` with
+    ``shards=`` the number of devices the pieces are on."""
+    if world > 1:
+        raise ValueError("coda_b200: a ShardedSlab holds the whole task in one process; under torch.distributed with "
+                         "world > 1 every rank passes its own N-range tensor (e.g. ShardedFileDataset)")
+    k = len(slab.pieces)
+    want = shards or gpus
+    if want and int(want) != k:
+        raise ValueError(f"coda_b200: the ShardedSlab has {k} pieces, one shard each; "
+                         f"{'shards' if shards else 'gpus'}={want} disagrees")
+    ndev = len({p.device for p in slab.pieces})
+    if shards and gpus and int(gpus) != ndev:
+        raise ValueError(f"coda_b200: the ShardedSlab's pieces are on {ndev} devices; gpus={gpus} disagrees")
+    return slab.layout()
 
 
 def split_slab(preds, nshards, ngpus):
@@ -235,6 +266,9 @@ class InProcessGroup:
         self._engines = list(engines)
         lib = nat.load()
         devs = sorted({e.dev.index for e in engines})
+        for d in devs:                      # before any exchange kernel spins (csrc/preload.cu): no first-launch load waits
+            with torch.cuda.device(d):      # for a peer that is waiting for this shard
+                preload_kernels()
         for a in devs:
             for b in devs:
                 if a != b:

@@ -1,4 +1,8 @@
 """Label oracle (reference coda/oracle.py:1-24)."""
+import ctypes as ct
+
+import numpy as np
+import torch
 
 
 class Oracle:
@@ -10,9 +14,66 @@ class Oracle:
         assert self.labels is not None, "Oracle needs labels!"
 
     def true_losses(self, preds):
-        """Mean loss of every model, (H,) (coda/oracle.py:9-21)."""
+        """Mean loss of every model, (H,) (coda/oracle.py:9-21).  A ``ShardedSlab`` takes the accuracy loss only, on
+        the pieces' devices (``sharded_true_losses``)."""
+        from .datasets import ShardedSlab
+        if isinstance(preds, ShardedSlab):
+            return sharded_true_losses(preds, self.labels, self.loss_fn, self.dataset.device)
         H, N, C = preds.shape
         return self.loss_fn(preds.reshape(-1, C), self.labels.repeat(H), reduction="none").view(H, N).mean(dim=1)
 
     def __call__(self, idx):
         return self.labels[idx].item()
+
+
+def mean_factor(H, N):
+    """The fp32 factor torch's CUDA mean over the last dim of an (H, N) fp32 tensor multiplies its sum by
+    (ReduceMomentKernel.cu: ``float(num_output_elements) / numel``, MeanOps::project is ``a * factor``)."""
+    return np.float32(H) / np.float32(H * N)
+
+
+def sharded_true_losses(slab, labels, loss_fn, device):
+    """``Oracle.true_losses`` of a ``ShardedSlab`` with the accuracy loss: one ``coda_b200_true_loss_counts`` launch per
+    piece, each on its device and a stream of its own, all in flight together.  The per-model wrong counts are exact
+    integers below 2^24, so they equal torch's fp32 sums; the result carries the bits of ``true_losses`` on the same
+    slab held as one tensor, on ``device``."""
+    from . import _native as nat
+    try:
+        from coda.options import accuracy_loss                # what LOSS_FNS["acc"] resolves to
+    except ImportError:
+        accuracy_loss = None
+    if accuracy_loss is None or loss_fn is not accuracy_loss:
+        raise NotImplementedError("Oracle.true_losses on a ShardedSlab takes the accuracy loss only "
+                                  "(coda.options.accuracy_loss, LOSS_FNS['acc'])")
+    if labels.dim() != 1:
+        raise NotImplementedError("Oracle.true_losses on a ShardedSlab takes 1-D class labels")
+    H, N, C = (int(s) for s in slab.shape)
+    if N >= 1 << 24:
+        raise NotImplementedError(f"Oracle.true_losses on a ShardedSlab: N = {N} >= 2^24, where fp32 sums of the "
+                                  f"per-item losses stop being exact counts")
+    if not slab.is_cuda:
+        raise NotImplementedError("coda_b200: the pieces of a ShardedSlab must be CUDA tensors; there is no CPU path")
+    lib = nat.load()
+    fmt = nat.slab_format(slab.dtype)
+    labels = labels.to(torch.int64)
+    parts = []
+    for piece, off in slab.layout():
+        dev = piece.device
+        with torch.cuda.device(dev):
+            st = torch.cuda.Stream(device=dev)
+            st.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(st):
+                lab = labels[off:off + piece.shape[1]].to(dev, non_blocking=False)
+                cnt = torch.empty(H, dtype=torch.int64, device=dev)
+                nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(piece.data_ptr()), fmt, int(piece.stride(0)), H,
+                                                         int(piece.shape[1]), C, ct.c_void_p(lab.data_ptr()),
+                                                         ct.c_void_p(cnt.data_ptr()), ct.c_void_p(st.cuda_stream)),
+                          "true_loss_counts")
+                lab.record_stream(st)
+        parts.append((cnt, st))
+    correct = torch.zeros(H, dtype=torch.int64, device=device)
+    for cnt, st in parts:
+        st.synchronize()
+        correct += cnt.to(device)
+    wrong = (N - correct).to(torch.float32)                 # sum of the 0/1 losses, exact
+    return wrong * torch.tensor(mean_factor(H, N), device=device)

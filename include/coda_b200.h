@@ -633,6 +633,20 @@ int coda_b200_majority(const uint16_t* hard, int H, int64_t N, int64_t* labels, 
 int coda_b200_pool_accuracy(const uint16_t* hard, const int64_t* labels, int H, const int64_t* pool, int64_t R, int P,
                             int32_t* acc, coda_stream_t stream);
 
+/* ---- true losses of a slab held as N-range pieces (coda/oracle.py:9-21 with coda/options.py's accuracy loss) --------
+ * counts[h] = number of items n of this piece with argmax_c preds[h][n][c] == labels[n], argmax as torch.argmax decides it
+ * on the device (first index of the maximum, a NaN is the maximum); a label outside [0, C) never matches.  preds is a
+ * CODA_B200_SLAB_* slab [H][N][C] with models `model_stride` elements apart, read at its stored width; labels [N] int64.
+ * counts [H] int64 is zeroed on `stream` first; the sums are exact, so they are the same for any split of the items. */
+/* ---- module loading --------------------------------------------------------------------------------------------------
+ * Load every kernel of this library into the current device's context now (*loaded_host = how many).  Under CUDA's lazy
+ * loading a kernel's first launch loads its code and can wait for the kernels running on the device; shards that share
+ * a GPU spin on each other inside the step kernels, so an in-process group calls this before any exchange can spin. */
+int coda_b200_preload_kernels(int64_t* loaded_host);
+
+int coda_b200_true_loss_counts(const void* preds, int fmt, int64_t model_stride, int H, int64_t N, int C,
+                               const int64_t* labels, int64_t* counts, coda_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

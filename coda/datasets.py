@@ -1,17 +1,28 @@
 import os
 
 from coda_b200.datasets import Dataset as _Dataset
-from coda_b200.datasets import shard_load_count
+from coda_b200.datasets import compact_load_count, is_compact_file, shard_load_count
 
 
 class Dataset(_Dataset):
     """reference coda/datasets.py.  ``CODA_B200_KEEP_DTYPE=1`` keeps a stored fp16 / bf16 slab at its width (half the
     device memory, the same results as the fp32 widening).  ``CODA_B200_SHARD_LOAD=1``, or a slab larger than the
     target device's free memory with more than one GPU visible, loads it as N-range pieces over the GPUs
-    (``coda_b200.datasets.ShardedSlab``; ``CODA_B200_GPUS`` pieces, else one per visible GPU)."""
+    (``coda_b200.datasets.ShardedSlab``; ``CODA_B200_GPUS`` pieces, else one per visible GPU).
+
+    A file written by ``coda_b200.CompactSlab.save`` loads as a compact slab, and ``CODA_B200_COMPACT_K=K`` compacts a
+    dense task file to its top-K form as it loads (opt-in: the compact form approximates the tail classes, so results
+    differ from the dense run).  The piece count follows the same rule on the compact byte count
+    (``coda_b200.datasets.ShardedCompactSlab`` for more than one piece)."""
 
     def __init__(self, filepath, device):
         keep = os.environ.get("CODA_B200_KEEP_DTYPE", "0") == "1"
+        k = os.environ.get("CODA_B200_COMPACT_K")
+        k = int(k) if k else None
+        if k or is_compact_file(filepath):
+            shards = compact_load_count(filepath, device, k)
+            super().__init__(filepath, device, compact_k=k, shards=shards or None)
+            return
         shards = shard_load_count(filepath, device, keep)
         if shards:
             super().__init__(filepath, device, keep_dtype=keep, shards=shards)

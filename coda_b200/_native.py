@@ -187,6 +187,8 @@ SIGNATURES = {
     "coda_b200_sample_eig": (i32, [p, i32, p, p, i32, i32, p, p, p, p, p, i32, p, p, p]),
     "coda_b200_true_loss_counts": (i32, [p, i32, i64, i32, i64, i32, p, p, p]),
     "coda_b200_preload_kernels": (i32, [p]),
+    "coda_b200_compact_build": (i32, [p, i32, i64, i32, i64, i32, i32, p, p, i64, p, p, p, p]),
+    "coda_b200_true_loss_counts_compact": (i32, [p, i64, i32, i64, i32, p, p, p]),
 }
 
 

@@ -467,9 +467,9 @@ def _check_rank_ranges(preds, n_offset, N, n_global, comm):
 
 def _layout(dataset, gpus, shards, comm):
     """-> (group, [(shard slab, n_offset)] of this process)."""
-    from .datasets import CompactSlab, ShardedSlab
+    from .datasets import CompactSlab, ShardedCompactSlab, ShardedSlab
     preds = getattr(dataset, "preds", None)
-    if isinstance(preds, ShardedSlab):                     # the pieces are the shards
+    if isinstance(preds, (ShardedSlab, ShardedCompactSlab)):    # the pieces are the shards
         layout = piece_layout(preds, gpus, shards, comm.world)
         if not preds.is_cuda:
             raise NotImplementedError(_NO_CPU)

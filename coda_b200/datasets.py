@@ -1,6 +1,7 @@
 """Datasets: the reference loader contract (coda/datasets.py:4-23) plus shard-aware variants."""
 from __future__ import annotations
 
+import ctypes as ct
 import os
 
 import torch
@@ -174,10 +175,9 @@ def _free_bytes(index):
     return torch.cuda.mem_get_info(index)[0]
 
 
-def shard_load_count(filepath, device, keep_dtype=False, env=None):
-    """How many pieces ``coda.datasets.Dataset`` loads ``filepath`` into: 0 for a plain load.  Sharded when
-    ``CODA_B200_SHARD_LOAD=1``, or when the slab (at the width it would be held) exceeds the free memory of the target
-    device and more than one GPU is visible.  The count is ``CODA_B200_GPUS`` if set, else the visible GPUs."""
+def _piece_count(held_bytes, device, env):
+    """The shim's piece-count rule: ``CODA_B200_GPUS`` (else the visible GPUs) pieces when ``CODA_B200_SHARD_LOAD=1``,
+    or when ``held_bytes()`` exceeds the free memory of the target device and more than one GPU is visible; else 0."""
     env = os.environ if env is None else env
     ngpus = torch.cuda.device_count()
     count = max(1, int(env["CODA_B200_GPUS"])) if env.get("CODA_B200_GPUS") else max(1, ngpus)
@@ -187,12 +187,215 @@ def shard_load_count(filepath, device, keep_dtype=False, env=None):
     if dev.type != "cuda" or ngpus < 2:
         return 0
     try:
-        full = _open_mmap(filepath)
+        nbytes = held_bytes()
     except Exception:                                              # legacy format: keep the plain load
         return 0
-    nbytes = full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep_dtype)).element_size()
     index = dev.index if dev.index is not None else torch.cuda.current_device()
     return count if nbytes > _free_bytes(index) else 0
+
+
+def shard_load_count(filepath, device, keep_dtype=False, env=None):
+    """How many pieces ``coda.datasets.Dataset`` loads ``filepath`` into: 0 for a plain load.  Sharded when
+    ``CODA_B200_SHARD_LOAD=1``, or when the slab (at the width it would be held) exceeds the free memory of the target
+    device and more than one GPU is visible.  The count is ``CODA_B200_GPUS`` if set, else the visible GPUs."""
+    def held():
+        full = _open_mmap(filepath)
+        return full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep_dtype)).element_size()
+    return _piece_count(held, device, env)
+
+
+def compact_load_count(filepath, device, K=None, env=None):
+    """``shard_load_count``'s rule for a compact load of ``filepath`` (a ``CompactSlab.save`` file, or a dense file
+    compacted at ``K``), applied to the compact byte count: 0 means one piece."""
+    def held():
+        obj = _open_compact(filepath)
+        if obj is not None:
+            return obj["ids"].numel() * 6
+        H, N, _ = _open_mmap(filepath).shape
+        return int(H) * int(N) * int(K) * 6
+    return _piece_count(held, device, env)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# compact slabs: built on the device from dense scores (csrc/compact_build.cu), saved and loaded as pieces
+# ---------------------------------------------------------------------------------------------------------------------
+COMPACT_FORMAT = "coda_b200.compact"
+COMPACT_VERSION = 1
+COMPACT_KS = (1, 2, 3, 4, 8)                    # the instantiated K of csrc/compact.cu and csrc/compact_build.cu
+
+
+def row_walk(lo, hi, C, esz, chunk_bytes):
+    """[(a, b)] item ranges covering [lo, hi) of one model: whole items of C elements of ``esz`` bytes, at most
+    ``chunk_bytes`` of them per range, and at least one item."""
+    step = max(1, int(chunk_bytes) // (int(C) * int(esz)))
+    return [(a, min(hi, a + step)) for a in range(lo, hi, step)]
+
+
+def _open_compact(filepath):
+    """The memory-mapped contents of a ``CompactSlab.save`` file, or None for any other file."""
+    import zipfile
+    if not zipfile.is_zipfile(filepath):
+        return None
+    obj = torch.load(filepath, map_location="cpu", mmap=True, weights_only=True)
+    if not (isinstance(obj, dict) and obj.get("format") == COMPACT_FORMAT):
+        return None
+    if obj.get("version") != COMPACT_VERSION:
+        raise ValueError(f"{filepath}: compact slab format version {obj.get('version')}, this loader reads "
+                         f"{COMPACT_VERSION}")
+    ids, probs = obj["ids"], obj["probs"]
+    if (ids.dim() != 3 or ids.shape != probs.shape or ids.dtype != torch.int16 or probs.dtype != torch.float32
+            or not ids.is_contiguous() or not probs.is_contiguous()):
+        raise ValueError(f"{filepath}: a compact slab file holds contiguous (H, N, K) int16 ids and float32 probs")
+    return obj
+
+
+def is_compact_file(filepath):
+    """True for a file written by ``CompactSlab.save``."""
+    try:
+        return _open_compact(filepath) is not None
+    except ValueError:                                             # a compact file this loader refuses: say why there
+        return True
+    except Exception:                                              # not something torch.load(weights_only) reads
+        return False
+
+
+def _raise_input_flags(flags):
+    from . import _native as nat
+    if flags & nat.FLAG_NONFINITE_INPUT:
+        raise RuntimeError("[NUMERIC ERROR] preds has bad values (NaN/Inf)")
+    if flags & nat.FLAG_RANGE_INPUT:
+        raise ValueError("coda_b200: dataset.preds must hold post-softmax scores in [0, 1] (coda/datasets.py:6)")
+
+
+def _compact_launch(lib, src, fmt, model_stride, H, N, C, K, ids, probs, out_stride, dropped, flat, flags, stream):
+    from . import _native as nat
+    nat.check(lib.coda_b200_compact_build(ct.c_void_p(src), fmt, int(model_stride), int(H), int(N), int(C), int(K),
+                                          ct.c_void_p(ids), ct.c_void_p(probs), int(out_stride), ct.c_void_p(dropped),
+                                          ct.c_void_p(flat), ct.c_void_p(flags), ct.c_void_p(stream)),
+              "compact_build")
+
+
+def _check_k(K, C):
+    if K is None or int(K) not in COMPACT_KS or not int(K) < int(C):
+        raise ValueError(f"coda_b200: compact K must be one of {COMPACT_KS} and below C = {C}, got {K}")
+    if int(C) > 4096:
+        raise ValueError(f"coda_b200: compacting takes C <= 4096 classes, got {C}")
+    return int(K)
+
+
+def _compact_device(full, todo, K, chunk_bytes):
+    """Compact the pieces ``todo`` = [(CompactSlab piece, lo, hi)] of one device from the memory-mapped dense slab
+    ``full``, model by model: whole items are staged through two pinned chunks and one device chunk at the file's dtype,
+    and the kernel writes from that chunk straight into the piece.  -> (dropped_max, flat_rows, flags) of this device."""
+    from . import _native as nat
+    lib = nat.load()
+    dev = todo[0][0].device
+    H, _, C = (int(s) for s in full.shape)
+    esz = full.element_size()
+    fmt = nat.slab_format(full.dtype)
+    step = max(1, int(chunk_bytes) // (C * esz)) * C
+    pins = [torch.empty(step, dtype=full.dtype, pin_memory=True) for _ in range(2)]
+    done = [None, None]
+    flat_src = full.view(H, -1)
+    with torch.cuda.device(dev):
+        stream = torch.cuda.Stream(device=dev)
+        with torch.cuda.stream(stream):
+            stage = torch.empty(step, dtype=full.dtype, device=dev)
+            dropped = torch.zeros(H, dtype=torch.float32, device=dev)
+            flat = torch.zeros(H, dtype=torch.int64, device=dev)
+            flags = torch.zeros(1, dtype=torch.int32, device=dev)
+            k = 0
+            for piece, lo, hi in todo:
+                for h in range(H):
+                    for a, b in row_walk(lo, hi, C, esz, chunk_bytes):
+                        j = k % 2
+                        if done[j] is not None:
+                            done[j].synchronize()             # the copy that last read this pinned chunk is over
+                        n = (b - a) * C
+                        pins[j][:n].copy_(flat_src[h, a * C:b * C])
+                        stage[:n].copy_(pins[j][:n], non_blocking=True)
+                        _compact_launch(lib, stage.data_ptr(), fmt, n, 1, b - a, C, K,
+                                        piece.ids[h, a - lo:].data_ptr(), piece.probs[h, a - lo:].data_ptr(), 0,
+                                        dropped[h:].data_ptr(), flat[h:].data_ptr(), flags.data_ptr(),
+                                        stream.cuda_stream)
+                        done[j] = torch.cuda.Event()
+                        done[j].record(stream)
+                        k += 1
+        stream.synchronize()
+        del stage
+    return dropped, flat, int(flags.item())
+
+
+def _copy_compact_device(obj, todo):
+    """Copy the pieces ``todo`` = [(CompactSlab piece, lo, hi)] of one device out of a memory-mapped compact file, one
+    model's item range at a time."""
+    dev = todo[0][0].device
+    with torch.cuda.device(dev):
+        for piece, lo, hi in todo:
+            for h in range(piece.shape[0]):
+                piece.ids[h].copy_(obj["ids"][h, lo:hi])
+                piece.probs[h].copy_(obj["probs"][h, lo:hi])
+        torch.cuda.synchronize(dev)
+
+
+def load_compact(filepath, device, K=None, *, shards=None, gpus=None, chunk_bytes=DEFAULT_CHUNK_BYTES):
+    """``filepath`` as a compact slab of ``shards`` N-range pieces over ``gpus`` devices (one piece on ``device`` when
+    neither is given): a ``CompactSlab`` for one piece, a ``ShardedCompactSlab`` for more.
+
+    * A ``CompactSlab.save`` file is copied piece by piece out of a memory map; ``K``, if given, must be the file's.
+    * A dense (H, N, C) fp32 / fp16 / bf16 file is compacted at ``K`` on the devices as it streams in (one host thread
+      per device, whole items per chunk of at most ``chunk_bytes``): no device holds more than its compact pieces plus
+      one chunk.  Every piece has the bits of ``CompactSlab.from_dense`` of the whole slab (a 16-bit file: of its fp32
+      widening).  ``slab.compaction`` then holds ``dropped_max`` (H,) fp32, the largest score dropped, and ``flat_rows``
+      (H,) int64, the rows whose remainder reaches ``probs[0]`` (see ``CompactSlab.from_dense``)."""
+    import concurrent.futures as cf
+    obj = _open_compact(filepath)
+    if obj is not None:
+        H, N, Kf = (int(s) for s in obj["ids"].shape)
+        C = int(obj["C"])
+        if K is not None and int(K) != Kf:
+            raise ValueError(f"{filepath}: a compact slab saved at K = {Kf}; K = {K} was asked for")
+        K = Kf
+    else:
+        full = _open_mmap(filepath)
+        H, N, C = (int(s) for s in full.shape)
+        if full.dtype not in _KEPT_DTYPES:
+            raise TypeError(f"{filepath}: compacting takes a float32, float16 or bfloat16 slab, got {full.dtype}")
+        K = _check_k(K, C)
+    nshards = int(shards) if shards else (int(gpus) if gpus else 1)
+    ngpus = int(gpus) if gpus else min(nshards, max(1, torch.cuda.device_count()))
+    nshards = max(1, min(nshards, N))
+    dev = torch.device(device)
+    home = dev.index if dev.index is not None else torch.cuda.current_device()
+    plan = piece_plan(N, nshards, ngpus, home, torch.cuda.device_count())
+    pieces, by_dev = [], {}
+    for lo, hi, d in plan:
+        dd = torch.device("cuda", d)
+        p = CompactSlab(torch.empty((H, hi - lo, K), dtype=torch.int16, device=dd),
+                        torch.empty((H, hi - lo, K), dtype=torch.float32, device=dd), C)
+        pieces.append(p)
+        by_dev.setdefault(d, []).append((p, lo, hi))
+    with cf.ThreadPoolExecutor(max_workers=len(by_dev)) as ex:     # one host thread per device
+        if obj is not None:
+            futs = [ex.submit(_copy_compact_device, obj, todo) for todo in by_dev.values()]
+        else:
+            futs = [ex.submit(_compact_device, full, todo, K, chunk_bytes) for todo in by_dev.values()]
+        outs = [f.result() for f in futs]
+    compaction = None
+    if obj is None:
+        homedev = torch.device("cuda", home)
+        flags = 0
+        dropped = torch.zeros(H, dtype=torch.float32, device=homedev)
+        flat = torch.zeros(H, dtype=torch.int64, device=homedev)
+        for dm, fr, fl in outs:
+            dropped = torch.maximum(dropped, dm.to(homedev))
+            flat += fr.to(homedev)
+            flags |= fl
+        _raise_input_flags(flags)
+        compaction = {"dropped_max": dropped, "flat_rows": flat}
+    slab = pieces[0] if len(pieces) == 1 else ShardedCompactSlab(pieces)
+    slab.compaction = compaction
+    return slab
 
 
 class Dataset:
@@ -200,11 +403,17 @@ class Dataset:
     (coda/datasets.py:12-23).  ``keep_dtype=True`` keeps a stored fp16 or bf16 slab at its width.
 
     With ``shards=`` / ``gpus=`` the slab is loaded as a ``ShardedSlab`` of N-range pieces over the GPUs
-    (``load_sharded``) and never held whole on one device; ``chunk_bytes`` bounds its staging chunks."""
+    (``load_sharded``) and never held whole on one device; ``chunk_bytes`` bounds its staging chunks.
 
-    def __init__(self, filepath, device, keep_dtype=False, *, shards=None, gpus=None, chunk_bytes=DEFAULT_CHUNK_BYTES):
+    A file written by ``CompactSlab.save`` loads as a compact slab, and ``compact_k=K`` compacts a dense file at K as it
+    loads (``load_compact``; a ``ShardedCompactSlab`` with more than one piece)."""
+
+    def __init__(self, filepath, device, keep_dtype=False, *, shards=None, gpus=None, chunk_bytes=DEFAULT_CHUNK_BYTES,
+                 compact_k=None):
         self.device = device
-        if shards or gpus:
+        if compact_k or is_compact_file(filepath):
+            self.preds = load_compact(filepath, device, compact_k, shards=shards, gpus=gpus, chunk_bytes=chunk_bytes)
+        elif shards or gpus:
             self.preds = load_sharded(filepath, device, keep_dtype, shards=shards, gpus=gpus, chunk_bytes=chunk_bytes)
         else:
             preds = torch.load(filepath, map_location=device)
@@ -281,6 +490,49 @@ class CompactSlab:
         self.device = ids.device
         self.is_cuda = ids.is_cuda
         self.dtype = torch.float32
+        self.compaction = None               # from_dense / load_compact: {"dropped_max", "flat_rows"} per model
+
+    @classmethod
+    def from_dense(cls, preds: torch.Tensor, K: int) -> "CompactSlab":
+        """The top-K form of a CUDA (H, N, C) fp32 / fp16 / bf16 slab or N-range view of one, built on its device
+        (``coda_b200_compact_build``): per (h, n) the K highest scores in descending order, equal scores by ascending
+        class, so ``ids[..., 0]`` is ``torch.argmax``'s first-index maximum and ``probs`` the scores' exact fp32 bits.
+        ``K`` in (1, 2, 3, 4, 8), K < C <= 4096.  Non-finite scores or scores outside [0, 1.0001] raise as a dense slab
+        does.
+
+        ``compaction`` holds two per-model diagnostics to choose K by: ``dropped_max`` (H,) fp32, the largest score the
+        compaction drops (the max over items of the (K+1)-th score), and ``flat_rows`` (H,) int64, the items whose
+        uniform remainder ``(1 - sum probs) * fp32(1 / (C - K))`` is >= ``probs[0]`` -- the only items where the arg-max
+        of ``densify()`` can differ from ``ids[0]``."""
+        from . import _native as nat
+        if not (isinstance(preds, torch.Tensor) and preds.dim() == 3 and preds.is_cuda):
+            raise TypeError("CompactSlab.from_dense: a CUDA (H, N, C) tensor expected")
+        fmt = nat.slab_format(preds.dtype)
+        H, N, C = (int(s) for s in preds.shape)
+        K = _check_k(K, C)
+        if not (preds.stride(2) == 1 and preds.stride(1) == C and (H == 1 or preds.stride(0) >= N * C)):
+            raise ValueError("CompactSlab.from_dense: preds must be (H, N, C) with contiguous items")
+        dev = preds.device
+        ids = torch.empty((H, N, K), dtype=torch.int16, device=dev)
+        probs = torch.empty((H, N, K), dtype=torch.float32, device=dev)
+        dropped = torch.zeros(H, dtype=torch.float32, device=dev)
+        flat = torch.zeros(H, dtype=torch.int64, device=dev)
+        flags = torch.zeros(1, dtype=torch.int32, device=dev)
+        if N:
+            with torch.cuda.device(dev):
+                _compact_launch(nat.load(), preds.data_ptr(), fmt, preds.stride(0) if H > 1 else N * C, H, N, C, K,
+                                ids.data_ptr(), probs.data_ptr(), N * K, dropped.data_ptr(), flat.data_ptr(),
+                                flags.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        _raise_input_flags(int(flags.item()))
+        slab = cls(ids, probs, C)
+        slab.compaction = {"dropped_max": dropped, "flat_rows": flat}
+        return slab
+
+    def save(self, path):
+        """Write this slab as a ``torch.save`` zip file ``{"format": "coda_b200.compact", "version": 1, "ids", "probs",
+        "C"}``; ``load_compact`` (and the ``Dataset`` loaders) read it back, whole or as N-range pieces."""
+        torch.save({"format": COMPACT_FORMAT, "version": COMPACT_VERSION, "ids": self.ids.contiguous().cpu(),
+                    "probs": self.probs.contiguous().cpu(), "C": self.C}, path)
 
     def numel(self):
         return self.ids.numel() * 2          # what it costs relative to a dense float count (for the auto-shard rule)
@@ -317,6 +569,54 @@ class CompactSlab:
         col = rest[:, None].expand(H, C).clone()
         col.scatter_(1, (self.ids[:, idx].to(torch.int64) & 0xFFFF), p)
         return col
+
+
+class ShardedCompactSlab:
+    """A compact slab held as contiguous N-range pieces, one ``CompactSlab`` per piece, each on its own device: the
+    compact twin of ``ShardedSlab``, with its surface and its rules.  The pieces ARE the shard layout: CODA and the
+    competing selectors run one shard per piece, in place, and give the bits of the whole ``CompactSlab`` with
+    ``shards=`` the piece count.  ``device`` is the first piece's."""
+
+    def __init__(self, pieces):
+        pieces = list(pieces)
+        if not pieces:
+            raise ValueError("ShardedCompactSlab: at least one piece expected")
+        for p in pieces:
+            if not isinstance(p, CompactSlab):
+                raise TypeError("ShardedCompactSlab: pieces must be CompactSlab (dense pieces make a ShardedSlab)")
+            if p.shape[1] < 1:
+                raise ValueError("ShardedCompactSlab: every piece must hold at least one item")
+        H, _, C = pieces[0].shape
+        K = pieces[0].K
+        if any(p.shape[0] != H or p.C != C or p.K != K for p in pieces):
+            raise TypeError("ShardedCompactSlab: all pieces must share H, C and K")
+        self.pieces = pieces
+        self.offsets = []
+        n = 0
+        for p in pieces:
+            self.offsets.append(n)
+            n += int(p.shape[1])
+        self.shape = (int(H), n, int(C))
+        self.C, self.K = int(C), int(K)
+        self.device = pieces[0].device
+        self.dtype = torch.float32
+        self.is_cuda = pieces[0].is_cuda
+        self.compaction = None
+
+    def layout(self):
+        """[(piece, n_offset)]: the shard layout selectors build from."""
+        return list(zip(self.pieces, self.offsets))
+
+    def numel(self):
+        return sum(p.numel() for p in self.pieces)
+
+    def item_column(self, idx) -> torch.Tensor:
+        """The dense (H, C) float32 scores of item ``idx`` (``CompactSlab.item_column``), on its piece's device."""
+        idx = int(idx)
+        if not 0 <= idx < self.shape[1]:
+            raise IndexError(f"ShardedCompactSlab: item {idx} outside [0, {self.shape[1]})")
+        r = max(i for i, off in enumerate(self.offsets) if off <= idx)
+        return self.pieces[r].item_column(idx - self.offsets[r])
 
 
 class CompactDataset:

@@ -106,11 +106,12 @@ def modelpicker_eps_search(dataset, epsilons=DEFAULT_EPSILONS, iterations=1000, 
     from .baselines import _DeviceState, _ptr
     from .dist import default_comm
     eps = _check_epsilons(epsilons)
-    from .datasets import ShardedSlab
+    from .datasets import ShardedCompactSlab, ShardedSlab
     preds = getattr(dataset, "preds", None)
-    if isinstance(preds, ShardedSlab):
-        raise NotImplementedError("modelpicker_eps_search: runs on one GPU over one (H, N, C) tensor; a ShardedSlab "
-                                  "(a slab loaded as N-range pieces) is not supported -- load the task unsharded")
+    if isinstance(preds, (ShardedSlab, ShardedCompactSlab)):
+        raise NotImplementedError(f"modelpicker_eps_search: runs on one GPU over one (H, N, C) tensor; a "
+                                  f"{type(preds).__name__} (a slab loaded as N-range pieces) is not supported -- load "
+                                  f"the task unsharded")
     if preds is None or len(preds.shape) != 3:
         raise TypeError("modelpicker_eps_search: dataset.preds must be an (H, N, C) slab")
     H, N, C = (int(s) for s in preds.shape)

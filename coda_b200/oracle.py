@@ -14,10 +14,10 @@ class Oracle:
         assert self.labels is not None, "Oracle needs labels!"
 
     def true_losses(self, preds):
-        """Mean loss of every model, (H,) (coda/oracle.py:9-21).  A ``ShardedSlab`` takes the accuracy loss only, on
-        the pieces' devices (``sharded_true_losses``)."""
-        from .datasets import ShardedSlab
-        if isinstance(preds, ShardedSlab):
+        """Mean loss of every model, (H,) (coda/oracle.py:9-21).  A ``ShardedSlab``, ``CompactSlab`` or
+        ``ShardedCompactSlab`` takes the accuracy loss only, on the pieces' devices (``sharded_true_losses``)."""
+        from .datasets import CompactSlab, ShardedCompactSlab, ShardedSlab
+        if isinstance(preds, (ShardedSlab, CompactSlab, ShardedCompactSlab)):
             return sharded_true_losses(preds, self.labels, self.loss_fn, self.dataset.device)
         H, N, C = preds.shape
         return self.loss_fn(preds.reshape(-1, C), self.labels.repeat(H), reduction="none").view(H, N).mean(dim=1)
@@ -36,39 +36,53 @@ def sharded_true_losses(slab, labels, loss_fn, device):
     """``Oracle.true_losses`` of a ``ShardedSlab`` with the accuracy loss: one ``coda_b200_true_loss_counts`` launch per
     piece, each on its device and a stream of its own, all in flight together.  The per-model wrong counts are exact
     integers below 2^24, so they equal torch's fp32 sums; the result carries the bits of ``true_losses`` on the same
-    slab held as one tensor, on ``device``."""
+    slab held as one tensor, on ``device``.
+
+    A ``CompactSlab`` (one piece) or ``ShardedCompactSlab`` counts the items whose ``ids[0]`` -- the hard prediction
+    every selector sees -- is the label (``coda_b200_true_loss_counts_compact``).  For a slab compacted from a dense one
+    (``CompactSlab.from_dense``, ``load_compact``) ``ids[0]`` is the dense arg-max, so the result has the bits of
+    ``true_losses`` on the dense slab.  It can differ from ``true_losses(slab.densify())`` only in the rows counted in
+    ``compaction["flat_rows"]``, where the uniform remainder reaches ``probs[0]``."""
     from . import _native as nat
+    from .datasets import CompactSlab
+    name = type(slab).__name__
     try:
         from coda.options import accuracy_loss                # what LOSS_FNS["acc"] resolves to
     except ImportError:
         accuracy_loss = None
     if accuracy_loss is None or loss_fn is not accuracy_loss:
-        raise NotImplementedError("Oracle.true_losses on a ShardedSlab takes the accuracy loss only "
+        raise NotImplementedError(f"Oracle.true_losses on a {name} takes the accuracy loss only "
                                   "(coda.options.accuracy_loss, LOSS_FNS['acc'])")
     if labels.dim() != 1:
-        raise NotImplementedError("Oracle.true_losses on a ShardedSlab takes 1-D class labels")
+        raise NotImplementedError(f"Oracle.true_losses on a {name} takes 1-D class labels")
     H, N, C = (int(s) for s in slab.shape)
     if N >= 1 << 24:
-        raise NotImplementedError(f"Oracle.true_losses on a ShardedSlab: N = {N} >= 2^24, where fp32 sums of the "
+        raise NotImplementedError(f"Oracle.true_losses on a {name}: N = {N} >= 2^24, where fp32 sums of the "
                                   f"per-item losses stop being exact counts")
     if not slab.is_cuda:
-        raise NotImplementedError("coda_b200: the pieces of a ShardedSlab must be CUDA tensors; there is no CPU path")
+        raise NotImplementedError(f"coda_b200: the pieces of a {name} must be CUDA tensors; there is no CPU path")
     lib = nat.load()
-    fmt = nat.slab_format(slab.dtype)
     labels = labels.to(torch.int64)
     parts = []
-    for piece, off in slab.layout():
+    for piece, off in (slab.layout() if hasattr(slab, "layout") else [(slab, 0)]):
         dev = piece.device
+        n = int(piece.shape[1])
         with torch.cuda.device(dev):
             st = torch.cuda.Stream(device=dev)
             st.wait_stream(torch.cuda.current_stream(dev))
             with torch.cuda.stream(st):
-                lab = labels[off:off + piece.shape[1]].to(dev, non_blocking=False)
+                lab = labels[off:off + n].to(dev, non_blocking=False)
                 cnt = torch.empty(H, dtype=torch.int64, device=dev)
-                nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(piece.data_ptr()), fmt, int(piece.stride(0)), H,
-                                                         int(piece.shape[1]), C, ct.c_void_p(lab.data_ptr()),
-                                                         ct.c_void_p(cnt.data_ptr()), ct.c_void_p(st.cuda_stream)),
-                          "true_loss_counts")
+                if isinstance(piece, CompactSlab):
+                    stride = int(piece.ids.stride(0)) if H > 1 else n * piece.K
+                    nat.check(lib.coda_b200_true_loss_counts_compact(
+                        ct.c_void_p(piece.ids.data_ptr()), stride, H, n, piece.K, ct.c_void_p(lab.data_ptr()),
+                        ct.c_void_p(cnt.data_ptr()), ct.c_void_p(st.cuda_stream)), "true_loss_counts_compact")
+                else:
+                    nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(piece.data_ptr()), nat.slab_format(slab.dtype),
+                                                             int(piece.stride(0)), H, n, C, ct.c_void_p(lab.data_ptr()),
+                                                             ct.c_void_p(cnt.data_ptr()), ct.c_void_p(st.cuda_stream)),
+                              "true_loss_counts")
                 lab.record_stream(st)
         parts.append((cnt, st))
     correct = torch.zeros(H, dtype=torch.int64, device=device)

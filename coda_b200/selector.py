@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from .base import ModelSelector
-from .datasets import ShardedSlab
+from .datasets import ShardedCompactSlab, ShardedSlab
 from .dist import InProcessGroup, ProcessGroup, SoloGroup, choose_among_ties, default_comm, piece_layout, split_slab
 from .engine import HIST_CAP, TIE_CAP, build_engines
 
@@ -122,7 +122,7 @@ class CODA(ModelSelector):
         n_global = int(getattr(dataset, "n_global", preds.shape[1]))
         kw = dict(alpha=alpha, learning_rate=learning_rate, multiplier=multiplier,
                   uniform_prior=bool(disable_diag_prior), mode=mode, n_global=n_global, prefilter_n=prefilter_n, q=q)
-        if isinstance(preds, ShardedSlab):                  # the pieces are the shards
+        if isinstance(preds, (ShardedSlab, ShardedCompactSlab)):    # the pieces are the shards
             layout = piece_layout(preds, gpus, shards, comm.world)
             self.group = SoloGroup() if len(layout) == 1 else InProcessGroup(len(layout))
         elif comm.world > 1:                                # one process per GPU: this is one shard of the task

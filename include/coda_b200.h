@@ -647,6 +647,24 @@ int coda_b200_preload_kernels(int64_t* loaded_host);
 int coda_b200_true_loss_counts(const void* preds, int fmt, int64_t model_stride, int H, int64_t N, int C,
                                const int64_t* labels, int64_t* counts, coda_stream_t stream);
 
+/* ---- building a compact slab from a dense one (csrc/compact_build.cu) -----------------------------------------------
+ * For every row (h, n) of the CODA_B200_SLAB_* slab `src` [H][N][C] (models `model_stride` elements apart, 2 <= C <=
+ * 4096): ids[h][n][0..K) the K highest-scoring classes in descending score order, equal scores by ascending class (so
+ * ids[h][n][0] is torch.argmax's first-index maximum), probs[h][n][0..K) their scores widened to fp32, bit for bit.
+ * K in {1, 2, 3, 4, 8}, K < C; ids and probs have models `out_stride` elements apart, items K apart.  ACCUMULATED into
+ * (the caller starts them at 0, i.e. +0.0 for dropped_max): dropped_max[h] = max over the rows of the (K+1)-th score
+ * (as the max of its int32 bits: exact for scores >= 0), flat_rows[h] += rows whose remainder (1 - sum_j probs) *
+ * fp32(1 / (C - K)) (coda_b200_scan_compact's arithmetic) is >= probs[0].  *flags gets CODA_B200_FLAG_NONFINITE_INPUT /
+ * CODA_B200_FLAG_RANGE_INPUT by the dense scan's rules. */
+int coda_b200_compact_build(const void* src, int fmt, int64_t model_stride, int H, int64_t N, int C, int K,
+                            uint16_t* ids, float* probs, int64_t out_stride, float* dropped_max, int64_t* flat_rows,
+                            uint32_t* flags, coda_stream_t stream);
+/* counts[h] = number of items n with ids[h][n][0] == labels[n] (ids [H][N][K], models model_stride elements apart;
+ * labels [N] int64); counts [H] int64 is zeroed on `stream` first.  For a slab built by coda_b200_compact_build these are
+ * coda_b200_true_loss_counts of the dense slab. */
+int coda_b200_true_loss_counts_compact(const uint16_t* ids, int64_t model_stride, int H, int64_t N, int K,
+                                       const int64_t* labels, int64_t* counts, coda_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

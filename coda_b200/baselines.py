@@ -40,7 +40,7 @@ import torch
 
 from . import _native as nat
 from .base import ModelSelector
-from .dist import InProcessGroup, ProcessGroup, SoloGroup, default_comm, piece_layout, split_slab
+from .dist import InProcessGroup, ProcessGroup, SoloGroup, default_comm, labels_per_device, piece_layout, split_slab
 from .selector import _Unlabeled
 
 _NO_CPU = ("coda_b200.baselines: dataset.preds must be a CUDA tensor on an sm_90a device; there is no CPU path in this "
@@ -655,16 +655,9 @@ class _Baseline(ModelSelector):
             raise ValueError(f"coda_b200.baselines: run_steps({k}) with {left} unlabeled items left")
 
     def _loop_bind_labels(self, labels):
-        cache = self._loop_labels
-        if cache is None or cache[0] is not labels:
-            per_dev = {}
-            for st in self.states:
-                if st.dev not in per_dev:
-                    per_dev[st.dev] = labels.to(st.dev, torch.int64).contiguous()
-            for d in per_dev:
-                torch.cuda.synchronize(d)
-            self._loop_labels = cache = (labels, per_dev)
-        return cache[1]
+        if self._loop_labels is None or self._loop_labels[0] is not labels:
+            self._loop_labels = (labels, labels_per_device(labels, [st.dev for st in self.states]))
+        return self._loop_labels[1]
 
     def _loop_upload(self, seed):
         """Write the host-side state (labels so far, the method's sums) into every shard's loop buffers."""

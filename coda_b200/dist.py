@@ -195,6 +195,18 @@ def split_slab(preds, nshards, ngpus):
     return out
 
 
+def labels_per_device(labels, devices):
+    """{device: ``labels`` as a contiguous int64 tensor there} for the host-free loops, one copy per distinct device.
+    Each device is synchronised once: the copies ran on the current streams, the shards read them on their own."""
+    per_dev = {}
+    for d in devices:
+        if d not in per_dev:
+            per_dev[d] = labels.to(d, torch.int64).contiguous()
+    for d in per_dev:
+        torch.cuda.synchronize(d)
+    return per_dev
+
+
 class SoloGroup:
     """world == 1: no exchange."""
     world = 1

@@ -11,7 +11,7 @@ Modes (what is kept between steps; results are the same):
   ``recompute_all`` additionally rebuilds all class tables and re-runs the full slab pass of
                     ``update_pi_hat`` every step -- the reference's literal per-step work.
 
-One acquisition step on the device (host-free loop, ``run_steps``; everything below is ONE CUDA graph):
+One acquisition step on the device (host-free loop, ``CODA.run_steps``; everything below is ONE CUDA graph):
 
     step_select   merge block records, exchange with the peers, arg-max, label lookup, D[h][t][p_h] += lr, gather list
     ---- fork ----  side stream: beta_tables(class t) -> pair_rows(class t)        main: pi_rank1 (marginal refresh)
@@ -162,6 +162,7 @@ class Engine:
         self.side = torch.cuda.Stream(device=self.dev)
         self.ev_fork, self.ev_join, self.ev_tables = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
         self.graphs = {}
+        self.loop_launches = {}                               # graph key -> launches of one replay
         self.labels_ptr = None
         # a private slot of the device's constant-memory term table (several selectors / shards may share a device)
         self.const_slot = _acquire_const_slot(self.dev.index, H) if os.environ.get("CODA_B200_R1_CONST", "1") != "0" else -1
@@ -745,16 +746,10 @@ class Engine:
     def pf_fallback_commit(self, rule, record_best):
         """The EIG loop's selection over those records (its tie rule), the label and the posterior update."""
         with self._on():
-            s, x = self._s(), self._x()
-            if rule == "reference":
-                self._call("coda_b200_step_select_defer", self.st, x, _ptr(self.ref_lw[3:]), s)
-                self._ref_tie(self.eig)
-            else:
-                self._call("coda_b200_step_select", self.st, x, s)
+            self._select(self.eig, rule)
             self._post_label()
             if record_best:
-                self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
-                           HIST_CAP, s)
+                self._record_best()
 
     def _post_label(self):
         """coda.py:317-319 after ``sel`` / ``jvec`` / D / the gather list are in place (step_select or step_label):
@@ -808,6 +803,18 @@ class Engine:
         self._mixture()
 
     # ------------------------------------------------------------------------ host-free loop
+    # One step body for every acquisition of CODA.run_steps, captured as one CUDA graph per (kind, record_best, rule):
+    #   "eig"           step_select over the scoring pass's block records -> refresh + mixture -> the scoring pass for
+    #                   the next step
+    #   "uncertainty"   block records from the static scores -> step_select -> refresh + mixture (no scoring pass)
+    #   "iid"           candidate ties -> k-th of them (pre-drawn k) -> commit -> step_label -> refresh + mixture
+    #   "prefilter"     candidate ties -> sampled positions resolved and reduced -> commit -> step_label -> refresh +
+    #                   mixture, then the scoring pass for the next step (with sample scoring a step scores its sample)
+    #   "prefilter_id"  the prefilter with the identity sample (sample scoring, steps with at most prefilter_n candidates)
+    # rule "reference" breaks isclose ties from the replica of Python's generator (ref_bind); record_best appends
+    # best_model -> hist_best.  The pre-draws of iid / prefilter (one row of `width` int64 per step,
+    # include/coda_b200.h) are replayed from a device buffer of `rows` rows that the caller refills chunk by chunk
+    # (abl_load).
     def _bind_labels(self, labels_dev):
         if labels_dev.data_ptr() != self.labels_ptr:
             if labels_dev.dtype != torch.int64 or labels_dev.device != self.dev or labels_dev.numel() < self.n_global:
@@ -815,33 +822,43 @@ class Engine:
             self.st.labels_global = labels_dev.data_ptr()
             self.labels_ptr = labels_dev.data_ptr()
             self._labels_keep = labels_dev
-            for key in ("loop", "loop_best", "loop_ref", "loop_ref_best"):
-                self.graphs.pop(key, None)
-            for key in [k for k in self.graphs if isinstance(k, tuple) and k[0] == "abl"]:
+            for key in [k for k in self.graphs if isinstance(k, tuple) and k[0] == "loop"]:
                 del self.graphs[key]
 
-    def _loop_body(self):
-        """select -> posterior update -> scoring pass for the next selection (one graph)."""
-        self._call("coda_b200_step_select", self.st, self._x(), self._s())
+    def _loop_body(self, kind="eig", record_best=False, rule="first"):
+        """One step: the kind's selection, the posterior update, the scoring pass for the next selection (see
+        ``_loop_scores``), and with ``record_best`` the step's best model."""
+        if kind == "eig":
+            self._select(self.eig, rule)
+        elif kind == "uncertainty":
+            self._call("coda_b200_static_records", _ptr(self.abl_score), _ptr(self.labeled), _ptr(self.disagree), self.N,
+                       self.n_offset, self.nblocks, _ptr(self.partials), self._s())
+            self._select(self.abl_score, rule)
+        else:
+            self._select_drawn(kind, rule)
         self._post_label()
-        self._score()
+        if self._loop_scores(kind):
+            self._score()
+        if record_best:
+            self._record_best()
 
-    def _loop_body_best(self):
-        """The loop body, then best_model (written by step_mixture on this stream) -> hist_best[step_ctr - 1]."""
-        self._loop_body()
+    def _loop_scores(self, kind):
+        """Whether the loop body of ``kind`` ends with the full scoring pass (the next step selects from it)."""
+        return kind == "eig" or (kind == "prefilter" and not self.sample_scoring)
+
+    def _select(self, v, rule):
+        """step_select over the block records; tie_rule="reference": the deferring select, and a step it leaves
+        pending draws its pick over score ``v`` from the Python generator's replica (_ref_tie)."""
+        if rule == "reference":
+            self._call("coda_b200_step_select_defer", self.st, self._x(), _ptr(self.ref_lw[3:]), self._s())
+            self._ref_tie(v)
+        else:
+            self._call("coda_b200_step_select", self.st, self._x(), self._s())
+
+    def _record_best(self):
+        """best_model (written by step_mixture on this stream) -> hist_best[step_ctr - 1]."""
         self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
                    HIST_CAP, self._s())
-
-    def _loop_body_ref(self, record_best):
-        """tie_rule="reference": the deferring select; a step it leaves pending draws its pick from the Python
-        generator's replica (_ref_tie); then the rest of the loop body."""
-        self._call("coda_b200_step_select_defer", self.st, self._x(), _ptr(self.ref_lw[3:]), self._s())
-        self._ref_tie(self.eig)
-        self._post_label()
-        self._score()
-        if record_best:
-            self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
-                       HIST_CAP, self._s())
 
     def _ref_tie(self, v):
         """A pending step's band of isclose candidates over score ``v`` -> _randbelow draw -> commit -> label."""
@@ -852,16 +869,60 @@ class Engine:
                    _ptr(self.pyrng), _ptr(self.ref_lw), x, s)
         self._call("coda_b200_step_label_if", self.st, x, pend, s)
 
-    def _loop_key(self, record_best, rule="first"):
-        if rule == "reference":
-            return ("loop_ref_best" if record_best else "loop_ref"), (lambda: self._loop_body_ref(record_best))
-        return ("loop_best", self._loop_body_best) if record_best else ("loop", self._loop_body)
+    def _select_drawn(self, kind, rule):
+        """iid / prefilter / prefilter_id: the candidates, the pick from this step's pre-draw row, the label.
+        tie_rule="reference" (prefilter): the row is drawn on the device and ties from the same generator; iid's
+        pre-drawn rows already are the reference's draws."""
+        s, x, pre, w = self._s(), self._x(), self.abl_pre, self.abl_width
+        ref = rule == "reference" and kind != "iid"
+        lw = self.ref_lw if ref else self.abl_lw
+        self._call("coda_b200_select_extreme_xchg", _ptr(self.abl_cand), _ptr(self.labeled), self.N, 1,
+                   _ptr(self.abl_xp), _ptr(self.abl_best), x, _ptr(self.flags), s, n=2)
+        if kind == "iid":
+            self._call("coda_b200_abl_draw", _ptr(pre), w, _ptr(lw), s)
+            self._call("coda_b200_select_kth_xchg_dev", _ptr(self.abl_cand), _ptr(self.labeled), self.N,
+                       _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(lw[1:]), _ptr(lw[2:]), self.n_offset,
+                       _ptr(self.abl_pick), x, _ptr(self.flags), s)
+            self._call("coda_b200_abl_commit", self.st, _ptr(self.abl_best), _ptr(self.abl_pick), _ptr(pre), w,
+                       _ptr(lw), s)
+        else:
+            if kind == "prefilter_id":
+                self._call("coda_b200_pf_identity", _ptr(self.abl_best), _ptr(pre), w - 1, _ptr(lw), _ptr(self.flags), s)
+            elif ref:
+                self._call("coda_b200_pf_sample", _ptr(self.abl_best), _ptr(pre), w - 1, self.ref_setsize,
+                           _ptr(self.pyrng), _ptr(self.ref_pool), _ptr(self.ref_seen), _ptr(lw), _ptr(self.flags), s)
+            self._pf_score_sample(pre, w, lw)
+            self._call("coda_b200_prefilter_pick", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
+                       self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw),
+                       _ptr(self.abl_recs), s)
+            if ref:
+                pend = _ptr(lw[3:])
+                self._call("coda_b200_prefilter_commit_defer", self.st, _ptr(self.abl_recs), self.abl_nrec,
+                           _ptr(self.abl_best), _ptr(pre), w, _ptr(lw), pend, x, s)
+                self._call("coda_b200_pf_band", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
+                           self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw), pend,
+                           _ptr(self.ref_band), s)
+                self._call("coda_b200_pf_tie_draw", self.st, _ptr(self.ref_band), w - 1, pend, _ptr(self.pyrng),
+                           _ptr(self.ref_bits), _ptr(lw), x, s)
+            else:
+                self._call("coda_b200_prefilter_commit", self.st, _ptr(self.abl_recs), self.abl_nrec,
+                           _ptr(self.abl_best), _ptr(pre), w, _ptr(lw), x, s)
+        self._call("coda_b200_step_label", self.st, x, s)
+
+    def _pf_score_sample(self, pre, w, lw):
+        """With sample scoring: this step's sample positions -> local items (as prefilter_pick resolves them) -> their
+        eig, which prefilter_pick then reads."""
+        if self.sample_scoring:
+            self._call("coda_b200_pf_resolve", _ptr(self.abl_cand), _ptr(self.labeled), self.N, _ptr(self.abl_xp),
+                       _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw), _ptr(self.sw["items"]), self._s())
+            self._score_sample()
 
     def device_step(self, labels_dev: torch.Tensor, step: int | None = None, hist_idx=None, hist_q=None):
         """One acquisition step with no host round trip: pick the arg-max (first index on equal values, coda.py:309;
         an isclose tie that the reference would break with random.choice is recorded in ``hist_tie``), look the label
-        up on the device (coda/oracle.py:23-24), update the posterior, score the next selection.  Eager launches; see
-        ``run_steps`` for the CUDA-graph loop.  ``hist_idx`` / ``hist_q``: optional caller-owned history (slot = step)."""
+        up on the device (coda/oracle.py:23-24), update the posterior, score the next selection.  Eager launches of the
+        "eig" loop body; see the phases below for the CUDA-graph loop.  ``hist_idx`` / ``hist_q``: optional
+        caller-owned history (slot = step)."""
         with self._on():
             self._bind_labels(labels_dev)
             if step is not None:
@@ -875,21 +936,21 @@ class Engine:
 
     # The graph loop in phases, so that a front end driving several shards from one thread never blocks on a shard
     # whose peers have not been enqueued yet: prepare (no exchange inside) -> one eager step -> capture -> replays.
-    # record_best: a separately captured graph that also records the best model of every step (hist_best); the
-    # default graph is the plain loop body.
-    def loop_prepare(self, labels_dev: torch.Tensor, record_best: bool = False):
+    # The defaults are the EIG loop with the first maximum of a tie and no best-model record.
+    def loop_prepare(self, labels_dev: torch.Tensor, record_best: bool = False, kind: str = "eig"):
         with self._on():
             self._bind_labels(labels_dev)
             if record_best and getattr(self, "hist_best", None) is None:
                 self.hist_best = torch.full((HIST_CAP,), -1, dtype=torch.int32, device=self.dev)
-            self._score()
+            if self._loop_scores(kind):
+                self._score()
 
-    def loop_ready(self, record_best: bool = False, rule: str = "first") -> bool:
-        return (not self.use_graph) or self.graphs.get(self._loop_key(record_best, rule)[0]) is not None
+    def loop_ready(self, record_best: bool = False, rule: str = "first", kind: str = "eig") -> bool:
+        return (not self.use_graph) or self.graphs.get(("loop", kind, bool(record_best), rule)) is not None
 
-    def loop_eager(self, record_best: bool = False, rule: str = "first"):
+    def loop_eager(self, record_best: bool = False, rule: str = "first", kind: str = "eig"):
         with self._on():
-            self._loop_key(record_best, rule)[1]()
+            self._loop_body(kind, record_best, rule)
 
     def _try_capture(self, key, body):
         """Capture `body` as graph `key`; a failed capture (driver / allocator state) falls back to eager launches."""
@@ -905,54 +966,24 @@ class Engine:
         self.graphs[key] = g
         return g, n
 
-    def loop_capture(self, record_best: bool = False, rule: str = "first"):
-        key, body = self._loop_key(record_best, rule)
+    def loop_capture(self, record_best: bool = False, rule: str = "first", kind: str = "eig"):
+        key = ("loop", kind, bool(record_best), rule)
         with self._on():
-            _g, n = self._try_capture(key, body)
-            if rule != "first":
-                self.ref_launches = getattr(self, "ref_launches", {})
-                self.ref_launches[key] = n
-            elif record_best:
-                self.launches_per_step_best = n
-            else:
-                self.launches_per_step = n
+            _g, self.loop_launches[key] = self._try_capture(key, lambda: self._loop_body(kind, record_best, rule))
 
-    def loop_replay(self, k: int = 1, record_best: bool = False, rule: str = "first"):
-        key, body = self._loop_key(record_best, rule)
+    def loop_replay(self, k: int = 1, record_best: bool = False, rule: str = "first", kind: str = "eig"):
+        key = ("loop", kind, bool(record_best), rule)
         with self._on():
             g = self.graphs.get(key)
             for _ in range(k):
                 if g is None:
-                    body()
+                    self._loop_body(kind, record_best, rule)
                 else:
                     g.replay()
             if g is not None:
-                if rule != "first":
-                    self.counters["launches"] += k * self.ref_launches[key]
-                else:
-                    self.counters["launches"] += k * (self.launches_per_step_best if record_best else self.launches_per_step)
+                self.counters["launches"] += k * self.loop_launches[key]
 
-    def run_steps(self, k: int, labels_dev: torch.Tensor, record_best: bool = False):
-        """``k`` acquisition steps as ``k`` replays of one captured CUDA graph (SURVEY.md 8f rank 2; replaces the
-        host loop of main.py:89-94 for offline runs).  History: ``hist_idx/hist_q/hist_tie[step_ctr % HIST_CAP]``,
-        with ``record_best`` also ``hist_best``."""
-        if k <= 0:
-            return
-        self.loop_prepare(labels_dev, record_best)
-        if not self.loop_ready(record_best):
-            self.loop_eager(record_best)                        # warm-up (module loading, attributes) outside capture
-            k -= 1
-            self.loop_capture(record_best)
-        self.loop_replay(k, record_best)
-
-    # ---- the loop of CODA's other acquisitions (CODA.run_steps with q='uncertainty' / 'iid' or prefilter_n) ----------
-    # kind "uncertainty": block records from the static scores -> step_select (no scoring pass);
-    # kind "iid":         candidate ties -> k-th of them (pre-drawn k) -> commit -> step_label (no scoring pass);
-    # kind "prefilter":   candidate ties -> sampled positions resolved and reduced -> commit -> step_label, then the
-    #                     scoring pass for the next step.  Steps the reference takes the plain arg-max for run the
-    #                     "loop" graph above.
-    # The pre-draws of iid / prefilter (one row of `width` int64 per step, include/coda_b200.h) are replayed from a
-    # device buffer of `rows` rows that the caller refills chunk by chunk (abl_load).
+    # Buffers of the kinds other than "eig": the static scores (uncertainty), the candidates and the pre-draw rows.
     def abl_bind(self, kind, score=None, width=0, rows=0):
         with self._on():
             if kind == "uncertainty":
@@ -972,7 +1003,8 @@ class Engine:
                 if kind == "prefilter":
                     self.abl_nrec = int(self.lib.coda_b200_prefilter_blocks(width - 1))
                     self.abl_recs = self._z((4 * self.abl_nrec,), torch.int64)
-                for key in [k for k in self.graphs if isinstance(k, tuple) and k[0] == "abl" and k[1] != "uncertainty"]:
+                drawn = ("iid", "prefilter", "prefilter_id")             # the graphs that read the old buffer
+                for key in [k for k in self.graphs if isinstance(k, tuple) and k[1] in drawn]:
                     del self.graphs[key]
 
     def abl_load(self, pre_host):
@@ -980,113 +1012,6 @@ class Engine:
         with self._on():
             self.abl_pre[: pre_host.numel()].copy_(pre_host, non_blocking=True)
             self.abl_lw[0:1].zero_()
-
-    def _abl_body(self, kind, record_best, rule="first"):
-        s, x = self._s(), self._x()
-        if kind == "uncertainty":
-            self._call("coda_b200_static_records", _ptr(self.abl_score), _ptr(self.labeled), _ptr(self.disagree), self.N,
-                       self.n_offset, self.nblocks, _ptr(self.partials), s)
-            if rule == "reference":
-                self._call("coda_b200_step_select_defer", self.st, x, _ptr(self.ref_lw[3:]), s)
-                self._ref_tie(self.abl_score)
-            else:
-                self._call("coda_b200_step_select", self.st, x, s)
-        elif rule == "reference":         # prefilter: the sample drawn on the device, ties from the same generator
-            lw, pre, w, pend = self.ref_lw, self.abl_pre, self.abl_width, _ptr(self.ref_lw[3:])
-            self._call("coda_b200_select_extreme_xchg", _ptr(self.abl_cand), _ptr(self.labeled), self.N, 1,
-                       _ptr(self.abl_xp), _ptr(self.abl_best), x, _ptr(self.flags), s, n=2)
-            if kind == "prefilter_id":
-                self._call("coda_b200_pf_identity", _ptr(self.abl_best), _ptr(pre), w - 1, _ptr(lw), _ptr(self.flags), s)
-            else:
-                self._call("coda_b200_pf_sample", _ptr(self.abl_best), _ptr(pre), w - 1, self.ref_setsize,
-                           _ptr(self.pyrng), _ptr(self.ref_pool), _ptr(self.ref_seen), _ptr(lw), _ptr(self.flags), s)
-            self._pf_score_sample(pre, w, lw)
-            self._call("coda_b200_prefilter_pick", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
-                       self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw),
-                       _ptr(self.abl_recs), s)
-            self._call("coda_b200_prefilter_commit_defer", self.st, _ptr(self.abl_recs), self.abl_nrec,
-                       _ptr(self.abl_best), _ptr(pre), w, _ptr(lw), pend, x, s)
-            self._call("coda_b200_pf_band", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
-                       self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw), pend,
-                       _ptr(self.ref_band), s)
-            self._call("coda_b200_pf_tie_draw", self.st, _ptr(self.ref_band), w - 1, pend, _ptr(self.pyrng),
-                       _ptr(self.ref_bits), _ptr(lw), x, s)
-            self._call("coda_b200_step_label", self.st, x, s)
-        else:
-            lw, pre, w = self.abl_lw, self.abl_pre, self.abl_width
-            self._call("coda_b200_select_extreme_xchg", _ptr(self.abl_cand), _ptr(self.labeled), self.N, 1,
-                       _ptr(self.abl_xp), _ptr(self.abl_best), x, _ptr(self.flags), s, n=2)
-            if kind == "iid":
-                self._call("coda_b200_abl_draw", _ptr(pre), w, _ptr(lw), s)
-                self._call("coda_b200_select_kth_xchg_dev", _ptr(self.abl_cand), _ptr(self.labeled), self.N,
-                           _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(lw[1:]), _ptr(lw[2:]), self.n_offset,
-                           _ptr(self.abl_pick), x, _ptr(self.flags), s)
-                self._call("coda_b200_abl_commit", self.st, _ptr(self.abl_best), _ptr(self.abl_pick), _ptr(pre), w,
-                           _ptr(lw), s)
-            else:
-                if kind == "prefilter_id":
-                    self._call("coda_b200_pf_identity", _ptr(self.abl_best), _ptr(pre), w - 1, _ptr(lw),
-                               _ptr(self.flags), s)
-                self._pf_score_sample(pre, w, lw)
-                self._call("coda_b200_prefilter_pick", _ptr(self.eig), _ptr(self.abl_cand), _ptr(self.labeled), self.N,
-                           self.n_offset, _ptr(self.abl_xp), _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw),
-                           _ptr(self.abl_recs), s)
-                self._call("coda_b200_prefilter_commit", self.st, _ptr(self.abl_recs), self.abl_nrec,
-                           _ptr(self.abl_best), _ptr(pre), w, _ptr(lw), x, s)
-            self._call("coda_b200_step_label", self.st, x, s)
-        self._post_label()
-        if kind == "prefilter" and not self.sample_scoring:
-            self._score()
-        if record_best:
-            self._call("coda_b200_record_best", _ptr(self.best_model), _ptr(self.step_ctr), _ptr(self.hist_best),
-                       HIST_CAP, s)
-
-    def _pf_score_sample(self, pre, w, lw):
-        """With sample scoring: this step's sample positions -> local items (as prefilter_pick resolves them) -> their
-        eig, which prefilter_pick then reads."""
-        if self.sample_scoring:
-            self._call("coda_b200_pf_resolve", _ptr(self.abl_cand), _ptr(self.labeled), self.N, _ptr(self.abl_xp),
-                       _ptr(self.abl_best), _ptr(pre), w, w - 1, _ptr(lw), _ptr(self.sw["items"]), self._s())
-            self._score_sample()
-
-    # the same phases as loop_prepare / loop_ready / loop_eager / loop_capture / loop_replay
-    def abl_prepare(self, labels_dev, kind, record_best=False):
-        with self._on():
-            self._bind_labels(labels_dev)
-            if record_best and getattr(self, "hist_best", None) is None:
-                self.hist_best = torch.full((HIST_CAP,), -1, dtype=torch.int32, device=self.dev)
-            if kind == "prefilter" and not self.sample_scoring:
-                self._score()
-
-    @staticmethod
-    def _abl_key(kind, record_best, rule):
-        return ("abl", kind, bool(record_best)) + (() if rule == "first" else (rule,))
-
-    def abl_ready(self, kind, record_best=False, rule="first") -> bool:
-        return (not self.use_graph) or self.graphs.get(self._abl_key(kind, record_best, rule)) is not None
-
-    def abl_eager(self, kind, record_best=False, rule="first"):
-        with self._on():
-            self._abl_body(kind, record_best, rule)
-
-    def abl_capture(self, kind, record_best=False, rule="first"):
-        key = self._abl_key(kind, record_best, rule)
-        with self._on():
-            _g, n = self._try_capture(key, lambda: self._abl_body(kind, record_best, rule))
-            self.abl_launches = getattr(self, "abl_launches", {})
-            self.abl_launches[key] = n
-
-    def abl_replay(self, kind, k=1, record_best=False, rule="first"):
-        key = self._abl_key(kind, record_best, rule)
-        with self._on():
-            g = self.graphs.get(key)
-            for _ in range(k):
-                if g is None:
-                    self._abl_body(kind, record_best, rule)
-                else:
-                    g.replay()
-            if g is not None:
-                self.counters["launches"] += k * self.abl_launches[key]
 
     # ---- tie_rule="reference": a replica of Python's generator on this shard (csrc/pyrandom.cuh) --------------------
     # pyrng [625] int32 (the uint32 words of random.getstate()[1]); ref_lw [8] int64 loop words of the reference-mode

@@ -23,7 +23,8 @@ import torch
 
 from .base import ModelSelector
 from .datasets import ShardedCompactSlab, ShardedSlab
-from .dist import InProcessGroup, ProcessGroup, SoloGroup, choose_among_ties, default_comm, piece_layout, split_slab
+from .dist import (InProcessGroup, ProcessGroup, SoloGroup, choose_among_ties, default_comm, labels_per_device,
+                   piece_layout, split_slab)
 from .engine import HIST_CAP, TIE_CAP, build_engines
 
 
@@ -421,25 +422,17 @@ class CODA(ModelSelector):
         rule = "reference" if tie_rule == "reference" and self.q != "iid" else "first"
         if rule == "reference":
             self._reference_refusals()
-        cache = getattr(self, "_labels_dev", None)
-        if cache is None or cache[0] is not labels:
-            per_dev = {}
-            for e in self.engines:
-                if e.dev not in per_dev:
-                    per_dev[e.dev] = labels.to(e.dev, torch.int64).contiguous()
-            for d in per_dev:
-                torch.cuda.synchronize(d)
-            self._labels_dev = cache = (labels, per_dev)
-        per_dev = cache[1]
+        if self._labels_dev is None or self._labels_dev[0] is not labels:
+            self._labels_dev = (labels, labels_per_device(labels, [e.dev for e in self.engines]))
+        per_dev = self._labels_dev[1]
         if k <= 0:
             return
         if rule == "reference":
             self._run_reference(k, per_dev, record_best)
-            return
-        if self.q != "eig" or self.prefilter_n:
+        elif self.q != "eig" or self.prefilter_n:
             self._run_ablation(k, per_dev, record_best)
-            return
-        self._run_eig(k, per_dev, record_best)
+        else:
+            self._steps("eig", k, per_dev, record_best)
 
     def _run_reference(self, k, per_dev, record_best):
         """run_steps(tie_rule="reference"): Python's state goes to every shard's replica before the steps and comes
@@ -452,7 +445,7 @@ class CODA(ModelSelector):
             e.ref_bind()
             e.rng_upload(words)
         if self.q == "eig" and not self.prefilter_n:
-            self._run_eig(k, per_dev, record_best, "reference")
+            self._steps("eig", k, per_dev, record_best, "reference")
         else:
             self._run_ablation(k, per_dev, record_best, "reference")
         states = [e.rng_download() for e in self.engines]
@@ -464,23 +457,25 @@ class CODA(ModelSelector):
             if bool(e0.hist_tie[slots].any()):
                 self.stochastic = True                      # coda.py:311
 
-    def _run_eig(self, k, per_dev, record_best, rule="first"):
+    def _steps(self, kind, k, per_dev, record_best, rule="first"):
+        """``k`` steps of the loop body ``kind`` (engine.py, "host-free loop") on every shard.  Phases in lock-step over
+        the shards, so that nobody waits on the host for a peer that has not been enqueued: prepare, then -- when a
+        graph is missing -- one eager step (module loading outside the capture) and the capture, then replays."""
         self._loop_dirty = True
-        # phases in lock-step over the shards: nobody waits on the host for a peer that has not been enqueued
         for e in self.engines:
-            e.loop_prepare(per_dev[e.dev], record_best)
-        if not all(e.loop_ready(record_best, rule) for e in self.engines):
+            e.loop_prepare(per_dev[e.dev], record_best, kind)
+        if not all(e.loop_ready(record_best, rule, kind) for e in self.engines):
             for e in self.engines:
-                e.loop_eager(record_best, rule)
+                e.loop_eager(record_best, rule, kind)
             k -= 1
             for e in self.engines:
-                e.loop_capture(record_best, rule)
+                e.loop_capture(record_best, rule, kind)
         for _ in range(k):
             for e in self.engines:
-                e.loop_replay(1, record_best, rule)
+                e.loop_replay(1, record_best, rule, kind)
 
     def _run_ablation(self, k, per_dev, record_best, rule="first"):
-        """run_steps for q='uncertainty' / 'iid' / prefilter_n (engine.py, "the loop of CODA's other acquisitions")."""
+        """run_steps for q='uncertainty' / 'iid' / prefilter_n (the loop kinds of engine.py's host-free loop)."""
         d0 = u0 = 0
         for e in self.engines:                              # the candidate counts once; every step removes a candidate
             d, u = e.candidate_counts()
@@ -495,8 +490,7 @@ class CODA(ModelSelector):
             base = self.engines[0].n_offset
             for e in self.engines:
                 e.abl_bind(kind, score=self._ens_entropy[e.n_offset - base: e.n_offset - base + e.N])
-            self._loop_dirty = True
-            self._abl_steps(kind, k, per_dev, record_best, rule)
+            self._steps(kind, k, per_dev, record_best, rule)
             return
         m = int(self.prefilter_n)
         counts = candidate_counts(d0, u0, k)
@@ -509,26 +503,24 @@ class CODA(ModelSelector):
             for e in self.engines:
                 e.abl_bind(kind, width=width, rows=1)
                 e.ref_bind_prefilter(m, sample_setsize(m))
-            self._loop_dirty = True
-            self._abl_steps(kind, drawn, per_dev, record_best, rule)
+            self._steps(kind, drawn, per_dev, record_best, rule)
             self.stochastic = True                          # coda.py:223
         elif drawn:
             for e in self.engines:
                 e.abl_bind(kind, width=width, rows=rows)
-            self._loop_dirty = True
             for s0 in range(0, drawn, rows):
                 c = min(rows, drawn - s0)
                 pre = torch.tensor([ablation_draw(kind, counts[s0 + i], m) for i in range(c)], dtype=torch.int64)
                 pre = pre.reshape(-1).pin_memory()
                 for e in self.engines:
                     e.abl_load(pre)
-                self._abl_steps(kind, c, per_dev, record_best)
+                self._steps(kind, c, per_dev, record_best)
             if kind == "prefilter" or any(n > 1 for n in counts):
                 self.stochastic = True                      # coda.py:223 / 311
         if k > drawn and kind == "prefilter" and self.engine.sample_scoring:
             self._run_unsampled(counts, drawn, k, m, per_dev, record_best, rule)
         elif k > drawn:
-            self._run_eig(k - drawn, per_dev, record_best, rule)
+            self._steps("eig", k - drawn, per_dev, record_best, rule)
 
     def _run_unsampled(self, counts, s, k, m, per_dev, record_best, rule):
         """Sample scoring, the prefilter steps without a sample (n_s <= prefilter_n, or the all-unlabeled fallback):
@@ -548,28 +540,15 @@ class CODA(ModelSelector):
                 t += 1
             if big:
                 for e in self.engines:
-                    e.abl_prepare(per_dev[e.dev], "prefilter_id", record_best)   # labels and hist_best
+                    e.loop_prepare(per_dev[e.dev], record_best, "prefilter_id")   # labels and hist_best
                 for _ in range(t - s):
                     for e in self.engines:
                         e.pf_fallback_score()
                     for e in self.engines:
                         e.pf_fallback_commit(rule, record_best)
             else:
-                self._abl_steps("prefilter_id", t - s, per_dev, record_best, rule)
+                self._steps("prefilter_id", t - s, per_dev, record_best, rule)
             s = t
-
-    def _abl_steps(self, kind, k, per_dev, record_best, rule="first"):
-        for e in self.engines:
-            e.abl_prepare(per_dev[e.dev], kind, record_best)
-        if not all(e.abl_ready(kind, record_best, rule) for e in self.engines):
-            for e in self.engines:
-                e.abl_eager(kind, record_best, rule)
-            k -= 1
-            for e in self.engines:
-                e.abl_capture(kind, record_best, rule)
-        for _ in range(k):
-            for e in self.engines:
-                e.abl_replay(kind, 1, record_best, rule)
 
     def history(self):
         """(idx, q, tie) arrays of the device-loop steps so far (the last HIST_CAP of them); also mirrors them into the

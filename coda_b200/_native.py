@@ -105,6 +105,7 @@ SIGNATURES = {
     "coda_b200_confusion_sorted": (i32, [p, i64, p, p, i32, i64, i32, i32, p, p]),
     "coda_b200_init_dirichlets": (i32, [p, p, i32, i32, i32, f64, f64, i32, p, p]),
     "coda_b200_scan_compact": (i32, [p, p, i64, i32, i64, i32, i32, p, p, p, p, p, p]),
+    "coda_b200_scan_compact_kernel": (i32, [p, p, i64, i32, i64, i32, i32, p, p, p, p, p, i32, p]),
     "coda_b200_confusion_compact": (i32, [p, p, i64, p, i32, i64, i32, i32, i32, p, p, p]),
     "coda_b200_pi_full_compact": (i32, [p, p, i64, p, i32, i64, i32, i32, p, p, p, p]),
     "coda_b200_pi_rank1_compact": (i32, [p, p, i64, p, i32, i64, i32, i32, p, f64, i32, p, p, p, p, p]),

@@ -115,16 +115,135 @@ __global__ void __launch_bounds__(256) k_scan_compact(const uint16_t* __restrict
   if (bad) atomicOr(flags, bad);
 }
 
-extern "C" int coda_b200_scan_compact(const uint16_t* ids, const float* probs, int64_t model_stride, int H, int64_t N,
-                                      int C, int K, uint16_t* hard, int32_t* pseudo, uint8_t* disagree, float* ens_out,
-                                      uint32_t* flags, coda_stream_t stream) {
+// ---------------------------------------------------------------------------------------
+// scan_compact for large C: one warp per item, the item's [C] row in shared memory (one row per warp).  Lane l loads
+// the entry of model h0 + l and stages its K (id, p - rest) pairs; the warp then applies models h0, h0 + 1, ... in
+// ascending order, lane j < K making the model's j-th add (a model's K ids are distinct: the adds of one model never
+// meet).  Every row[c] receives its adds in ascending h with k_scan_compact's arithmetic, and rsum is the same
+// ascending fp32 sum, so hard / pseudo / disagree / ens have k_scan_compact's bits.
+// ---------------------------------------------------------------------------------------
+#define SCW_WARPS 8
+
+template <int K>
+__global__ void __launch_bounds__(SCW_WARPS * 32) k_scan_compact_warp(const uint16_t* __restrict__ ids,
+                                                                     const float* __restrict__ probs, int H, long long N,
+                                                                     int C, long long model_stride_e,
+                                                                     uint16_t* __restrict__ hard, int32_t* __restrict__ pseudo,
+                                                                     uint8_t* __restrict__ disagree,
+                                                                     float* __restrict__ ens_out,
+                                                                     uint32_t* __restrict__ flags) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* row = reinterpret_cast<float*>(smem_raw) + (size_t)warp * C;                                   // [SCW_WARPS][C]
+  int2* stg = reinterpret_cast<int2*>(smem_raw + (size_t)SCW_WARPS * C * 4) + (size_t)warp * 32 * K;   // [32][K] per warp
+  const long long n = (long long)blockIdx.x * SCW_WARPS + warp;
+  if (n >= N) return;                                           // whole warps only: no block-wide barrier below
+  for (int c = lane; c < C; c += 32) row[c] = 0.f;
+  const float inv_cmk = 1.0f / (float)(C - K);
+  float rsum = 0.f;
+  uint32_t bad = 0;
+  int first = 0;
+  bool diff = false;
+  for (int h0 = 0; h0 < H; h0 += 32) {
+    const int h = h0 + lane;
+    float r = 0.f;
+    int id0 = 0;
+    bool dup = false;
+    if (h < H) {
+      float p[K];
+      int id[K];
+      compact_load<K>(ids, probs, (size_t)h * model_stride_e + (size_t)n * K, p, id);
+#pragma unroll
+      for (int j = 0; j < K; ++j) {
+        if (!isfinite(p[j])) bad |= CODA_B200_FLAG_NONFINITE_INPUT;
+        if (p[j] < 0.f || p[j] > 1.0001f || id[j] >= C) bad |= CODA_B200_FLAG_RANGE_INPUT;
+      }
+      r = compact_rest<K>(p, inv_cmk);
+      if (r < -1e-6f) bad |= CODA_B200_FLAG_RANGE_INPUT;
+#pragma unroll
+      for (int j = 0; j < K; ++j) {
+        stg[lane * K + j] = make_int2(id[j], __float_as_int(p[j] - r));
+#pragma unroll
+        for (int i = 0; i < j; ++i) dup |= id[i] == id[j];
+      }
+      hard[(size_t)n * H + h] = (uint16_t)id[0];               // ids are sorted by score: the first is the argmax
+      id0 = id[0];
+    }
+    if (h0 == 0) first = __shfl_sync(CODA_FULL, id0, 0);
+    diff |= __any_sync(CODA_FULL, h < H && id0 != first);
+    // a hand-built entry that repeats an id: this chunk's adds go one after another from lane 0, in k_scan_compact's order
+    const bool serial = __any_sync(CODA_FULL, dup);
+    __syncwarp();                                              // the staged pairs (and, the first time, the zeroed row)
+    const int hn = min(32, H - h0);
+    for (int k = 0; k < hn; ++k) {
+      rsum += __shfl_sync(CODA_FULL, r, k);
+      if (!serial && lane < K) {
+        const int2 a = stg[k * K + lane];
+        if (a.x < C) row[a.x] += __int_as_float(a.y);
+      } else if (serial && lane == 0) {
+        for (int j = 0; j < K; ++j) {
+          const int2 a = stg[k * K + j];
+          if (a.x < C) row[a.x] += __int_as_float(a.y);
+        }
+      }
+      __syncwarp();                                            // the next model may add to the same class
+    }
+  }
+  float bv = -INFINITY;
+  int bi = INT_MAX;
+  const float fH = (float)H;
+  for (int c = lane; c < C; c += 32) {
+    const float v = row[c] + rsum;
+    if (ens_out) ens_out[(size_t)n * C + c] = v;
+    const float mean = v / fH;                                 // util.py:14 mean(dim=0), then coda.py:194 argmax
+    if (mean > bv) { bv = mean; bi = c; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {                           // the largest mean, the first class among equal ones
+    const float ov = __shfl_xor_sync(CODA_FULL, bv, o);
+    const int oi = __shfl_xor_sync(CODA_FULL, bi, o);
+    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+  }
+  bad = __reduce_or_sync(CODA_FULL, bad);
+  if (lane == 0) {
+    pseudo[n] = bi == INT_MAX ? 0 : bi;
+    disagree[n] = (uint8_t)(diff ? 1 : 0);
+    if (bad) atomicOr(flags, bad);
+  }
+}
+
+// one thread per item holds a [C] row per thread in shared memory: it runs up to C = 1599 (32-thread blocks), but its
+// blocks shrink from C = 200.  On an H100 (H = 64, N = 1e5) the warp kernel is faster from C = 400 at K = 4 and 8 and
+// slower at C = 200, K = 8 (BASELINE §9), so it takes over at C = 400.
+#define SCAN_WARP_FROM_C 400
+
+// kernel: 0 = chosen by C, 1 = one thread per item (C <= SCAN_THREAD_MAX_C), 2 = one warp per item
+extern "C" int coda_b200_scan_compact_kernel(const uint16_t* ids, const float* probs, int64_t model_stride, int H,
+                                             int64_t N, int C, int K, uint16_t* hard, int32_t* pseudo,
+                                             uint8_t* disagree, float* ens_out, uint32_t* flags, int kernel,
+                                             coda_stream_t stream) {
   CODA_CHECK_ARG(ids && probs && hard && pseudo && disagree && flags, "scan_compact: null pointer");
   CODA_CHECK_ARG(K >= 1 && K <= CK_MAX && K < C && H >= 1 && N >= 1, "scan_compact: bad dims (K=%d)", K);
+  CODA_CHECK_ARG(C <= 4096, "scan_compact: C=%d too large for the compact path (C <= 4096)", C);
+  CODA_CHECK_ARG(kernel >= 0 && kernel <= 2, "scan_compact: bad kernel %d", kernel);
+  if (kernel == 0) kernel = C >= SCAN_WARP_FROM_C ? 2 : 1;
+  if (kernel == 2) {
+    const size_t smem = (size_t)SCW_WARPS * ((size_t)C * 4 + (size_t)32 * K * sizeof(int2));
+    const long long grid = (N + SCW_WARPS - 1) / SCW_WARPS;
+    CODA_CHECK_ARG(grid < (1LL << 31), "scan_compact: N=%lld too large", (long long)N);
+    CK_DISPATCH(K, {
+      CODA_CUDA_OK(cudaFuncSetAttribute(k_scan_compact_warp<KK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      k_scan_compact_warp<KK><<<(unsigned)grid, SCW_WARPS * 32, smem, as_stream(stream)>>>(
+          ids, probs, H, N, C, (long long)model_stride, hard, pseudo, disagree, ens_out, flags);
+    });
+    CODA_LAUNCH_OK("k_scan_compact_warp");
+    return CODA_B200_OK;
+  }
   const int cpad = C | 1;
   int threads = 256;
   while (threads > 32 && (size_t)threads * cpad * 4 > 200 * 1024) threads >>= 1;
   const size_t smem = (size_t)threads * cpad * 4;
-  CODA_CHECK_ARG(smem <= 200 * 1024, "scan_compact: C=%d too large for the compact path", C);
+  CODA_CHECK_ARG(smem <= 200 * 1024, "scan_compact: C=%d too large for one thread per item", C);
   const long long grid = (N + threads - 1) / threads;
   CK_DISPATCH(K, {
     CODA_CUDA_OK(cudaFuncSetAttribute(k_scan_compact<KK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -133,6 +252,13 @@ extern "C" int coda_b200_scan_compact(const uint16_t* ids, const float* probs, i
   });
   CODA_LAUNCH_OK("k_scan_compact");
   return CODA_B200_OK;
+}
+
+extern "C" int coda_b200_scan_compact(const uint16_t* ids, const float* probs, int64_t model_stride, int H, int64_t N,
+                                      int C, int K, uint16_t* hard, int32_t* pseudo, uint8_t* disagree, float* ens_out,
+                                      uint32_t* flags, coda_stream_t stream) {
+  return coda_b200_scan_compact_kernel(ids, probs, model_stride, H, N, C, K, hard, pseudo, disagree, ens_out, flags, 0,
+                                       stream);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -256,11 +382,59 @@ __global__ void __launch_bounds__(256) k_pi_full_compact(const uint16_t* __restr
   }
 }
 
+// C > 1024: the same per-warp body on the class window [c0, c0 + 1024) of blockIdx.y (c0 = 1024 blockIdx.y): the loads
+// of a DT row and of RS stay contiguous, and every element gets k_pi_full_compact's fmaf chain over (h, j).
+#define PFC_WIN 1024
+template <int K>
+__global__ void __launch_bounds__(256, 1) k_pi_full_compact_win(const uint16_t* __restrict__ ids, const float* __restrict__ probs,
+                                                             int H, long long N, int C, long long model_stride_e,
+                                                             const float* __restrict__ DT, const float* __restrict__ RS,
+                                                             float* __restrict__ U) {
+  constexpr int KCU = PFC_WIN / 32;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int c0 = blockIdx.y * PFC_WIN;
+  const float inv_cmk = 1.0f / (float)(C - K);
+  for (long long n = (long long)blockIdx.x * 8 + warp; n < N; n += (long long)gridDim.x * 8) {
+    float u[KCU];
+#pragma unroll
+    for (int k = 0; k < KCU; ++k) u[k] = 0.f;
+    for (int h = 0; h < H; ++h) {
+      const size_t e = (size_t)h * model_stride_e + (size_t)n * K;
+      float p[K];
+      int id[K];
+      compact_load<K>(ids, probs, e, p, id);          // broadcast loads (every lane the same address)
+      const float r = compact_rest<K>(p, inv_cmk);
+      const float* rs = RS + (size_t)h * C + c0;
+#pragma unroll
+      for (int k = 0; k < KCU; ++k) {
+        const int c = lane + 32 * k;
+        if (c0 + c < C) u[k] = fmaf(r, __ldg(rs + c), u[k]);
+      }
+#pragma unroll
+      for (int j = 0; j < K; ++j) {
+        if (id[j] >= C) continue;
+        const float w = p[j] - r;
+        const float* col = DT + ((size_t)h * C + id[j]) * C + c0;
+#pragma unroll
+        for (int k = 0; k < KCU; ++k) {
+          const int c = lane + 32 * k;
+          if (c0 + c < C) u[k] = fmaf(w, __ldg(col + c), u[k]);
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < KCU; ++k) {
+      const int c = lane + 32 * k;
+      if (c0 + c < C) U[(size_t)n * C + c0 + c] = u[k];
+    }
+  }
+}
+
 extern "C" int coda_b200_pi_full_compact(const uint16_t* ids, const float* probs, int64_t model_stride, const float* D,
                                          int H, int64_t N, int C, int K, float* DT_scratch, float* RS_scratch, float* U,
                                          coda_stream_t stream) {
   CODA_CHECK_ARG(ids && probs && D && DT_scratch && RS_scratch && U, "pi_full_compact: null pointer");
-  CODA_CHECK_ARG(K >= 1 && K <= CK_MAX && K < C && C <= 1024, "pi_full_compact: K=%d C=%d out of range", K, C);
+  CODA_CHECK_ARG(K >= 1 && K <= CK_MAX && K < C && C <= 4096, "pi_full_compact: K=%d C=%d out of range", K, C);
   cudaStream_t st = as_stream(stream);
   dim3 tg((unsigned)((C + 31) / 32), (unsigned)((C + 31) / 32), (unsigned)H), tb(32, 8);
   k_transpose_D<<<tg, tb, 0, st>>>(D, C, DT_scratch);
@@ -270,6 +444,13 @@ extern "C" int coda_b200_pi_full_compact(const uint16_t* ids, const float* probs
   CODA_LAUNCH_OK("k_rowsum_D");
   int grid = (int)min((long long)(N + 7) / 8, (long long)coda_sm_count() * 8);
   if (grid < 1) grid = 1;
+  if (C > PFC_WIN) {
+    const dim3 wg((unsigned)grid, (unsigned)((C + PFC_WIN - 1) / PFC_WIN));
+    CK_DISPATCH(K, (k_pi_full_compact_win<KK><<<wg, 256, 0, st>>>(ids, probs, H, N, C, (long long)model_stride, DT_scratch,
+                                                                  RS_scratch, U)));
+    CODA_LAUNCH_OK("k_pi_full_compact_win");
+    return CODA_B200_OK;
+  }
 #define LAUNCH_PFC(KCU) \
   CK_DISPATCH(K, (k_pi_full_compact<KCU, KK><<<grid, 256, 0, st>>>(ids, probs, H, N, C, (long long)model_stride, DT_scratch, RS_scratch, U)))
   if (C <= 32) LAUNCH_PFC(1);
@@ -298,13 +479,17 @@ __global__ void __launch_bounds__(256) k_pi_rank1_compact(const uint16_t* __rest
                                                           unsigned long long* __restrict__ pisum_fx,
                                                           uint32_t* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  long long* wacc_all = reinterpret_cast<long long*>(smem_raw);                 // [8][C]
-  R1Term* terms = reinterpret_cast<R1Term*>(wacc_all + (size_t)8 * C);          // [nt]
+  constexpr int NACC = KCU > 0 ? 8 : 1;                                         // KCU > 0: one [C] per warp; KCU == 0: one
+  long long* wacc_all = reinterpret_cast<long long*>(smem_raw);                 // [NACC][C]   for the block
+  R1Term* terms = reinterpret_cast<R1Term*>(wacc_all + (size_t)NACC * C);       // [nt]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t = (int)sel[1];
   const int nt = hdr[0], tp = hdr[1];
-  long long* wacc = wacc_all + (size_t)warp * C;
-  for (int c = lane; c < C; c += 32) wacc[c] = 0;
+  long long* wacc = wacc_all + (size_t)(KCU > 0 ? warp : 0) * C;
+  if (KCU > 0)
+    for (int c = lane; c < C; c += 32) wacc[c] = 0;
+  else
+    for (int c = threadIdx.x; c < C; c += blockDim.x) wacc[c] = 0;
   for (int k = threadIdx.x; k < nt; k += blockDim.x) terms[k] = gterms[k];
   __syncthreads();
   const float inv_cmk = 1.0f / (float)(C - K);
@@ -382,7 +567,8 @@ __global__ void __launch_bounds__(256) k_pi_rank1_compact(const uint16_t* __rest
       if (!isfinite(s)) bad |= CODA_B200_FLAG_NONFINITE_PI;
       const float den = fmaxf(s, 1e-12f);                               // coda.py:230 clamp_(min=1e-12)
       const float rden = 1.0f / den;
-      for (int c = lane; c < C; c += 32) wacc[c] += to_fx(row_quot(urow[c], den, rden), fxs);   // column t was rewritten by this lane
+      for (int c = lane; c < C; c += 32)        // column t was rewritten by this lane; integer sums: any order, same bits
+        atomicAdd(reinterpret_cast<unsigned long long*>(wacc) + c, (unsigned long long)to_fx(row_quot(urow[c], den, rden), fxs));
     }
   }
   if (KCU > 0) {
@@ -395,7 +581,7 @@ __global__ void __launch_bounds__(256) k_pi_rank1_compact(const uint16_t* __rest
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     long long s2 = 0;
-    for (int w = 0; w < 8; ++w) s2 += wacc_all[(size_t)w * C + c];
+    for (int w = 0; w < NACC; ++w) s2 += wacc_all[(size_t)w * C + c];
     if (s2) atomicAdd(pisum_fx + c, (unsigned long long)s2);
   }
   if (bad) atomicOr(flags, bad);
@@ -407,8 +593,8 @@ extern "C" int coda_b200_pi_rank1_compact(const uint16_t* ids, const float* prob
                                           coda_stream_t stream) {
   CODA_CHECK_ARG(ids && probs && sel && terms && U && pisum_fx && flags, "pi_rank1_compact: null pointer");
   CODA_CHECK_ARG(K >= 1 && K <= CK_MAX && K < C && 2 * H <= R1_MAXT, "pi_rank1_compact: bad dims");
-  const size_t smem = (size_t)8 * C * 8 + (size_t)2 * H * sizeof(R1Term);
-  CODA_CHECK_ARG(smem <= 200 * 1024, "pi_rank1_compact: C=%d too large", C);
+  CODA_CHECK_ARG(C <= 4096, "pi_rank1_compact: C=%d too large", C);
+  const size_t smem = (size_t)(C <= 1024 ? 8 : 1) * C * 8 + (size_t)2 * H * sizeof(R1Term);   // NACC of the KCU below
   int grid = (int)min((long long)(N + 255) / 256, (long long)coda_sm_count() * 4);
   if (grid < 1) grid = 1;
 #define LAUNCH_R1C(KCU)                                                                                                  \
@@ -574,12 +760,16 @@ __global__ void __launch_bounds__(256) k_r1i_rows(const float* __restrict__ R, u
                                                   float* __restrict__ U, unsigned long long* __restrict__ pisum_fx,
                                                   uint32_t* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  long long* wacc_all = reinterpret_cast<long long*>(smem_raw);                 // [8][C]
+  constexpr int NACC = KCU > 0 ? 8 : 1;                                         // as in k_pi_rank1_compact
+  long long* wacc_all = reinterpret_cast<long long*>(smem_raw);                 // [NACC][C]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t = (int)sel[1];
   const bool valid = !(hdr[0] == 0 && hdr[1] < 0);
-  long long* wacc = wacc_all + (size_t)warp * C;
-  for (int c = lane; c < C; c += 32) wacc[c] = 0;
+  long long* wacc = wacc_all + (size_t)(KCU > 0 ? warp : 0) * C;
+  if (KCU > 0)
+    for (int c = lane; c < C; c += 32) wacc[c] = 0;
+  else
+    for (int c = threadIdx.x; c < C; c += blockDim.x) wacc[c] = 0;
   __syncthreads();
   uint32_t bad = 0;
   long long racc[KCU > 0 ? KCU : 1];
@@ -639,7 +829,8 @@ __global__ void __launch_bounds__(256) k_r1i_rows(const float* __restrict__ R, u
       if (!isfinite(s)) bad |= CODA_B200_FLAG_NONFINITE_PI;
       const float den = fmaxf(s, 1e-12f);                               // coda.py:230 clamp_(min=1e-12)
       const float rden = 1.0f / den;
-      for (int c = lane; c < C; c += 32) wacc[c] += to_fx(row_quot(urow[c], den, rden), fxs);   // column t was rewritten by this lane
+      for (int c = lane; c < C; c += 32)        // column t was rewritten by this lane; integer sums: any order, same bits
+        atomicAdd(reinterpret_cast<unsigned long long*>(wacc) + c, (unsigned long long)to_fx(row_quot(urow[c], den, rden), fxs));
     }
   }
   if (KCU > 0) {
@@ -652,7 +843,7 @@ __global__ void __launch_bounds__(256) k_r1i_rows(const float* __restrict__ R, u
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     long long s2 = 0;
-    for (int w = 0; w < 8; ++w) s2 += wacc_all[(size_t)w * C + c];
+    for (int w = 0; w < NACC; ++w) s2 += wacc_all[(size_t)w * C + c];
     if (s2) atomicAdd(pisum_fx + c, (unsigned long long)s2);
   }
   if (bad) atomicOr(flags, bad);
@@ -667,8 +858,8 @@ extern "C" int coda_b200_pi_rank1_index(const int64_t* offsets, const void* entr
   CODA_CHECK_ARG(offsets && entries && rest_sum && jvec && sel && terms && delta && U && pisum_fx && flags,
                  "pi_rank1_index: null pointer");
   CODA_CHECK_ARG(H >= 1 && H <= 2048 && N >= 1 && C >= 2, "pi_rank1_index: bad dims");
-  const size_t smem = (size_t)8 * C * 8;
-  CODA_CHECK_ARG(smem <= 200 * 1024, "pi_rank1_index: C=%d too large", C);
+  CODA_CHECK_ARG(C <= 4096, "pi_rank1_index: C=%d too large", C);
+  const size_t smem = (size_t)(C <= 1024 ? 8 : 1) * C * 8;                     // NACC of the KCU below
   k_r1i_scatter<<<dim3(8, (unsigned)H), 256, 0, as_stream(stream)>>>(
       reinterpret_cast<const long long*>(offsets), reinterpret_cast<const uint2*>(entries), jvec, terms, C,
       exp2f((float)CIDX_FX_SHIFT), reinterpret_cast<unsigned long long*>(delta));

@@ -199,11 +199,17 @@ int coda_b200_pi_rank1_x(const void* preds, int fmt, const float* ens_base, int 
 int coda_b200_scan_compact(const uint16_t* ids, const float* probs, int64_t model_stride, int H, int64_t N, int C,
                            int K, uint16_t* hard, int32_t* pseudo, uint8_t* disagree, float* ens_out, uint32_t* flags,
                            coda_stream_t stream);
+/* coda_b200_scan_compact with its kernel named: 0 = the one it chooses by C, 1 = one thread per item (C <= 1599),
+ * 2 = one warp per item (C <= 4096).  Both give the same bits; this lets a benchmark time one against the other. */
+int coda_b200_scan_compact_kernel(const uint16_t* ids, const float* probs, int64_t model_stride, int H, int64_t N,
+                                  int C, int K, uint16_t* hard, int32_t* pseudo, uint8_t* disagree, float* ens_out,
+                                  uint32_t* flags, int kernel, coda_stream_t stream);
 /* coda.py:42: conf[h][y][j] == conf_fx[h][y][j] + conf_rest[h][y] (both ACCUMULATED into, int64 fixed point). */
 int coda_b200_confusion_compact(const uint16_t* ids, const float* probs, int64_t model_stride, const int32_t* pseudo,
                                 int H, int64_t N, int C, int K, int fx_shift, int64_t* conf_fx, int64_t* conf_rest,
                                 coda_stream_t stream);
-/* coda.py:227-229.  DT_scratch [H][C][C] and RS_scratch [H][C] floats are overwritten (D transposed, row sums). */
+/* coda.py:227-229, K < C <= 4096.  DT_scratch [H][C][C] and RS_scratch [H][C] floats are overwritten (D transposed,
+ * row sums). */
 int coda_b200_pi_full_compact(const uint16_t* ids, const float* probs, int64_t model_stride, const float* D, int H,
                               int64_t N, int C, int K, float* DT_scratch, float* RS_scratch, float* U,
                               coda_stream_t stream);

@@ -25,6 +25,10 @@ and device loops can follow each other.  Draws whose consumption is known up fro
 draws the reference makes from torch's generators (tie breaks, ModelPicker's draws) come from a Philox4x32-10 stream
 by default, or with ``tie_rule="reference"`` from device replicas of torch's CPU and CUDA generators, call for call
 (``include/coda_b200.h``, DESIGN.md §5b).
+
+Checkpoints: ``state_dict()`` / ``load_state_dict()`` save and restore what a run has learned (labels, removed items,
+the method's host-side sums, the loop history) and the three generators, with no layout; the next ``run_steps`` rebuilds
+the device loop's sums from that host state (``_loop_upload``), so a resumed run continues bit for bit in one process.
 """
 from __future__ import annotations
 
@@ -117,6 +121,68 @@ def cuda_rng_words(state: torch.Tensor) -> torch.Tensor:
 
 def cuda_rng_state(words: torch.Tensor) -> torch.Tensor:
     return torch.from_numpy(words.numpy().astype("<i8").view(np.uint8).copy())
+
+
+# -- checkpoints (state_dict / load_state_dict) ---------------------------------------------------------------------
+STATE_VERSION = 1
+# what each method (by its main.py --method name) has learned beyond the labels: the "fields" of its state
+STATE_FIELDS = {"iid": ("risk_sum",), "uncertainty": ("risk_sum",), "activetesting": ("losses", "qs", "M"),
+                "vma": ("losses", "qs", "M"), "model_picker": ("posterior", "correct_counts", "n_disagree")}
+_HIST_KEYS = (("idx", torch.int64), ("q", torch.float64), ("tie", torch.int32), ("best", torch.int32),
+              ("best_tie", torch.int32))
+_STATE_KEYS = ("d_l_idxs", "d_l_ys", "removed", "stochastic", "dev_steps", "history", "fields", "rng")
+
+
+def pack_state(method, H, N, C, epsilon=None, *, labeled=(), labels=(), removed=(), stochastic=False, history=None,
+               fields=None, rng=None):
+    """A competing selector's checkpoint from host values.  It holds ints, floats, strings, lists, tuples, dicts, None
+    and CPU tensors only, so ``torch.save`` / ``torch.load`` (``weights_only=True``) round-trip it, and no shard layout.
+    ``labeled`` / ``labels``: ``d_l_idxs`` / ``d_l_ys``; ``removed``: the items taken out of ``d_u_idxs`` without a label;
+    ``history``: the device-loop arrays of ``history()`` / ``best_history()`` by key (idx, q, tie, best, best_tie;
+    a missing key is empty); ``fields``: the method's own (``STATE_FIELDS``); ``rng``: ``{"python": random.getstate(),
+    "torch": torch.get_rng_state(), "cuda": torch.cuda.get_rng_state(device)}``."""
+    history = history or {}
+    hist = {k: torch.tensor(np.asarray(history.get(k, ())), dtype=dt).reshape(-1) for k, dt in _HIST_KEYS}
+    return {"version": STATE_VERSION, "method": method, "H": int(H), "N": int(N), "C": int(C),
+            "epsilon": None if epsilon is None else float(epsilon),
+            "d_l_idxs": [int(i) for i in labeled], "d_l_ys": [int(y) for y in labels],
+            "removed": sorted(int(i) for i in removed), "stochastic": bool(stochastic),
+            "dev_steps": int(hist["idx"].numel()), "history": hist, "fields": dict(fields or {}), "rng": dict(rng or {})}
+
+
+def check_state(sd, method, H, N, C, epsilon=None):
+    """Raise ``ValueError`` unless ``sd`` is a version-1 checkpoint of ``method`` on an (H, N, C) task (and, for
+    ModelPicker, with this ``epsilon``) whose item lists and sums fit that task."""
+    if not isinstance(sd, dict):
+        raise ValueError(f"coda_b200.baselines: a state_dict is a dict, got {type(sd).__name__}")
+    if sd.get("version") != STATE_VERSION:
+        raise ValueError(f"coda_b200.baselines: state_dict version {sd.get('version')!r}; this package reads version "
+                         f"{STATE_VERSION}")
+    if sd.get("method") != method:
+        raise ValueError(f"coda_b200.baselines: the state_dict is of method {sd.get('method')!r}, not {method!r}")
+    if (sd.get("H"), sd.get("N"), sd.get("C")) != (H, N, C):
+        raise ValueError(f"coda_b200.baselines: the state_dict belongs to a task of (H, N, C) = "
+                         f"{(sd.get('H'), sd.get('N'), sd.get('C'))}, not {(H, N, C)}")
+    eps = None if epsilon is None else float(epsilon)
+    if sd.get("epsilon") != eps:
+        raise ValueError(f"coda_b200.baselines: the state_dict has epsilon {sd.get('epsilon')!r}, this selector {eps!r}")
+    missing = [k for k in _STATE_KEYS if k not in sd]
+    missing += [k for k in STATE_FIELDS[method] if k not in (sd.get("fields") or {})]
+    missing += [k for k, _ in _HIST_KEYS if k not in (sd.get("history") or {})]
+    if missing:
+        raise ValueError(f"coda_b200.baselines: the state_dict lacks {missing}")
+    items = list(sd["d_l_idxs"]) + list(sd["removed"])
+    if len(sd["d_l_ys"]) != len(sd["d_l_idxs"]) or len(set(items)) != len(items) or any(
+            not 0 <= int(i) < N for i in items):
+        raise ValueError("coda_b200.baselines: the state_dict's labeled and removed items are not distinct items of "
+                         "the task with one label each")
+    if any(int(sd["history"][k].numel()) != int(sd["dev_steps"]) for k, _ in _HIST_KEYS):
+        raise ValueError("coda_b200.baselines: the state_dict's history arrays do not all hold dev_steps entries")
+    f = sd["fields"]
+    sizes = {"risk_sum": H, "posterior": H, "correct_counts": H}
+    if any(k in f and f[k].numel() != n for k, n in sizes.items()) or (
+            "losses" in f and (tuple(f["losses"].shape) != (int(f["M"]), H) or len(f["qs"]) != int(f["M"]))):
+        raise ValueError(f"coda_b200.baselines: the state_dict's sums do not fit a task of H = {H} models")
 
 
 def _synced(fn):
@@ -897,6 +963,67 @@ class _Baseline(ModelSelector):
             self._pull()
         return self._hist_arrays("best", "best_tie")
 
+    # -- checkpoint / resume (the reference restarts a killed seed from step 0) -------------------------------------
+    _state_method = None            # the method's name in its state dict (main.py --method)
+
+    def _state_refusals(self):
+        if self.group.world > 1 and len(self.states) == 1:
+            raise NotImplementedError("coda_b200.baselines: state_dict / load_state_dict need all items in one "
+                                      "process: build the selector with gpus= / shards= (one process driving all "
+                                      "GPUs) instead of one process per GPU")
+
+    def state_dict(self):
+        """The run so far as a plain dict (``pack_state``): the labels, the items removed without one, the method's
+        sums, ``stochastic``, the device-loop history and the states of Python ``random``, torch's CPU generator and
+        the CUDA generator of the dataset's device.  Device-loop steps not yet mirrored are pulled first.  It holds
+        no layout: a selector of the same method on the same slab values loads it under any shard layout, slab width
+        or piece split."""
+        self._state_refusals()
+        if self._loop_dirty:
+            self._pull()
+        labeled = set(self.d_l_idxs)
+        keys = [k for k, _ in _HIST_KEYS]
+        rng = {"python": random.getstate(), "torch": torch.get_rng_state(),
+               "cuda": torch.cuda.get_rng_state(self.device)}
+        return pack_state(self._state_method, self.H, self.N, self.C, getattr(self, "epsilon", None),
+                          labeled=self.d_l_idxs, labels=self.d_l_ys,
+                          removed=[i for i in self.d_u_idxs._removed if i not in labeled], stochastic=self.stochastic,
+                          history=dict(zip(keys, self._hist_arrays(*keys))), fields=self._state_fields(), rng=rng)
+
+    def load_state_dict(self, sd, restore_rng=True):
+        """Resume a run saved by ``state_dict`` on a freshly built selector of the same method on the same task: the
+        next API steps and ``run_steps`` continue it bit for bit.  Every shard's labeled mask is rebuilt from the item
+        lists, and the device loop is re-uploaded from the restored host state on the next ``run_steps``.
+        ``restore_rng=False`` leaves the caller's generators as they are."""
+        self._state_refusals()
+        check_state(sd, self._state_method, self.H, self.N, self.C, getattr(self, "epsilon", None))
+        items = [int(i) for i in sd["d_l_idxs"]] + [int(i) for i in sd["removed"]]
+        for st in self.states:
+            st.enter()
+            loc = [i - st.n_offset for i in items if 0 <= i - st.n_offset < st.N]
+            with st._on():
+                st.labeled.zero_()
+                if loc:
+                    st.labeled[torch.tensor(loc, dtype=torch.int64, device=st.dev)] = 1
+            st.leave()
+            st.lgraph = None                                   # captured graphs and loop words are of the old run
+        self.d_u_idxs._removed = set(items)
+        self.d_u_idxs._sorted = sorted(items)
+        self.d_l_idxs = [int(i) for i in sd["d_l_idxs"]]
+        self.d_l_ys = [int(y) for y in sd["d_l_ys"]]
+        self.stochastic = bool(sd["stochastic"])
+        h = sd["history"]
+        self._hist = {k: [h[k].numpy().copy()] if h[k].numel() else [] for k, _ in _HIST_KEYS}
+        self._dev_steps = self._hist_seen = int(sd["dev_steps"])
+        self._loop_dirty = False
+        self._dev_nlab = -1                                    # the next run_steps uploads the restored sums
+        self._load_fields(sd["fields"])
+        if restore_rng:
+            rng = sd["rng"]
+            random.setstate(rng["python"])
+            torch.set_rng_state(rng["torch"])
+            torch.cuda.set_rng_state(rng["cuda"], self.device)
+
     def close(self):
         """Free the device buffers and mailboxes of every shard now (a script can then build the next selector on the
         same card)."""
@@ -915,12 +1042,19 @@ class IID(_Baseline):
     """Uniform sampling of the unlabeled items; the best model has the lowest mean loss on the labels (iid.py)."""
 
     _loop_method, _loop_draw = nat.BL_IID, "choice"
+    _state_method = "iid"
 
     def __init__(self, dataset, loss_fn, *, gpus=None, shards=None, comm=None):
         self._setup(dataset, gpus, shards, comm)
         self.loss_fn = loss_fn
         self.stochastic = True
         self._risk_sum = torch.zeros(self.H, device=self.device)
+
+    def _state_fields(self):
+        return {"risk_sum": self._risk_sum.cpu()}
+
+    def _load_fields(self, f):
+        self._risk_sum = f["risk_sum"].to(self.device, torch.float32)
 
     def _loss(self, col, true_class, dev):
         return self.loss_fn(col, torch.tensor([true_class], device=dev).expand(self.H))
@@ -955,6 +1089,7 @@ class Uncertainty(IID):
     """The unlabeled item of highest ensemble-mean entropy (uncertainty.py); a static score."""
 
     _loop_method, _loop_draw = nat.BL_UNCERTAINTY, None
+    _state_method = "uncertainty"
 
     def __init__(self, dataset, loss_fn, *, gpus=None, shards=None, comm=None):
         super().__init__(dataset, loss_fn, gpus=gpus, shards=shards, comm=comm)
@@ -984,6 +1119,7 @@ class ActiveTesting(IID):
 
     _vma = False
     _loop_method, _loop_draw = nat.BL_ACTIVETESTING, "random"
+    _state_method = "activetesting"
 
     def __init__(self, dataset, loss_fn, *, gpus=None, shards=None, comm=None):
         super().__init__(dataset, loss_fn, gpus=gpus, shards=shards, comm=comm)
@@ -995,6 +1131,16 @@ class ActiveTesting(IID):
         self.losses = []
         self.qs = []
         self.stochastic = True
+
+    def _state_fields(self):
+        # one [H] row per label (get_lure_risks_and_vars stacks and views them as [H][M] whatever their shape)
+        losses = torch.stack([L.reshape(-1) for L in self.losses]).cpu() if self.losses else torch.zeros(0, self.H)
+        return {"losses": losses, "qs": [float(q) for q in self.qs], "M": int(self.M)}
+
+    def _load_fields(self, f):
+        self.losses = list(f["losses"].to(self.device).unbind(0))
+        self.qs = [float(q) for q in f["qs"]]
+        self.M = int(f["M"])
 
     def _loss(self, col, true_class, dev):
         return self.loss_fn(col, torch.tensor([true_class], device=dev).repeat(self.H), reduction="none")
@@ -1046,6 +1192,7 @@ class VMA(ActiveTesting):
 
     _vma = True
     _loop_method = nat.BL_VMA
+    _state_method = "vma"
 
     @_synced
     def get_next_item_to_label(self):
@@ -1060,6 +1207,7 @@ class ModelPicker(_Baseline):
     the one with the most correct labels (modelpicker.py)."""
 
     _loop_method = nat.BL_MODELPICKER
+    _state_method = "model_picker"
 
     def __init__(self, dataset, epsilon=0.46, *, gpus=None, shards=None, comm=None):
         self._setup(dataset, gpus, shards, comm)
@@ -1077,6 +1225,15 @@ class ModelPicker(_Baseline):
         self.posterior = torch.ones(self.H, device=self.device) / self.H
         self.correct_counts = torch.zeros(self.H, dtype=torch.long, device=self.device)
         self.stochastic = True
+
+    def _state_fields(self):
+        return {"posterior": self.posterior.cpu(), "correct_counts": self.correct_counts.cpu(),
+                "n_disagree": int(self._n_disagree)}
+
+    def _load_fields(self, f):
+        self.posterior = f["posterior"].to(self.device, torch.float32)
+        self.correct_counts = f["correct_counts"].to(self.device, torch.int64)
+        self._n_disagree = int(f["n_disagree"])
 
     def _all_disagree(self):
         """The unanimity bits of ALL items on the host (one process per GPU: all-gathered from the ranks)."""

@@ -854,7 +854,7 @@ __global__ void __launch_bounds__(BL_THREADS) k_bl_step(const coda_bl_loop_t a, 
       a.s1[h] = s1;
       a.s2[h] = s2;
       if (a.hist_loss) a.hist_loss[(size_t)slot * H + h] = L;
-      rv[h] = (s1 + (Ng - m) * s2) / m;
+      rv[h] = bl_lure_risk(s1, s2, Ng, m);
     }
   } else if (a.method == CODA_B200_BL_MODELPICKER) {
     // modelpicker.py:89-95: post * gamma^agree / sum (fp32 products, the sum in fp64 in a fixed order, rounded once)

@@ -8,6 +8,7 @@
 //     below 2^28, and advances the offset by 4 (one element: one curand4 per thread, 4 counter words).
 // Each kernel is one warp; the words of the CPU replica live in shared memory between a load and a store, as
 // pyrandom.cuh's do.  Every shard runs the same kernels on the same global counts, so the replicas need no exchange.
+#include "modelpicker.cuh"
 #include "pyrandom.cuh"
 #include <curand_kernel.h>
 
@@ -94,10 +95,7 @@ __global__ void __launch_bounds__(32) k_bl_best_ref(const coda_bl_loop_t a, uint
   const bool mp = a.method == CODA_B200_BL_MODELPICKER;
   const double Ng = (double)a.n_global, m = (double)M;
   auto rv = [&](int h) -> double {                          // the value bl_step's best model minimises
-    if (lure) {
-      const double s1 = a.s1[h], s2 = a.s2[h];
-      return (s1 + (Ng - m) * s2) / m;
-    }
+    if (lure) return bl_lure_risk(a.s1[h], a.s2[h], Ng, m);
     return mp ? -(double)a.counts[h] : (double)a.counts[h];
   };
   double mn = INFINITY;

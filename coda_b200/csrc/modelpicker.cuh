@@ -94,3 +94,11 @@ __device__ __forceinline__ long long bl_tie_pick(unsigned r, long long cnt) {
   const unsigned long long c = (unsigned long long)cnt, lo = (unsigned long long)r * (c & 0xffffffffull);
   return (long long)(((unsigned long long)r * (c >> 32)) + (lo >> 32));
 }
+
+// One model's LURE risk from the loop's running sums after m labels of Ng items: (s1 + (Ng - m) s2) / m, the product
+// and the sum as one explicit fused multiply-add.  k_bl_step and k_bl_best_ref both decide the best model's exact ties
+// on it, so they see the same bits whatever the compiler would contract (tests/test_selector_kernels.py models it as
+// fl(fma(Ng - m, s2, s1) / m)).  At m = Ng it is s1 / m, the plain mean loss.
+__device__ __forceinline__ double bl_lure_risk(double s1, double s2, double Ng, double m) {
+  return __fma_rn(Ng - m, s2, s1) / m;
+}

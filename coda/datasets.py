@@ -1,7 +1,7 @@
 import os
 
 from coda_b200.datasets import Dataset as _Dataset
-from coda_b200.datasets import compact_load_count, is_compact_file, shard_load_count
+from coda_b200.datasets import compact_load_count, host_load_wanted, is_compact_file, shard_load_count
 
 
 class Dataset(_Dataset):
@@ -13,7 +13,11 @@ class Dataset(_Dataset):
     A file written by ``coda_b200.CompactSlab.save`` loads as a compact slab, and ``CODA_B200_COMPACT_K=K`` compacts a
     dense task file to its top-K form as it loads (opt-in: the compact form approximates the tail classes, so results
     differ from the dense run).  The piece count follows the same rule on the compact byte count
-    (``coda_b200.datasets.ShardedCompactSlab`` for more than one piece)."""
+    (``coda_b200.datasets.ShardedCompactSlab`` for more than one piece).
+
+    ``CODA_B200_HOST_SLAB=1``, or a dense slab larger than the target device's free memory with exactly one GPU
+    visible, keeps it in host memory (``coda_b200.datasets.HostSlab``) and runs it exactly on that GPU;
+    ``CODA_B200_HOST_SLAB=0`` never does.  Compact files and ``CODA_B200_COMPACT_K`` take precedence."""
 
     def __init__(self, filepath, device):
         keep = os.environ.get("CODA_B200_KEEP_DTYPE", "0") == "1"
@@ -22,6 +26,9 @@ class Dataset(_Dataset):
         if k or is_compact_file(filepath):
             shards = compact_load_count(filepath, device, k)
             super().__init__(filepath, device, compact_k=k, shards=shards or None)
+            return
+        if host_load_wanted(filepath, device, keep):
+            super().__init__(filepath, device, keep_dtype=keep, host=True)
             return
         shards = shard_load_count(filepath, device, keep)
         if shards:

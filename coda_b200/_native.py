@@ -67,7 +67,7 @@ class StepStruct(C.Structure):
         ("pisum_fx", p), ("PB", p), ("pi_hat", p), ("m0", p), ("h_before", p), ("best_model", p),
         ("partials", p), ("nblocks", i32), ("eig", p), ("bestrec", p),
         ("labels_global", p), ("hist_idx", p), ("hist_q", p), ("hist_tie", p), ("hist_cap", i64), ("step_ctr", p),
-        ("flags", p),
+        ("flags", p), ("n_host", i64), ("host_shadow", p), ("stage", p), ("stage_off", i64),
     ]
 
 
@@ -140,6 +140,9 @@ SIGNATURES = {
     "coda_b200_step_select": (i32, [PS, PX, p]),
     "coda_b200_step_merge": (i32, [PS, PX, p]),
     "coda_b200_step_label": (i32, [PS, PX, p]),
+    "coda_b200_host_stage": (i32, [PS, i32, p, p]),
+    "coda_b200_host_register": (i32, [p, sz]),
+    "coda_b200_host_unregister": (i32, [p]),
     "coda_b200_step_mixture": (i32, [PS, PX, p]),
     "coda_b200_record_best": (i32, [p, p, p, i64, p]),
     "coda_b200_ties": (i32, [p, i64, p, p, i64, p, i32, p, p, p, p]),

@@ -241,14 +241,18 @@ class _DeviceState:
     rep_words = 8          # the exchanges use the mailbox's record slot; the report slot is kept at its minimum
 
     def __init__(self, preds, n_offset=0, world=1, own_stream=False):
-        from .datasets import CompactSlab
+        from .datasets import CompactSlab, HostSlab
         self.compact = preds if isinstance(preds, CompactSlab) else None
-        if not ((isinstance(preds, torch.Tensor) or self.compact is not None) and preds.is_cuda):
+        self.host = preds if isinstance(preds, HostSlab) else None       # streamed through the device by the scan
+        if not ((isinstance(preds, torch.Tensor) or self.compact is not None or self.host is not None) and preds.is_cuda):
             raise NotImplementedError(_NO_CPU)
         H, N, C = (int(s) for s in preds.shape)
         if self.compact is not None:
             self.fmt = None
             self.model_stride = int(preds.ids.stride(0)) if H > 1 else N * preds.K
+        elif self.host is not None:
+            self.fmt = nat.slab_format(preds.dtype)
+            self.model_stride = N * C
         else:
             self.fmt = nat.slab_format(preds.dtype)  # float32, float16 or bfloat16 (read at its stored width)
             if preds.dim() != 3:
@@ -315,12 +319,12 @@ class _DeviceState:
                 cs = self.compact
                 self._call("coda_b200_scan_compact", _ptr(cs.ids), _ptr(cs.probs), self.model_stride, H, N, C, cs.K,
                            _ptr(hard), _ptr(pseudo), _ptr(disagree), _ptr(e), _ptr(self.flags), self._s())
-            elif self.fmt == nat.SLAB_F32:
-                self._call("coda_b200_scan_slab", _ptr(self.preds), self.model_stride, H, N, C, _ptr(hard), _ptr(pseudo),
-                           _ptr(disagree), _ptr(e), _ptr(self.flags), self._s())
+            elif self.host is not None:                    # N-range chunks: the scan is per item
+                self.host.walk(lambda n0, n1, v: self._scan_dense(_ptr(v), (n1 - n0) * C, n1 - n0, _ptr(hard[n0:]),
+                                                                  _ptr(pseudo[n0:]), _ptr(disagree[n0:]),
+                                                                  _ptr(e[n0:]) if e is not None else None))
             else:
-                self._call("coda_b200_scan_slab_x", _ptr(self.preds), self.fmt, self.model_stride, H, N, C, _ptr(hard),
-                           _ptr(pseudo), _ptr(disagree), _ptr(e), _ptr(self.flags), self._s())
+                self._scan_dense(_ptr(self.preds), self.model_stride, N, _ptr(hard), _ptr(pseudo), _ptr(disagree), _ptr(e))
             flags = int(self.flags.item())
         if flags & nat.FLAG_NONFINITE_INPUT:
             raise RuntimeError("[NUMERIC ERROR] preds has bad values (NaN/Inf)")
@@ -328,10 +332,21 @@ class _DeviceState:
             raise ValueError("coda_b200: dataset.preds must hold post-softmax scores in [0, 1] (coda/datasets.py:6)")
         return hard, disagree, e
 
+    def _scan_dense(self, base, model_stride, n, hard, pseudo, disagree, e):
+        H, C = self.H, self.C
+        if self.fmt == nat.SLAB_F32:
+            self._call("coda_b200_scan_slab", base, model_stride, H, n, C, hard, pseudo, disagree, e, _ptr(self.flags),
+                       self._s())
+        else:
+            self._call("coda_b200_scan_slab_x", base, self.fmt, model_stride, H, n, C, hard, pseudo, disagree, e,
+                       _ptr(self.flags), self._s())
+
     def column(self, loc):
         """The (H, C) fp32 scores of local item ``loc`` (a 16-bit slab widened, a compact slab densified)."""
         if self.compact is not None:
             return self.compact.item_column(loc)
+        if self.host is not None:
+            return self.host.item_column(loc)
         return self.preds[:, loc, :].float()
 
     def static_scores(self, hard, ens, vma):
@@ -533,8 +548,12 @@ def _check_rank_ranges(preds, n_offset, N, n_global, comm):
 
 def _layout(dataset, gpus, shards, comm):
     """-> (group, [(shard slab, n_offset)] of this process)."""
-    from .datasets import CompactSlab, ShardedCompactSlab, ShardedSlab
+    from .datasets import CompactSlab, HostSlab, ShardedCompactSlab, ShardedSlab
+    from .selector import host_slab_refusals
     preds = getattr(dataset, "preds", None)
+    if isinstance(preds, HostSlab):                             # one shard on the slab's compute device
+        host_slab_refusals(gpus, shards, comm.world)
+        return SoloGroup(), [(preds, 0)]
     if isinstance(preds, (ShardedSlab, ShardedCompactSlab)):    # the pieces are the shards
         layout = piece_layout(preds, gpus, shards, comm.world)
         if not preds.is_cuda:
@@ -1287,7 +1306,7 @@ class ModelPicker(_Baseline):
             preds = self.state.hard[int(chosen_idx)].to(torch.int64) & 0xFFFF
         else:
             st = self.state                                   # the one shard's slab (a ShardedSlab's only piece)
-            preds = st.preds[:, int(chosen_idx) - st.n_offset].argmax(dim=1)
+            preds = st.column(int(chosen_idx) - st.n_offset).argmax(dim=1)
         self.correct_counts += (preds == true_class).long()
         self.posterior = self.update_posterior(self.posterior, preds, true_class, self.gamma)
 

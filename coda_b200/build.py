@@ -12,7 +12,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libcoda_b200.so")
 SOURCES = ["api.cu", "xchg.cu", "slab.cu", "tables.cu", "pairs.cu", "pairs_tc.cu", "pi_tc.cu", "gain.cu", "step.cu", "step_defer.cu", "compact.cu", "baselines.cu",
-           "eps_search.cu", "sample.cu", "bl_ref.cu", "true_loss.cu", "compact_build.cu", "preload.cu"]
+           "eps_search.cu", "sample.cu", "bl_ref.cu", "true_loss.cu", "compact_build.cu", "preload.cu",
+           "host_stage.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",

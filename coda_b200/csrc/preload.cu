@@ -22,6 +22,7 @@ const void* coda_anchor_compact(void);
 const void* coda_anchor_compact_build(void);
 const void* coda_anchor_eps_search(void);
 const void* coda_anchor_gain(void);
+const void* coda_anchor_host_stage(void);
 const void* coda_anchor_pairs(void);
 const void* coda_anchor_pairs_tc(void);
 const void* coda_anchor_pi_tc(void);
@@ -67,7 +68,8 @@ extern "C" int coda_b200_preload_kernels(int64_t* loaded_host) {
   const void* anchors[] = {coda_anchor_baselines(), coda_anchor_bl_ref(), coda_anchor_compact(), coda_anchor_eps_search(),
                            coda_anchor_gain(),      coda_anchor_pairs(),  coda_anchor_pairs_tc(), coda_anchor_pi_tc(),
                            coda_anchor_sample(),    coda_anchor_slab(),   coda_anchor_step(),     coda_anchor_step_defer(),
-                           coda_anchor_tables(),    coda_anchor_true_loss(),  coda_anchor_compact_build()};
+                           coda_anchor_tables(),    coda_anchor_true_loss(),  coda_anchor_compact_build(),
+                           coda_anchor_host_stage()};
   int64_t loaded = 0;
   for (const void* a : anchors) {
     cudaKernel_t k;

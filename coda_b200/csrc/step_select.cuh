@@ -73,6 +73,12 @@ STEP_LINKAGE __device__ void apply_label(const coda_step_t& a, int t, const int*
       // compact slab: a term names (model, class); pi_rank1_compact resolves it by a K-way match
       terms[k] = R1Term{(long long)h, 1.f, j};
       if (n == 2) terms[k + 1] = R1Term{(long long)h, -1.f, tp};
+    } else if (n && a.n_host > 0 && a.slot_of_model[h] >= H - a.n_host) {
+      // host slot: column (slot - S, class) of the pinned host slots, item stride 0 until coda_b200_host_stage
+      // copies it to a staging column and points the term there
+      const long long hb = (long long)(a.slot_of_model[h] - (H - a.n_host)) * C * a.shadow_col_stride;
+      terms[k] = R1Term{hb + (long long)j * a.shadow_col_stride, 1.f, 0};
+      if (n == 2) terms[k + 1] = R1Term{hb + (long long)tp * a.shadow_col_stride, -1.f, 0};
     } else if (n) {
       const int slot = a.slot_of_model ? a.slot_of_model[h] : -1;
       // shadow: [slot][class][col_stride] (item stride 1); reference layout: [model][item][class] (item stride C)

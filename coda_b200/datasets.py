@@ -70,6 +70,136 @@ class ShardedSlab:
         return self.pieces[r][:, idx - self.offsets[r]].float()
 
 
+HOST_CHUNK_BYTES = 1 << 30
+HOST_CHUNK_ALIGN = 32           # items: a multiple of the slab scan's tile, so a chunk takes the scan the whole slab takes
+
+
+class HostSlab:
+    """An (H, N, C) slab kept in host memory -- a contiguous CPU tensor, possibly memory-mapped from a ``torch.save``
+    file -- for one compute ``device``: a task larger than one GPU, run exactly on that GPU.  CODA, the competing
+    selectors and ``Oracle.true_losses`` stream it through the device in N-range chunks of ``chunk_items`` items (two
+    device buffers of one chunk each); the slab is never copied whole to the device.  Duck-types ``ShardedSlab``'s
+    surface: ``shape``, ``dtype`` (the width the kernels read: the tensor's, or float32 to widen a 16-bit tensor on
+    the device), ``device``, ``numel``, ``element_size``, ``item_column``."""
+
+    def __init__(self, preds: torch.Tensor, device, dtype=None, chunk_items=None):
+        if not isinstance(preds, torch.Tensor) or preds.device.type != "cpu":
+            raise TypeError("HostSlab: a CPU (H, N, C) tensor expected")
+        if preds.dim() != 3 or preds.dtype not in _KEPT_DTYPES:
+            raise TypeError(f"HostSlab: a float32, float16 or bfloat16 (H, N, C) tensor expected, got {preds.dtype} "
+                            f"{tuple(preds.shape)}")
+        if not preds.is_contiguous() or preds.shape[1] < 1:
+            raise ValueError("HostSlab: the tensor must be contiguous and hold at least one item")
+        dtype = preds.dtype if dtype is None else dtype
+        if dtype not in (preds.dtype, torch.float32):
+            raise TypeError(f"HostSlab: a {preds.dtype} slab is read as {preds.dtype} or widened to float32, not {dtype}")
+        self.host = preds
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise TypeError("HostSlab: the compute device must be a CUDA device")
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.is_cuda = True
+        self.dtype = dtype
+        H, N, C = (int(s) for s in preds.shape)
+        self.shape = torch.Size([H, N, C])
+        if chunk_items is None:
+            chunk_items = HOST_CHUNK_BYTES // (H * C * self.element_size())
+        a = HOST_CHUNK_ALIGN
+        self.chunk_items = min(max(a, (int(chunk_items) + a - 1) // a * a), (N + a - 1) // a * a)
+
+    def numel(self):
+        return self.shape[0] * self.shape[1] * self.shape[2]
+
+    def element_size(self):
+        return torch.empty(0, dtype=self.dtype).element_size()
+
+    def chunk_bytes(self):
+        """Device bytes of one chunk buffer."""
+        return self.shape[0] * self.chunk_items * self.shape[2] * self.element_size()
+
+    def item_column(self, idx) -> torch.Tensor:
+        """The (H, C) float32 scores of item ``idx`` on the compute device."""
+        idx = int(idx)
+        if not 0 <= idx < self.shape[1]:
+            raise IndexError(f"HostSlab: item {idx} outside [0, {self.shape[1]})")
+        return self.host[:, idx].to(self.device).float()
+
+    def walk(self, body, lo=0, hi=None):
+        """Stream items [lo, hi) through the device: ``body(n0, n1, view)`` enqueues, on the current stream, the kernels
+        that read ``view``, a contiguous (H, n1 - n0, C) device tensor at ``dtype`` holding items [n0, n1).  Each
+        model's range is read from the host tensor through two pinned chunks (``_fill_device``); chunk i + 1 is copied
+        into the second device buffer while the kernels of chunk i run.  Returns when every body's kernels are done."""
+        H, N, C = self.shape
+        hi = N if hi is None else hi
+        step = self.chunk_items
+        nb = min(2, (hi - lo + step - 1) // step)
+        cur = torch.cuda.current_stream(self.device)
+        bufs = [torch.empty(H * min(step, hi - lo) * C, dtype=self.dtype, device=self.device) for _ in range(nb)]
+        used = [None] * nb
+        for i, n0 in enumerate(range(lo, hi, step)):
+            n1, j = min(hi, n0 + step), i % nb
+            if used[j] is not None:
+                used[j].synchronize()                              # the kernels that last read this buffer are done
+            view = bufs[j][: H * (n1 - n0) * C].view(H, n1 - n0, C)
+            _fill_device(self.host, [(view, n0, n1)], self.dtype, DEFAULT_CHUNK_BYTES)
+            body(n0, n1, view)
+            used[j] = torch.cuda.Event()
+            used[j].record(cur)
+        for ev in used:
+            if ev is not None:
+                ev.synchronize()
+
+
+class HostDataset:
+    """``dataset`` wrapper of a ``HostSlab`` for callers that already hold the CPU tensor (``labels`` on the device)."""
+
+    def __init__(self, slab: HostSlab, labels=None):
+        self.preds, self.labels, self.device = slab, labels, slab.device
+        self.n_offset, self.n_global = 0, slab.shape[1]
+
+
+def host_slab_wanted(held_bytes, free_bytes, device_count, env=None):
+    """The shim's rule for a ``HostSlab`` load: ``CODA_B200_HOST_SLAB=1``, or a slab that, at the width it would be
+    held, exceeds the target device's free memory while exactly one GPU is visible (with more, it is split into
+    per-GPU pieces instead).  ``CODA_B200_HOST_SLAB=0`` never loads one."""
+    env = os.environ if env is None else env
+    v = env.get("CODA_B200_HOST_SLAB")
+    if v is not None and v != "":
+        return v == "1"
+    return device_count == 1 and held_bytes > free_bytes
+
+
+def host_load_wanted(filepath, device, keep_dtype=False, env=None):
+    """Whether ``coda.datasets.Dataset`` loads ``filepath`` as a ``HostSlab`` (``host_slab_wanted`` on the slab's bytes
+    at the width it would be held and the target device's free memory)."""
+    env = os.environ if env is None else env
+    if env.get("CODA_B200_HOST_SLAB") not in (None, ""):
+        return host_slab_wanted(0, 0, 0, env)
+    dev = torch.device(device)
+    ngpus = torch.cuda.device_count()
+    if dev.type != "cuda" or ngpus != 1:
+        return False
+    try:
+        full = _open_mmap(filepath)
+    except Exception:                                              # legacy format: keep the plain load
+        return False
+    held = full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep_dtype)).element_size()
+    try:
+        index = dev.index if dev.index is not None else torch.cuda.current_device()
+        free = _free_bytes(index)
+    except RuntimeError:                                           # no usable device: keep the plain load
+        return False
+    return host_slab_wanted(held, free, ngpus, env)
+
+
+def load_host(filepath, device, keep_dtype=False, chunk_items=None):
+    """``filepath``'s (H, N, C) slab as a ``HostSlab`` over its memory map: a 16-bit file is read at its width with
+    ``keep_dtype``, else widened to fp32 on the device chunk by chunk."""
+    full = _open_mmap(filepath)
+    return HostSlab(full, device, dtype=_slab_dtype(full, keep_dtype), chunk_items=chunk_items)
+
+
 def piece_plan(N, nshards, ngpus, home, device_count):
     """[(lo, hi, device index)] of ``nshards`` N-range pieces: the ranges ``shard_range(N, r, nshards)`` and the device
     assignment of ``dist.split_slab`` -- the home device first, consecutive pieces sharing a device when there are more
@@ -406,13 +536,20 @@ class Dataset:
     (``load_sharded``) and never held whole on one device; ``chunk_bytes`` bounds its staging chunks.
 
     A file written by ``CompactSlab.save`` loads as a compact slab, and ``compact_k=K`` compacts a dense file at K as it
-    loads (``load_compact``; a ``ShardedCompactSlab`` with more than one piece)."""
+    loads (``load_compact``; a ``ShardedCompactSlab`` with more than one piece).
+
+    ``host=True`` keeps the slab in host memory as a ``HostSlab`` over the file's memory map, computed on ``device``
+    (``load_host``)."""
 
     def __init__(self, filepath, device, keep_dtype=False, *, shards=None, gpus=None, chunk_bytes=DEFAULT_CHUNK_BYTES,
-                 compact_k=None):
+                 compact_k=None, host=False):
         self.device = device
         if compact_k or is_compact_file(filepath):
             self.preds = load_compact(filepath, device, compact_k, shards=shards, gpus=gpus, chunk_bytes=chunk_bytes)
+        elif host:
+            if shards or gpus:
+                raise NotImplementedError("coda_b200: a host-resident slab runs on one GPU in one shard")
+            self.preds = load_host(filepath, device, keep_dtype)
         elif shards or gpus:
             self.preds = load_sharded(filepath, device, keep_dtype, shards=shards, gpus=gpus, chunk_bytes=chunk_bytes)
         else:

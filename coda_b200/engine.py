@@ -66,6 +66,33 @@ def _ptr(t):
     return t.data_ptr() if t is not None else None
 
 
+class _PinnedHost:
+    """A host tensor page-locked and mapped for the device at its own address (coda_b200_host_register) for as long as
+    this object lives: the host shadow slots of a host-resident slab."""
+
+    def __init__(self, shape, dtype, lib):
+        nbytes = math.prod(shape) * torch.empty(0, dtype=dtype).element_size()
+        try:
+            self.t = torch.empty(shape, dtype=dtype)
+        except RuntimeError as e:
+            raise MemoryError(f"coda_b200: cannot allocate {nbytes} bytes of host memory for the host shadow slots "
+                              f"{tuple(shape)}: {e}") from e
+        self.lib = lib
+        if lib.coda_b200_host_register(self.t.data_ptr(), nbytes) != nat.OK:
+            msg = nat.last_error()
+            self.t = None
+            raise MemoryError(f"coda_b200: cannot page-lock {nbytes} bytes of host memory for the host shadow slots "
+                              f"{tuple(shape)}: {msg}")
+
+    def data_ptr(self):
+        return self.t.data_ptr()
+
+    def __del__(self):
+        if getattr(self, "t", None) is not None:
+            self.lib.coda_b200_host_unregister(self.t.data_ptr())
+            self.t = None
+
+
 def shadow_slots(free: int, reserve: int, slot_bytes: int, want: int, ens: bool, left: int = 1, total: int = 1,
                  ens_slot_bytes: int | None = None):
     """-> (model slots, ensemble slots) of one shard's shadow.  ``free``: device bytes free now; ``total`` shards on
@@ -86,11 +113,13 @@ class Engine:
                  uniform_prior: bool, hyp_w: float = 1.0, mode: str = "incremental", n_offset: int = 0,
                  n_global: int | None = None, world: int = 1, own_stream: bool = False, prefilter_n: int = 0,
                  q: str = "eig"):
-        from .datasets import CompactSlab
+        from .datasets import CompactSlab, HostSlab
         if mode not in MODES:
             raise ValueError(f"mode must be one of {MODES}")
         self.compact = preds if isinstance(preds, CompactSlab) else None
-        if not ((isinstance(preds, torch.Tensor) or self.compact is not None) and preds.is_cuda):
+        # a host-resident slab: streamed through the device for construction, every model in a shadow slot afterwards
+        self.host = preds if isinstance(preds, HostSlab) else None
+        if not ((isinstance(preds, torch.Tensor) or self.compact is not None or self.host is not None) and preds.is_cuda):
             raise RuntimeError("coda_b200: dataset.preds must live on a CUDA (sm_90a) device; "
                                "there is no CPU path in this package")
         H, N, Cc = (int(s) for s in preds.shape)
@@ -100,6 +129,12 @@ class Engine:
             if mode == "recompute_all":
                 raise NotImplementedError("coda_b200: mode='recompute_all' is not offered for a compact slab")
             self.K = self.compact.K
+        elif self.host is not None:
+            if mode == "recompute_all":
+                raise NotImplementedError("coda_b200: mode='recompute_all' re-reads the whole slab every step; it is not "
+                                          "offered for a host-resident slab")
+            if n_offset or (n_global is not None and n_global != N) or world != 1:
+                raise NotImplementedError("coda_b200: a host-resident slab runs as one shard on one GPU")
         else:
             nat.slab_format(preds.dtype)          # float32, float16 or bfloat16, else TypeError
             if preds.dim() != 3:
@@ -112,6 +147,7 @@ class Engine:
         # slab element type: a 16-bit slab is read at its stored width and widened to fp32 in every kernel
         self.fmt = nat.slab_format(preds.dtype) if self.compact is None else nat.SLAB_F32
         self.esz = int(preds.element_size()) if self.compact is None else 4
+        self.kernels = {}                                     # construction kernels that ran (see _record_kernels)
         self.dev = preds.device
         with torch.cuda.device(self.dev):
             nat.require_device()
@@ -121,6 +157,8 @@ class Engine:
         self.H, self.N, self.C = H, N, Cc
         if self.compact is not None:
             self.model_stride = int(self.compact.ids.stride(0)) if H > 1 else N * self.K     # elements of ids / probs
+        elif self.host is not None:
+            self.model_stride = N * Cc                        # the contiguous host tensor
         else:
             self.model_stride = int(preds.stride(0)) if H > 1 else N * Cc
         self.Hp = (H + 31) // 32 * 32
@@ -218,12 +256,14 @@ class Engine:
         self.profile = None
         return out
 
-    def _slab_call(self, name, *args, n=1):
-        """An entry point that reads the slab: the fp32 one, or its ``_x`` twin with the slab's element type."""
+    def _slab_call(self, name, *args, n=1, base=None):
+        """An entry point that reads the slab (or, ``base``, a chunk of it or the host-mode shadow): the fp32 one, or
+        its ``_x`` twin with the slab's element type."""
+        base = _ptr(self.preds) if base is None else base
         if self.fmt == nat.SLAB_F32:
-            self._call(name, _ptr(self.preds), *args, n=n)
+            self._call(name, base, *args, n=n)
         else:
-            self._call(name + "_x", _ptr(self.preds), self.fmt, *args, n=n)
+            self._call(name + "_x", base, self.fmt, *args, n=n)
 
     def _z(self, shape, dtype):
         return torch.zeros(shape, dtype=dtype, device=self.dev)
@@ -279,6 +319,8 @@ class Engine:
         self.jvec = self._z((H,), torch.int32)
         self.terms = self._z((2 + 8 * H + 2,), torch.int64).view(torch.int32)[: 2 + 8 * H]   # 8-byte aligned
         self.step_ctr = self._z((1,), torch.int64)
+        self.host_cols = self._z((1,), torch.int64) if self.host is not None else None   # host columns staged, ever
+        self.n_host, self.host_slots = 0, None
         self.hist_idx = self._z((HIST_CAP,), torch.int64)
         self.hist_q = self._z((HIST_CAP,), torch.float32)
         self.hist_tie = self._z((HIST_CAP,), torch.int32)
@@ -315,9 +357,16 @@ class Engine:
         st.hist_idx, st.hist_q, st.hist_tie, st.hist_cap = _ptr(self.hist_idx), _ptr(self.hist_q), _ptr(self.hist_tie), HIST_CAP
         st.step_ctr = _ptr(self.step_ctr)
         st.flags = _ptr(self.flags)
+        if self.host is not None and self.n_host:
+            st.n_host, st.host_shadow, st.stage = self.n_host, _ptr(self.host_slots), _ptr(self.stage)
+            st.stage_off = (self.stage.data_ptr() - self._slab_ptr()) // self.esz
         self.st = st
 
     def _slab_ptr(self):
+        """Base address of the gather list's slab terms: the slab, or with a host-resident slab the device shadow
+        buffer (model slots, fp32 ensemble slot, staging columns)."""
+        if self.host is not None:
+            return self.dshadow.data_ptr()
         return self.preds.data_ptr() if self.compact is None else 0
 
     def _ens_base(self):
@@ -343,16 +392,41 @@ class Engine:
                            _ptr(self.pseudo), H, N, C, self.K, self.fx_shift, _ptr(self.conf_fx), _ptr(self.conf_rest), s)
                 self._build_compact_index()
                 return
-            self._slab_call("coda_b200_scan_slab", self.model_stride, H, N, C, _ptr(self.hard),
-                            _ptr(self.pseudo), _ptr(self.disagree), _ptr(self.ens), _ptr(self.flags), s)
-            if C <= 128:
-                order = torch.argsort(self.pseudo).to(torch.int32)      # init-time plumbing: any grouping by label will do
-                self._slab_call("coda_b200_confusion_sorted", self.model_stride, _ptr(self.pseudo),
-                                _ptr(order), H, N, C, self.fx_shift, _ptr(self.conf_fx), s)
-                del order
+            self._record_kernels()
+            if self.host is not None:                           # per chunk; the confusion sums are order-free integers
+                self.host.walk(lambda n0, n1, v: self._scan_range(_ptr(v), (n1 - n0) * C, n0, n1 - n0))
             else:
-                self._slab_call("coda_b200_confusion_accum", self.model_stride, _ptr(self.pseudo), H, N, C,
-                                self.fx_shift, _ptr(self.conf_fx), s)
+                self._scan_range(_ptr(self.preds), self.model_stride, 0, N)
+
+    def _scan_range(self, base, model_stride, n0, n):
+        """The slab scan and the confusion sums of items [n0, n0 + n), read from ``base`` (their first item)."""
+        H, C, s = self.H, self.C, self._s()
+        pseudo = _ptr(self.pseudo[n0:])
+        self._slab_call("coda_b200_scan_slab", model_stride, H, n, C, _ptr(self.hard[n0:]), pseudo,
+                        _ptr(self.disagree[n0:]), _ptr(self.ens[n0:]) if self.ens is not None else None,
+                        _ptr(self.flags), s, base=base)
+        if self.kernels["confusion"] == "sorted":
+            order = torch.argsort(self.pseudo[n0:n0 + n]).to(torch.int32)   # init-time plumbing: any grouping by label will do
+            self._slab_call("coda_b200_confusion_sorted", model_stride, pseudo, _ptr(order), H, n, C, self.fx_shift,
+                            _ptr(self.conf_fx), s, base=base)
+            del order
+        else:
+            self._slab_call("coda_b200_confusion_accum", model_stride, pseudo, H, n, C, self.fx_shift,
+                            _ptr(self.conf_fx), s, base=base)
+
+    def _record_kernels(self):
+        """Which construction kernels this dense slab takes, decided from the whole task (H, N, C, dtype, model
+        stride): a host-resident slab, streamed in chunks, takes the kernels the same slab takes on the device.
+        ``scan``: the bulk-TMA scan or the generic one (the rule of csrc/slab.cu scan_slab; chunks are whole multiples
+        of its 32-item tile, so each chunk meets it exactly when the whole slab does); ``pi_full``: the tensor-core
+        marginal pass or the SIMT one; ``confusion``: the pseudo-label-sorted sums or the accumulating ones."""
+        H, N, C, esz = self.H, self.N, self.C, self.esz
+        e16 = 16 // esz
+        aligned = self.host is not None or self.preds.data_ptr() % 16 == 0
+        tma = (C <= 128 and self.model_stride % e16 == 0 and (32 * C) % e16 == 0 and ((N % 32) * C) % e16 == 0
+               and aligned)
+        self.kernels["scan"] = "tma" if tma else "generic"
+        self.kernels["confusion"] = "sorted" if C <= 128 else "accum"
 
     def construct_posterior(self):
         with self._on():
@@ -421,20 +495,23 @@ class Engine:
             self._call("coda_b200_pi_full_compact", _ptr(cs.ids), _ptr(cs.probs), self.model_stride, _ptr(self.D), H, N, C,
                        self.K, _ptr(dt), _ptr(rs), _ptr(self.U), s, n=3)
             del dt, rs
+        elif self.host is not None:
+            self.host.walk(lambda n0, n1, v: self._pi_full(_ptr(v), (n1 - n0) * C, n0, n1 - n0))
         else:
             self._pi_full()
         self._call("coda_b200_pi_reduce", _ptr(self.U), N, C, self.fx_shift, None, _ptr(self.pisum),
                    _ptr(self.flags), s)
 
-    def _pi_full(self):
-        """coda.py:227-229 over the dense slab: the wgmma kernel when the shape allows it (pi_tc.cu), else fp32 SIMT.
-        ``CODA_B200_PI_FULL=simt`` forces the SIMT kernel."""
+    def _pi_full(self, base=None, model_stride=None, n0=0, n=None):
+        """coda.py:227-229 over the dense slab (or items [n0, n0 + n) of it at ``base``): the wgmma kernel when the
+        shape of the whole slab allows it (pi_tc.cu), else fp32 SIMT.  ``CODA_B200_PI_FULL=simt`` forces the SIMT
+        kernel."""
         H, N, C, s = self.H, self.N, self.C, self._s()
         if self._pi_tc is None:
             want = os.environ.get("CODA_B200_PI_FULL", "tc") != "simt"
             if self.fmt == nat.SLAB_F32:
-                self._pi_tc = bool(want and self.lib.coda_b200_pi_full_tc_ok(H, N, C, self.model_stride)
-                                   and self.preds.data_ptr() % 16 == 0)
+                aligned = self.host is not None or self.preds.data_ptr() % 16 == 0
+                self._pi_tc = bool(want and self.lib.coda_b200_pi_full_tc_ok(H, N, C, self.model_stride) and aligned)
             else:
                 # the tensor-core and SIMT passes differ in the last bits: a 16-bit slab takes the pass its fp32
                 # widening (contiguous, aligned) would take, or stops
@@ -446,11 +523,15 @@ class Engine:
                 self._pi_tc = bool(want and tc32)
             if self._pi_tc:
                 self._pi_scratch = self._e((int(self.lib.coda_b200_pi_full_tc_scratch_bytes(H, C)),), torch.uint8)
+            self.kernels["pi_full"] = "tc" if self._pi_tc else "simt"
+        ms = self.model_stride if model_stride is None else model_stride
+        n = N if n is None else n
+        U = _ptr(self.U[n0:])
         if self._pi_tc:
-            self._slab_call("coda_b200_pi_full_tc", self.model_stride, _ptr(self.D), H, N, C, _ptr(self.U),
-                            _ptr(self._pi_scratch), _ptr(self.flags), s, n=2)
+            self._slab_call("coda_b200_pi_full_tc", ms, _ptr(self.D), H, n, C, U, _ptr(self._pi_scratch),
+                            _ptr(self.flags), s, n=2, base=base)
         else:
-            self._slab_call("coda_b200_pi_full", self.model_stride, _ptr(self.D), H, N, C, _ptr(self.U), s)
+            self._slab_call("coda_b200_pi_full", ms, _ptr(self.D), H, n, C, U, s, base=base)
 
     def _build_rows(self):
         H, N, C, W, T, s = self.H, self.N, self.C, self.W, self.T, self._s()
@@ -576,9 +657,17 @@ class Engine:
         (the largest is a U-sized ``pi_hat_xi`` read-out; graph instantiation, lazily loaded kernels, the report and
         history read-outs are small) plus a 1 GiB margin for the caller.  ``CODA_B200_SHADOW_RESERVE_GB`` overrides."""
         env = os.environ.get("CODA_B200_SHADOW_RESERVE_GB")
-        if env is not None:
-            return int(float(env) * 2 ** 30)
-        return 4 * self.N * self.C + (1 << 30)
+        base = int(float(env) * 2 ** 30) if env is not None else 4 * self.N * self.C + (1 << 30)
+        if self.host is not None:
+            # a host-resident slab also keeps, at worst, two staging columns per model, and the shadow pass streams the
+            # slab through two chunk buffers (plus one widening chunk)
+            from .datasets import DEFAULT_CHUNK_BYTES
+            base += 2 * self.H * self._shadow_cs() * self.esz + 2 * self.host.chunk_bytes() + DEFAULT_CHUNK_BYTES
+        return base
+
+    def _shadow_cs(self):
+        """Column stride of the shadow: every (slot, class) column starts 16-byte aligned."""
+        return (self.N + 7) // 8 * 8 if self.esz == 2 else (self.N + 3) // 4 * 4
 
     def _build_shadow(self, left: int = 1, total: int = 1):
         """Class-major shadow copy of the ensemble sums and of as many models as spare HBM allows (least accurate
@@ -587,14 +676,16 @@ class Engine:
         what is free once every shard's reserve is set aside."""
         self.shadow, self.slot_of_model, self.n_shadow, self.shadow_cs = None, None, 0, 0
         self.ens_shadow = None
-        if self.mode == "recompute_all" or os.environ.get("CODA_B200_SHADOW", "1") == "0" or self.compact is not None:
+        host = self.host is not None
+        if not host and (self.mode == "recompute_all" or os.environ.get("CODA_B200_SHADOW", "1") == "0"
+                         or self.compact is not None):
             return
         H, N, C = self.H, self.N, self.C
-        cs = (N + 7) // 8 * 8 if self.esz == 2 else (N + 3) // 4 * 4    # every (slot, class) column starts 16-byte aligned
+        cs = self._shadow_cs()
         cap = os.environ.get("CODA_B200_SHADOW_MODELS")
         want = H if cap is None else max(0, min(H, int(cap)))
         order = None
-        if want > 0:
+        if want > 0 or host:
             # disagreement of every model with the ensemble pseudo-label: the models that will need gathers most often
             dis = torch.zeros(H, dtype=torch.int64, device=self.dev)
             step = max(1, (64 << 20) // max(1, H))
@@ -609,6 +700,9 @@ class Engine:
         # model slots hold the slab's own element type (exact); the ensemble slot is fp32
         S, ne = shadow_slots(free, self.shadow_reserve(), cs * C * self.esz, want, self.ens is not None, left, total,
                              ens_slot_bytes=cs * C * 4)
+        if host:
+            self._build_host_shadow(order, S, ne, cs)
+            return
         if S + ne == 0:
             return
         slot = torch.full((H,), -1, dtype=torch.int32, device=self.dev)
@@ -627,6 +721,42 @@ class Engine:
             first = torch.zeros(1, dtype=torch.int32, device=self.dev)
             self._call("coda_b200_shadow_build", _ptr(self.ens), N * C, 1, N, C, _ptr(first), 1, cs,
                        _ptr(self.ens_shadow), self._s())
+        self.slot_of_model, self.n_shadow, self.shadow_cs = slot, S, cs
+
+    def _build_host_shadow(self, order, S, ne, cs):
+        """A host-resident slab: every model gets a shadow slot.  ``order`` (least accurate first) puts models
+        [0, S) in device slots and the rest in pinned host slots [H - S][C][cs] at the slab's width, mapped for the
+        device; both are transposed from each chunk as the slab streams through.  One device buffer ``dshadow`` holds
+        the device slots, the fp32 ensemble slot (fp32 slab) and the 2 (H - S) staging columns of k_host_stage: it is
+        the base every slab term of the gather list counts from."""
+        H, N, C, esz, s = self.H, self.N, self.C, self.esz, self._s()
+        nh = H - S
+        ne_in = ne if esz == 4 else 0                           # the fp32 ensemble slot shares the buffer
+        self.dshadow = self._e(((S + ne_in) * C * cs + max(1, 2 * nh) * cs,), self.host.dtype)
+        if S + ne_in:
+            self.shadow = self.dshadow[: (S + ne_in) * C * cs].view(S + ne_in, C, cs)
+        if ne:
+            self.ens_shadow = self.shadow[S] if ne_in else self._e((C, cs), torch.float32)
+        self.stage = self.dshadow[(S + ne_in) * C * cs:]
+        self.host_slots = _PinnedHost((nh, C, cs), self.host.dtype, self.lib) if nh else None
+        self.n_host = nh
+        slot = torch.empty((H,), dtype=torch.int32, device=self.dev)
+        slot[order.long()] = torch.arange(H, dtype=torch.int32, device=self.dev)
+        dev_order, host_order = order[:S].contiguous(), order[S:].contiguous()
+
+        def body(n0, n1, v):
+            n = n1 - n0
+            if S:
+                self._slab_call("coda_b200_shadow_build", n * C, H, n, C, _ptr(dev_order), S, cs,
+                                _ptr(self.shadow) + n0 * esz, s, base=_ptr(v))
+            if nh:                                              # written straight into the mapped host slots
+                self._slab_call("coda_b200_shadow_build", n * C, H, n, C, _ptr(host_order), nh, cs,
+                                _ptr(self.host_slots) + n0 * esz, s, base=_ptr(v))
+        self.host.walk(body)
+        if ne:
+            first = torch.zeros(1, dtype=torch.int32, device=self.dev)
+            self._call("coda_b200_shadow_build", _ptr(self.ens), N * C, 1, N, C, _ptr(first), 1, cs,
+                       _ptr(self.ens_shadow), s)
         self.slot_of_model, self.n_shadow, self.shadow_cs = slot, S, cs
 
     # ------------------------------------------------------------------------ step pieces (enqueue only)
@@ -793,10 +923,14 @@ class Engine:
                        C, self.K, _ptr(self.sel), self.lr, self.fx_shift, _ptr(self.terms), _ptr(self.U),
                        _ptr(self.pisum), _ptr(self.flags), s)
         else:
+            base = None
+            if self.host is not None:                           # host-slot columns -> staging columns, terms rewritten
+                self._call("coda_b200_host_stage", self.st, self.fmt, _ptr(self.host_cols), s, n=2)
+                base = self._slab_ptr()
             ens = _ptr(self.ens) if self.fmt == nat.SLAB_F32 else self._ens_base()
             self._slab_call("coda_b200_pi_rank1", ens, H, N, C, _ptr(self.sel), self.lr,
                             self.fx_shift, _ptr(self.terms), _ptr(self.U), _ptr(self.pisum), _ptr(self.flags),
-                            4 if fork else 8, self.const_slot, s)
+                            4 if fork else 8, self.const_slot, s, base=base)
         if fork:
             main.wait_event(self.ev_tables)     # the mixture needs PB[t]; the rows are awaited by the scoring pass
             self.pending = True
@@ -1236,7 +1370,8 @@ class Engine:
             self._mailbox.close()
             self._mailbox = None
         for k, v in list(self.__dict__.items()):
-            if isinstance(v, torch.Tensor) or k in ("preds", "compact", "st", "xchg", "_labels_keep", "cidx"):
+            if isinstance(v, torch.Tensor) or k in ("preds", "compact", "host", "host_slots", "st", "xchg", "_labels_keep",
+                                                    "cidx"):
                 setattr(self, k, None)
 
 

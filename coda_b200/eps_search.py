@@ -106,12 +106,12 @@ def modelpicker_eps_search(dataset, epsilons=DEFAULT_EPSILONS, iterations=1000, 
     from .baselines import _DeviceState, _ptr
     from .dist import default_comm
     eps = _check_epsilons(epsilons)
-    from .datasets import ShardedCompactSlab, ShardedSlab
+    from .datasets import HostSlab, ShardedCompactSlab, ShardedSlab
     preds = getattr(dataset, "preds", None)
-    if isinstance(preds, (ShardedSlab, ShardedCompactSlab)):
+    if isinstance(preds, (ShardedSlab, ShardedCompactSlab, HostSlab)):
         raise NotImplementedError(f"modelpicker_eps_search: runs on one GPU over one (H, N, C) tensor; a "
-                                  f"{type(preds).__name__} (a slab loaded as N-range pieces) is not supported -- load "
-                                  f"the task unsharded")
+                                  f"{type(preds).__name__} (a slab loaded as N-range pieces or kept in host memory) is "
+                                  f"not supported -- load the task as one device tensor")
     if preds is None or len(preds.shape) != 3:
         raise TypeError("modelpicker_eps_search: dataset.preds must be an (H, N, C) slab")
     H, N, C = (int(s) for s in preds.shape)

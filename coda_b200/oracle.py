@@ -16,8 +16,8 @@ class Oracle:
     def true_losses(self, preds):
         """Mean loss of every model, (H,) (coda/oracle.py:9-21).  A ``ShardedSlab``, ``CompactSlab`` or
         ``ShardedCompactSlab`` takes the accuracy loss only, on the pieces' devices (``sharded_true_losses``)."""
-        from .datasets import CompactSlab, ShardedCompactSlab, ShardedSlab
-        if isinstance(preds, (ShardedSlab, CompactSlab, ShardedCompactSlab)):
+        from .datasets import CompactSlab, HostSlab, ShardedCompactSlab, ShardedSlab
+        if isinstance(preds, (ShardedSlab, CompactSlab, ShardedCompactSlab, HostSlab)):
             return sharded_true_losses(preds, self.labels, self.loss_fn, self.dataset.device)
         H, N, C = preds.shape
         return self.loss_fn(preds.reshape(-1, C), self.labels.repeat(H), reduction="none").view(H, N).mean(dim=1)
@@ -42,9 +42,11 @@ def sharded_true_losses(slab, labels, loss_fn, device):
     every selector sees -- is the label (``coda_b200_true_loss_counts_compact``).  For a slab compacted from a dense one
     (``CompactSlab.from_dense``, ``load_compact``) ``ids[0]`` is the dense arg-max, so the result has the bits of
     ``true_losses`` on the dense slab.  It can differ from ``true_losses(slab.densify())`` only in the rows counted in
-    ``compaction["flat_rows"]``, where the uniform remainder reaches ``probs[0]``."""
+    ``compaction["flat_rows"]``, where the uniform remainder reaches ``probs[0]``.
+
+    A ``HostSlab`` is counted chunk by chunk as it streams through its device (``HostSlab.walk``)."""
     from . import _native as nat
-    from .datasets import CompactSlab
+    from .datasets import CompactSlab, HostSlab
     name = type(slab).__name__
     try:
         from coda.options import accuracy_loss                # what LOSS_FNS["acc"] resolves to
@@ -63,6 +65,23 @@ def sharded_true_losses(slab, labels, loss_fn, device):
         raise NotImplementedError(f"coda_b200: the pieces of a {name} must be CUDA tensors; there is no CPU path")
     lib = nat.load()
     labels = labels.to(torch.int64)
+    if isinstance(slab, HostSlab):
+        dev = slab.device
+        with torch.cuda.device(dev):
+            lab = labels.to(dev)
+            correct = torch.zeros(H, dtype=torch.int64, device=dev)
+
+            def body(n0, n1, v):
+                cnt = torch.zeros(H, dtype=torch.int64, device=dev)
+                nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(v.data_ptr()), nat.slab_format(v.dtype),
+                                                         (n1 - n0) * C, H, n1 - n0, C, ct.c_void_p(lab[n0:].data_ptr()),
+                                                         ct.c_void_p(cnt.data_ptr()),
+                                                         ct.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                          "true_loss_counts")
+                correct.add_(cnt)
+            slab.walk(body)
+        wrong = (N - correct.to(device)).to(torch.float32)
+        return wrong * torch.tensor(mean_factor(H, N), device=device)
     parts = []
     for piece, off in (slab.layout() if hasattr(slab, "layout") else [(slab, 0)]):
         dev = piece.device

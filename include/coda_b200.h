@@ -335,6 +335,13 @@ typedef struct coda_step { /* host struct: this shard's device state */
   int64_t hist_cap;
   int64_t* step_ctr; /* [1] */
   uint32_t* flags;
+  /* host-resident slab (HostSlab): every model has a shadow slot; slots [H - n_host, H) live in pinned host memory.
+   * The step kernels emit a host slot's term as {element offset into host_shadow, sign, item stride 0}, which only
+   * coda_b200_host_stage resolves.  n_host = 0: no host slots (every other field below is ignored). */
+  int64_t n_host;
+  const void* host_shadow; /* device-visible address of the pinned slots [n_host][C][shadow_col_stride] */
+  void* stage;             /* device staging columns [2 * n_host][shadow_col_stride], slab element type */
+  int64_t stage_off;       /* element offset of `stage` relative to the slab base pointer pi_rank1 is given */
 } coda_step_t;
 
 /* coda.py:306/309 + oracle(idx) + coda.py:316-317 with no host in the loop: merge the block records, exchange
@@ -342,6 +349,16 @@ typedef struct coda_step { /* host struct: this shard's device state */
  * is recorded in hist_tie), look the label up in labels_global, mark the item labeled, D[h][t][p_h(idx)] += lr,
  * build the rank-1 gather list, zero pisum. */
 int coda_b200_step_select(const coda_step_t* st, const coda_xchg_t* x, coda_stream_t stream);
+/* Host-resident slab: after step_select / step_label and before pi_rank1, copy the host-slot column of every term
+ * the step kernel left unresolved (item stride 0) from mapped pinned memory into the next free staging column (cs
+ * slab elements at the width `fmt`), and point the term there (offset stage_off + k * cs, item stride 1).  Term
+ * count, order and signs are unchanged; every other term is untouched.  census (optional, device): += host columns
+ * staged.  A fixed grid reads the term count on the device (graph-capturable); no-op when st->n_host == 0. */
+int coda_b200_host_stage(const coda_step_t* st, int fmt, int64_t* census, coda_stream_t stream);
+/* Page-lock `bytes` of an existing host allocation and map them for every device at the same address (the host
+ * slots of a HostSlab); fails when the device address would differ.  unregister undoes it. */
+int coda_b200_host_register(void* ptr, size_t bytes);
+int coda_b200_host_unregister(void* ptr);
 /* API path, get_next_item_to_label: merge + exchange only -> bestrec. */
 int coda_b200_step_merge(const coda_step_t* st, const coda_xchg_t* x, coda_stream_t stream);
 /* API path, add_label (coda.py:315-317): sel = {local idx or -1, class} given; the owner shares p_h(idx). */

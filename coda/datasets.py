@@ -1,7 +1,8 @@
 import os
 
 from coda_b200.datasets import Dataset as _Dataset
-from coda_b200.datasets import compact_load_count, host_load_wanted, is_compact_file, shard_load_count
+from coda_b200.datasets import (compact_load_count, host_load_wanted, host_piece_count, is_compact_file,
+                                shard_load_count)
 
 
 class Dataset(_Dataset):
@@ -17,7 +18,10 @@ class Dataset(_Dataset):
 
     ``CODA_B200_HOST_SLAB=1``, or a dense slab larger than the target device's free memory with exactly one GPU
     visible, keeps it in host memory (``coda_b200.datasets.HostSlab``) and runs it exactly on that GPU;
-    ``CODA_B200_HOST_SLAB=0`` never does.  Compact files and ``CODA_B200_COMPACT_K`` take precedence."""
+    ``CODA_B200_HOST_SLAB=0`` never does.  With more than one GPU visible and neither ``CODA_B200_HOST_SLAB`` nor
+    ``CODA_B200_SHARD_LOAD`` set, a dense slab larger than the summed free memory of the GPUs its pieces would use stays
+    in host memory as N-range pieces, one per GPU (``coda_b200.datasets.ShardedHostSlab``; ``CODA_B200_GPUS`` pieces,
+    else one per visible GPU).  Compact files and ``CODA_B200_COMPACT_K`` take precedence."""
 
     def __init__(self, filepath, device):
         keep = os.environ.get("CODA_B200_KEEP_DTYPE", "0") == "1"
@@ -29,6 +33,10 @@ class Dataset(_Dataset):
             return
         if host_load_wanted(filepath, device, keep):
             super().__init__(filepath, device, keep_dtype=keep, host=True)
+            return
+        shards = host_piece_count(filepath, device, keep)
+        if shards:
+            super().__init__(filepath, device, keep_dtype=keep, host=True, shards=shards)
             return
         shards = shard_load_count(filepath, device, keep)
         if shards:

@@ -8,12 +8,12 @@ _os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
 from .base import ModelSelector
 from .datasets import (CompactDataset, CompactSlab, Dataset, HostDataset, HostSlab, ShardedCompactSlab,
-                       ShardedFileDataset, ShardedSlab, SyntheticCompactDataset, SyntheticDataset, TensorDataset,
-                       load_compact)
+                       ShardedFileDataset, ShardedHostSlab, ShardedSlab, SyntheticCompactDataset, SyntheticDataset,
+                       TensorDataset, load_compact)
 from .oracle import Oracle
 from .selector import CODA
 from .baselines import IID, VMA, ActiveTesting, ModelPicker, Uncertainty
 
 __all__ = ["CODA", "Dataset", "Oracle", "ModelSelector", "TensorDataset", "SyntheticDataset", "ShardedFileDataset",
            "ShardedSlab", "CompactSlab", "ShardedCompactSlab", "load_compact", "CompactDataset", "SyntheticCompactDataset",
-           "HostSlab", "HostDataset", "IID", "Uncertainty", "ActiveTesting", "VMA", "ModelPicker"]
+           "HostSlab", "ShardedHostSlab", "HostDataset", "IID", "Uncertainty", "ActiveTesting", "VMA", "ModelPicker"]

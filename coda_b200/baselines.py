@@ -548,13 +548,13 @@ def _check_rank_ranges(preds, n_offset, N, n_global, comm):
 
 def _layout(dataset, gpus, shards, comm):
     """-> (group, [(shard slab, n_offset)] of this process)."""
-    from .datasets import CompactSlab, HostSlab, ShardedCompactSlab, ShardedSlab
+    from .datasets import CompactSlab, HostSlab, ShardedCompactSlab, ShardedHostSlab, ShardedSlab
     from .selector import host_slab_refusals
     preds = getattr(dataset, "preds", None)
     if isinstance(preds, HostSlab):                             # one shard on the slab's compute device
         host_slab_refusals(gpus, shards, comm.world)
         return SoloGroup(), [(preds, 0)]
-    if isinstance(preds, (ShardedSlab, ShardedCompactSlab)):    # the pieces are the shards
+    if isinstance(preds, (ShardedSlab, ShardedCompactSlab, ShardedHostSlab)):    # the pieces are the shards
         layout = piece_layout(preds, gpus, shards, comm.world)
         if not preds.is_cuda:
             raise NotImplementedError(_NO_CPU)

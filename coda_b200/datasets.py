@@ -76,11 +76,12 @@ HOST_CHUNK_ALIGN = 32           # items: a multiple of the slab scan's tile, so 
 
 class HostSlab:
     """An (H, N, C) slab kept in host memory -- a contiguous CPU tensor, possibly memory-mapped from a ``torch.save``
-    file -- for one compute ``device``: a task larger than one GPU, run exactly on that GPU.  CODA, the competing
-    selectors and ``Oracle.true_losses`` stream it through the device in N-range chunks of ``chunk_items`` items (two
-    device buffers of one chunk each); the slab is never copied whole to the device.  Duck-types ``ShardedSlab``'s
-    surface: ``shape``, ``dtype`` (the width the kernels read: the tensor's, or float32 to widen a 16-bit tensor on
-    the device), ``device``, ``numel``, ``element_size``, ``item_column``."""
+    file, or an N-range view of one (each model's items one contiguous range) -- for one compute ``device``: a task
+    larger than one GPU, run exactly on that GPU.  CODA, the competing selectors and ``Oracle.true_losses`` stream it
+    through the device in N-range chunks of ``chunk_items`` items (two device buffers of one chunk each); the slab is
+    never copied whole to the device.  Duck-types ``ShardedSlab``'s surface: ``shape``, ``dtype`` (the width the
+    kernels read: the tensor's, or float32 to widen a 16-bit tensor on the device), ``device``, ``numel``,
+    ``element_size``, ``item_column``."""
 
     def __init__(self, preds: torch.Tensor, device, dtype=None, chunk_items=None):
         if not isinstance(preds, torch.Tensor) or preds.device.type != "cpu":
@@ -88,8 +89,10 @@ class HostSlab:
         if preds.dim() != 3 or preds.dtype not in _KEPT_DTYPES:
             raise TypeError(f"HostSlab: a float32, float16 or bfloat16 (H, N, C) tensor expected, got {preds.dtype} "
                             f"{tuple(preds.shape)}")
-        if not preds.is_contiguous() or preds.shape[1] < 1:
-            raise ValueError("HostSlab: the tensor must be contiguous and hold at least one item")
+        H, N, C = (int(s) for s in preds.shape)
+        if N < 1 or not (preds.stride(2) == 1 and preds.stride(1) == C and (H == 1 or preds.stride(0) >= N * C)):
+            raise ValueError("HostSlab: the tensor must hold at least one item, with contiguous items (a contiguous "
+                             "tensor or an N-range view of one)")
         dtype = preds.dtype if dtype is None else dtype
         if dtype not in (preds.dtype, torch.float32):
             raise TypeError(f"HostSlab: a {preds.dtype} slab is read as {preds.dtype} or widened to float32, not {dtype}")
@@ -101,7 +104,6 @@ class HostSlab:
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.is_cuda = True
         self.dtype = dtype
-        H, N, C = (int(s) for s in preds.shape)
         self.shape = torch.Size([H, N, C])
         if chunk_items is None:
             chunk_items = HOST_CHUNK_BYTES // (H * C * self.element_size())
@@ -159,6 +161,53 @@ class HostDataset:
         self.n_offset, self.n_global = 0, slab.shape[1]
 
 
+class ShardedHostSlab:
+    """An (H, N, C) slab kept in host memory as contiguous N-range pieces, one ``HostSlab`` per piece, each computed on
+    its own device (consecutive pieces may share one): the host-resident twin of ``ShardedSlab``, with its surface and
+    its rules.  The pieces ARE the shard layout: CODA and the competing selectors run one host-resident shard per piece,
+    each streaming its piece through its own device and staging its own host columns each step, and give the bits of
+    the whole slab.  ``device`` is the first piece's."""
+
+    def __init__(self, pieces):
+        pieces = list(pieces)
+        if not pieces:
+            raise ValueError("ShardedHostSlab: at least one piece expected")
+        for p in pieces:
+            if not isinstance(p, HostSlab):
+                raise TypeError("ShardedHostSlab: pieces must be HostSlab (device pieces make a ShardedSlab)")
+        H, _, C = pieces[0].shape
+        if any(p.shape[0] != H or p.shape[2] != C or p.dtype != pieces[0].dtype for p in pieces):
+            raise TypeError("ShardedHostSlab: all pieces must share one dtype, H and C")
+        self.pieces = pieces
+        self.offsets = []
+        n = 0
+        for p in pieces:
+            self.offsets.append(n)
+            n += int(p.shape[1])
+        self.shape = torch.Size([int(H), n, int(C)])
+        self.device = pieces[0].device
+        self.dtype = pieces[0].dtype
+        self.is_cuda = True
+
+    def layout(self):
+        """[(piece, n_offset)]: the shard layout selectors build from."""
+        return list(zip(self.pieces, self.offsets))
+
+    def numel(self):
+        return self.shape[0] * self.shape[1] * self.shape[2]
+
+    def element_size(self):
+        return self.pieces[0].element_size()
+
+    def item_column(self, idx) -> torch.Tensor:
+        """The (H, C) float32 scores of item ``idx``, on the compute device of the piece that holds it."""
+        idx = int(idx)
+        if not 0 <= idx < self.shape[1]:
+            raise IndexError(f"ShardedHostSlab: item {idx} outside [0, {self.shape[1]})")
+        r = max(i for i, off in enumerate(self.offsets) if off <= idx)
+        return self.pieces[r].item_column(idx - self.offsets[r])
+
+
 def host_slab_wanted(held_bytes, free_bytes, device_count, env=None):
     """The shim's rule for a ``HostSlab`` load: ``CODA_B200_HOST_SLAB=1``, or a slab that, at the width it would be
     held, exceeds the target device's free memory while exactly one GPU is visible (with more, it is split into
@@ -193,11 +242,44 @@ def host_load_wanted(filepath, device, keep_dtype=False, env=None):
     return host_slab_wanted(held, free, ngpus, env)
 
 
-def load_host(filepath, device, keep_dtype=False, chunk_items=None):
+def host_piece_count(filepath, device, keep_dtype=False, env=None):
+    """How many host-resident pieces (``ShardedHostSlab``) ``coda.datasets.Dataset`` loads ``filepath`` into: 0 for
+    none.  With more than one GPU visible and neither ``CODA_B200_HOST_SLAB`` nor ``CODA_B200_SHARD_LOAD`` set, a slab
+    that, at the width it would be held, exceeds the summed free memory of the devices its pieces would use (a shared
+    device counted once) stays in host memory in ``CODA_B200_GPUS`` pieces, else one per visible GPU."""
+    env = os.environ if env is None else env
+    if env.get("CODA_B200_HOST_SLAB") or env.get("CODA_B200_SHARD_LOAD"):
+        return 0
+    dev = torch.device(device)
+    ngpus = torch.cuda.device_count()
+    if dev.type != "cuda" or ngpus < 2:
+        return 0
+    try:
+        full = _open_mmap(filepath)
+    except Exception:                                              # legacy format: keep the plain load
+        return 0
+    held = full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep_dtype)).element_size()
+    count = max(1, int(env["CODA_B200_GPUS"])) if env.get("CODA_B200_GPUS") else ngpus
+    try:
+        plan = _load_plan(int(full.shape[1]), dev, count, None)
+        free = sum(_free_bytes(d) for d in {d for _, _, d in plan})
+    except RuntimeError:                                           # no usable device: keep the plain load
+        return 0
+    return count if held > free else 0
+
+
+def load_host(filepath, device, keep_dtype=False, chunk_items=None, *, shards=None, gpus=None):
     """``filepath``'s (H, N, C) slab as a ``HostSlab`` over its memory map: a 16-bit file is read at its width with
-    ``keep_dtype``, else widened to fp32 on the device chunk by chunk."""
+    ``keep_dtype``, else widened to fp32 on the device chunk by chunk.  With ``shards=`` / ``gpus=``, a
+    ``ShardedHostSlab`` of N-range views of that one memory map, with the ranges and devices of ``load_sharded``:
+    nothing is copied on the host, and each piece streams through its own device."""
     full = _open_mmap(filepath)
-    return HostSlab(full, device, dtype=_slab_dtype(full, keep_dtype), chunk_items=chunk_items)
+    dtype = _slab_dtype(full, keep_dtype)
+    if not (shards or gpus):
+        return HostSlab(full, device, dtype=dtype, chunk_items=chunk_items)
+    plan = _load_plan(int(full.shape[1]), torch.device(device), shards, gpus)
+    return ShardedHostSlab([HostSlab(full[:, lo:hi], torch.device("cuda", d), dtype=dtype, chunk_items=chunk_items)
+                            for lo, hi, d in plan])
 
 
 def piece_plan(N, nshards, ngpus, home, device_count):
@@ -207,6 +289,16 @@ def piece_plan(N, nshards, ngpus, home, device_count):
     devs = [home] + [d for d in range(device_count) if d != home]
     devs = devs[:max(1, ngpus)]
     return [(*shard_range(N, r, nshards), devs[r * len(devs) // nshards]) for r in range(nshards)]
+
+
+def _load_plan(N, device, shards, gpus):
+    """``piece_plan`` of a load into ``shards`` pieces (else ``gpus``) over ``gpus`` devices (else as many as there are
+    pieces, up to the visible GPUs), the first on ``device``."""
+    nshards = int(shards) if shards else int(gpus)
+    ngpus = int(gpus) if gpus else min(nshards, max(1, torch.cuda.device_count()))
+    nshards = max(1, min(nshards, N))
+    home = device.index if device.index is not None else torch.cuda.current_device()
+    return piece_plan(N, nshards, ngpus, home, torch.cuda.device_count())
 
 
 def chunk_walk(lo, hi, C, esz, chunk_bytes):
@@ -240,7 +332,8 @@ def _open_mmap(filepath):
 
 def _fill_device(full, todo, dtype, chunk_bytes):
     """Fill the pieces ``todo`` = [(piece, lo, hi)] of one device model by model: each model's range is one contiguous
-    read of the file, staged through two pinned chunks; a 16-bit file read into fp32 pieces is widened on the device."""
+    read of the file, staged through two pinned chunks; a 16-bit file read into fp32 pieces is widened on the device.
+    ``full`` is an (H, N, C) tensor with contiguous items: the file, or an N-range view of it."""
     dev = todo[0][0].device
     H, _, C = full.shape
     src_t = full.dtype
@@ -251,18 +344,18 @@ def _fill_device(full, todo, dtype, chunk_bytes):
     with torch.cuda.device(dev):
         stream = torch.cuda.Stream(device=dev)
         stage = torch.empty(step, dtype=src_t, device=dev) if src_t != dtype else None
-        flat = full.view(H, -1)
         k = 0
         with torch.cuda.stream(stream):
             for piece, lo, hi in todo:
                 dst = piece.view(H, -1)
                 for h in range(H):
+                    src = full[h].view(-1)                      # one model's items: contiguous
                     for a, b in chunk_walk(lo, hi, C, esz, chunk_bytes):
                         j = k % 2
                         if done[j] is not None:
                             done[j].synchronize()             # the copy that last read this pinned chunk is over
                         n = b - a
-                        pins[j][:n].copy_(flat[h, a:b])
+                        pins[j][:n].copy_(src[a:b])
                         out = dst[h, a - lo * C:b - lo * C]
                         if stage is None:
                             out.copy_(pins[j][:n], non_blocking=True)
@@ -284,12 +377,7 @@ def load_sharded(filepath, device, keep_dtype=False, shards=None, gpus=None, chu
     full = _open_mmap(filepath)
     H, N, C = (int(s) for s in full.shape)
     dtype = _slab_dtype(full, keep_dtype)
-    nshards = int(shards) if shards else int(gpus)
-    ngpus = int(gpus) if gpus else min(nshards, max(1, torch.cuda.device_count()))
-    nshards = max(1, min(nshards, N))
-    dev = torch.device(device)
-    home = dev.index if dev.index is not None else torch.cuda.current_device()
-    plan = piece_plan(N, nshards, ngpus, home, torch.cuda.device_count())
+    plan = _load_plan(N, torch.device(device), shards, gpus)
     pieces, by_dev = [], {}
     for lo, hi, d in plan:
         p = torch.empty((H, hi - lo, C), dtype=dtype, device=torch.device("cuda", d))
@@ -539,7 +627,8 @@ class Dataset:
     loads (``load_compact``; a ``ShardedCompactSlab`` with more than one piece).
 
     ``host=True`` keeps the slab in host memory as a ``HostSlab`` over the file's memory map, computed on ``device``
-    (``load_host``)."""
+    (``load_host``); with ``shards=`` / ``gpus=`` as well, as a ``ShardedHostSlab`` of N-range pieces of that memory
+    map, each computed on its own device."""
 
     def __init__(self, filepath, device, keep_dtype=False, *, shards=None, gpus=None, chunk_bytes=DEFAULT_CHUNK_BYTES,
                  compact_k=None, host=False):
@@ -547,9 +636,7 @@ class Dataset:
         if compact_k or is_compact_file(filepath):
             self.preds = load_compact(filepath, device, compact_k, shards=shards, gpus=gpus, chunk_bytes=chunk_bytes)
         elif host:
-            if shards or gpus:
-                raise NotImplementedError("coda_b200: a host-resident slab runs on one GPU in one shard")
-            self.preds = load_host(filepath, device, keep_dtype)
+            self.preds = load_host(filepath, device, keep_dtype, shards=shards, gpus=gpus)
         elif shards or gpus:
             self.preds = load_sharded(filepath, device, keep_dtype, shards=shards, gpus=gpus, chunk_bytes=chunk_bytes)
         else:

@@ -150,20 +150,21 @@ class Mailbox:
 
 
 def piece_layout(slab, gpus, shards, world):
-    """A ``ShardedSlab`` is its own shard layout: [(piece, n_offset)], used in place (no peer copy, no re-split, and
-    ``CODA_B200_GPUS`` is not consulted).  ``shards=`` (or ``gpus=`` alone) must equal the piece count, ``gpus=`` with
-    ``shards=`` the number of devices the pieces are on."""
+    """A ``ShardedSlab`` (``ShardedCompactSlab``, ``ShardedHostSlab``) is its own shard layout: [(piece, n_offset)],
+    used in place (no peer copy, no re-split, and ``CODA_B200_GPUS`` is not consulted).  ``shards=`` (or ``gpus=``
+    alone) must equal the piece count, ``gpus=`` with ``shards=`` the number of devices the pieces are on."""
+    name = type(slab).__name__
     if world > 1:
-        raise ValueError("coda_b200: a ShardedSlab holds the whole task in one process; under torch.distributed with "
+        raise ValueError(f"coda_b200: a {name} holds the whole task in one process; under torch.distributed with "
                          "world > 1 every rank passes its own N-range tensor (e.g. ShardedFileDataset)")
     k = len(slab.pieces)
     want = shards or gpus
     if want and int(want) != k:
-        raise ValueError(f"coda_b200: the ShardedSlab has {k} pieces, one shard each; "
+        raise ValueError(f"coda_b200: the {name} has {k} pieces, one shard each; "
                          f"{'shards' if shards else 'gpus'}={want} disagrees")
     ndev = len({p.device for p in slab.pieces})
     if shards and gpus and int(gpus) != ndev:
-        raise ValueError(f"coda_b200: the ShardedSlab's pieces are on {ndev} devices; gpus={gpus} disagrees")
+        raise ValueError(f"coda_b200: the {name}'s pieces are on {ndev} devices; gpus={gpus} disagrees")
     return slab.layout()
 
 

@@ -133,8 +133,6 @@ class Engine:
             if mode == "recompute_all":
                 raise NotImplementedError("coda_b200: mode='recompute_all' re-reads the whole slab every step; it is not "
                                           "offered for a host-resident slab")
-            if n_offset or (n_global is not None and n_global != N) or world != 1:
-                raise NotImplementedError("coda_b200: a host-resident slab runs as one shard on one GPU")
         else:
             nat.slab_format(preds.dtype)          # float32, float16 or bfloat16, else TypeError
             if preds.dim() != 3:
@@ -158,7 +156,7 @@ class Engine:
         if self.compact is not None:
             self.model_stride = int(self.compact.ids.stride(0)) if H > 1 else N * self.K     # elements of ids / probs
         elif self.host is not None:
-            self.model_stride = N * Cc                        # the contiguous host tensor
+            self.model_stride = N * Cc                        # each chunk the slab streams through is contiguous
         else:
             self.model_stride = int(preds.stride(0)) if H > 1 else N * Cc
         self.Hp = (H + 31) // 32 * 32

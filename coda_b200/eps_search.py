@@ -106,9 +106,9 @@ def modelpicker_eps_search(dataset, epsilons=DEFAULT_EPSILONS, iterations=1000, 
     from .baselines import _DeviceState, _ptr
     from .dist import default_comm
     eps = _check_epsilons(epsilons)
-    from .datasets import HostSlab, ShardedCompactSlab, ShardedSlab
+    from .datasets import HostSlab, ShardedCompactSlab, ShardedHostSlab, ShardedSlab
     preds = getattr(dataset, "preds", None)
-    if isinstance(preds, (ShardedSlab, ShardedCompactSlab, HostSlab)):
+    if isinstance(preds, (ShardedSlab, ShardedCompactSlab, HostSlab, ShardedHostSlab)):
         raise NotImplementedError(f"modelpicker_eps_search: runs on one GPU over one (H, N, C) tensor; a "
                                   f"{type(preds).__name__} (a slab loaded as N-range pieces or kept in host memory) is "
                                   f"not supported -- load the task as one device tensor")

@@ -16,8 +16,8 @@ class Oracle:
     def true_losses(self, preds):
         """Mean loss of every model, (H,) (coda/oracle.py:9-21).  A ``ShardedSlab``, ``CompactSlab`` or
         ``ShardedCompactSlab`` takes the accuracy loss only, on the pieces' devices (``sharded_true_losses``)."""
-        from .datasets import CompactSlab, HostSlab, ShardedCompactSlab, ShardedSlab
-        if isinstance(preds, (ShardedSlab, CompactSlab, ShardedCompactSlab, HostSlab)):
+        from .datasets import CompactSlab, HostSlab, ShardedCompactSlab, ShardedHostSlab, ShardedSlab
+        if isinstance(preds, (ShardedSlab, CompactSlab, ShardedCompactSlab, HostSlab, ShardedHostSlab)):
             return sharded_true_losses(preds, self.labels, self.loss_fn, self.dataset.device)
         H, N, C = preds.shape
         return self.loss_fn(preds.reshape(-1, C), self.labels.repeat(H), reduction="none").view(H, N).mean(dim=1)
@@ -44,9 +44,10 @@ def sharded_true_losses(slab, labels, loss_fn, device):
     ``true_losses`` on the dense slab.  It can differ from ``true_losses(slab.densify())`` only in the rows counted in
     ``compaction["flat_rows"]``, where the uniform remainder reaches ``probs[0]``.
 
-    A ``HostSlab`` is counted chunk by chunk as it streams through its device (``HostSlab.walk``)."""
+    A ``HostSlab`` is counted chunk by chunk as it streams through its device (``HostSlab.walk``); a
+    ``ShardedHostSlab`` piece by piece, each through its own device."""
     from . import _native as nat
-    from .datasets import CompactSlab, HostSlab
+    from .datasets import CompactSlab, HostSlab, ShardedHostSlab
     name = type(slab).__name__
     try:
         from coda.options import accuracy_loss                # what LOSS_FNS["acc"] resolves to
@@ -65,22 +66,26 @@ def sharded_true_losses(slab, labels, loss_fn, device):
         raise NotImplementedError(f"coda_b200: the pieces of a {name} must be CUDA tensors; there is no CPU path")
     lib = nat.load()
     labels = labels.to(torch.int64)
-    if isinstance(slab, HostSlab):
-        dev = slab.device
-        with torch.cuda.device(dev):
-            lab = labels.to(dev)
-            correct = torch.zeros(H, dtype=torch.int64, device=dev)
+    if isinstance(slab, (HostSlab, ShardedHostSlab)):
+        correct = torch.zeros(H, dtype=torch.int64, device=device)
+        for piece, off in (slab.layout() if isinstance(slab, ShardedHostSlab) else [(slab, 0)]):
+            dev = piece.device
+            with torch.cuda.device(dev):
+                lab = labels[off:off + int(piece.shape[1])].to(dev)
+                part = torch.zeros(H, dtype=torch.int64, device=dev)
 
-            def body(n0, n1, v):
-                cnt = torch.zeros(H, dtype=torch.int64, device=dev)
-                nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(v.data_ptr()), nat.slab_format(v.dtype),
-                                                         (n1 - n0) * C, H, n1 - n0, C, ct.c_void_p(lab[n0:].data_ptr()),
-                                                         ct.c_void_p(cnt.data_ptr()),
-                                                         ct.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-                          "true_loss_counts")
-                correct.add_(cnt)
-            slab.walk(body)
-        wrong = (N - correct.to(device)).to(torch.float32)
+                def body(n0, n1, v):
+                    cnt = torch.zeros(H, dtype=torch.int64, device=dev)
+                    nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(v.data_ptr()), nat.slab_format(v.dtype),
+                                                             (n1 - n0) * C, H, n1 - n0, C,
+                                                             ct.c_void_p(lab[n0:].data_ptr()),
+                                                             ct.c_void_p(cnt.data_ptr()),
+                                                             ct.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                              "true_loss_counts")
+                    part.add_(cnt)
+                piece.walk(body)
+                correct += part.to(device)
+        wrong = (N - correct).to(torch.float32)
         return wrong * torch.tensor(mean_factor(H, N), device=device)
     parts = []
     for piece, off in (slab.layout() if hasattr(slab, "layout") else [(slab, 0)]):

@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from .base import ModelSelector
-from .datasets import HostSlab, ShardedCompactSlab, ShardedSlab
+from .datasets import HostSlab, ShardedCompactSlab, ShardedHostSlab, ShardedSlab
 from .dist import (InProcessGroup, ProcessGroup, SoloGroup, choose_among_ties, default_comm, labels_per_device,
                    piece_layout, split_slab)
 from .engine import HIST_CAP, TIE_CAP, build_engines
@@ -111,7 +111,8 @@ def host_slab_refusals(gpus, shards, world):
     """What a host-resident slab (``HostSlab``) does not offer: it runs as one shard on one GPU in one process."""
     if (gpus and int(gpus) > 1) or (shards and int(shards) > 1) or world > 1:
         raise NotImplementedError("coda_b200: a HostSlab runs as one shard on one GPU (gpus=1, shards=1, one process); "
-                                  "load the task as per-GPU pieces (ShardedSlab) to use several GPUs")
+                                  "load the task as per-GPU pieces (ShardedHostSlab, ShardedSlab) to use several "
+                                  "GPUs")
 
 
 class CODA(ModelSelector):
@@ -134,7 +135,7 @@ class CODA(ModelSelector):
             host_slab_refusals(gpus, shards, comm.world)
             self.group = SoloGroup()
             layout = [(preds, 0)]
-        elif isinstance(preds, (ShardedSlab, ShardedCompactSlab)):    # the pieces are the shards
+        elif isinstance(preds, (ShardedSlab, ShardedCompactSlab, ShardedHostSlab)):    # the pieces are the shards
             layout = piece_layout(preds, gpus, shards, comm.world)
             self.group = SoloGroup() if len(layout) == 1 else InProcessGroup(len(layout))
         elif comm.world > 1:                                # one process per GPU: this is one shard of the task

@@ -183,6 +183,7 @@ SIGNATURES = {
     "coda_b200_mp_runs": (i32, [p, p, p, i32, i32, p, i64, i32, i32, p, p, i32, p, sz, p, p, p, p, p, p]),
     "coda_b200_majority": (i32, [p, i32, i64, p, p]),
     "coda_b200_pool_accuracy": (i32, [p, p, i32, p, i64, i32, p, p]),
+    "coda_b200_pool_gather": (i32, [p, p, p, i32, p, p, i64, p, p, p, p]),
     "coda_b200_pf_resolve": (i32, [p, p, i64, p, p, p, i32, i32, p, p, p]),
     "coda_b200_pf_identity": (i32, [p, p, i32, p, p, p]),
     "coda_b200_sample_plan": (i32, [p, i32, p, p, p, p, i32, i32, i32, p, p, p, p, p, p]),

@@ -376,4 +376,60 @@ extern "C" int coda_b200_pool_accuracy(const uint16_t* hard, const int64_t* labe
   return CODA_B200_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// A search's pool table: the rows of one piece's items that a block of realisations draws, copied to table slots
+// ---------------------------------------------------------------------------------------------------------------
+// one warp per pair: out_hard[slot] = hard[item] (H u16 as V words), out_disagree[slot], out_labels[slot].  A row is
+// 2H bytes, so with H a multiple of 8 (4, 2) every row starts 16 (8, 4) bytes into an aligned buffer.
+template <typename V>
+__global__ void __launch_bounds__(MR_THREADS) k_pool_gather(const uint16_t* __restrict__ hard,
+                                                           const uint8_t* __restrict__ disagree,
+                                                           const int64_t* __restrict__ labels, int H,
+                                                           const int64_t* __restrict__ slots,
+                                                           const int64_t* __restrict__ items, long long K,
+                                                           uint16_t* __restrict__ out_hard,
+                                                           uint8_t* __restrict__ out_disagree,
+                                                           int64_t* __restrict__ out_labels) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int W = H * (int)sizeof(uint16_t) / (int)sizeof(V);
+  const long long nw = (long long)gridDim.x * MR_WARPS;
+  for (long long k = (long long)blockIdx.x * MR_WARPS + warp; k < K; k += nw) {
+    const long long n = items[k], s = slots[k];
+    const V* src = reinterpret_cast<const V*>(hard + (size_t)n * H);
+    V* dst = reinterpret_cast<V*>(out_hard + (size_t)s * H);
+    for (int w = lane; w < W; w += 32) dst[w] = src[w];
+    if (lane == 0) {
+      out_disagree[s] = disagree[n];
+      out_labels[s] = labels[n];
+    }
+  }
+}
+
+extern "C" int coda_b200_pool_gather(const uint16_t* hard, const uint8_t* disagree, const int64_t* labels, int H,
+                                     const int64_t* slots, const int64_t* items, int64_t K, uint16_t* out_hard,
+                                     uint8_t* out_disagree, int64_t* out_labels, coda_stream_t stream) {
+  CODA_CHECK_ARG(H >= 1 && H <= 1024 && K >= 0, "pool_gather: bad shape H=%d K=%lld", H, (long long)K);
+  if (K == 0) return CODA_B200_OK;
+  CODA_CHECK_ARG(hard && disagree && labels && slots && items && out_hard && out_disagree && out_labels,
+                 "pool_gather: null pointer");
+  CODA_CHECK_ARG(((uintptr_t)hard | (uintptr_t)out_hard) % 16 == 0, "pool_gather: hard tables must be 16-byte aligned");
+  long long grid = (K + MR_WARPS - 1) / MR_WARPS;
+  grid = min(grid, (long long)coda_sm_count() * 16);
+  const cudaStream_t s = as_stream(stream);
+  if (H % 8 == 0)
+    k_pool_gather<uint4><<<(unsigned)grid, MR_THREADS, 0, s>>>(hard, disagree, labels, H, slots, items, K, out_hard,
+                                                               out_disagree, out_labels);
+  else if (H % 4 == 0)
+    k_pool_gather<uint2><<<(unsigned)grid, MR_THREADS, 0, s>>>(hard, disagree, labels, H, slots, items, K, out_hard,
+                                                               out_disagree, out_labels);
+  else if (H % 2 == 0)
+    k_pool_gather<uint32_t><<<(unsigned)grid, MR_THREADS, 0, s>>>(hard, disagree, labels, H, slots, items, K,
+                                                                  out_hard, out_disagree, out_labels);
+  else
+    k_pool_gather<uint16_t><<<(unsigned)grid, MR_THREADS, 0, s>>>(hard, disagree, labels, H, slots, items, K,
+                                                                  out_hard, out_disagree, out_labels);
+  CODA_LAUNCH_OK("k_pool_gather");
+  return CODA_B200_OK;
+}
+
 CODA_MODULE_ANCHOR(eps_search, k_mp_runs)

@@ -655,6 +655,14 @@ int coda_b200_majority(const uint16_t* hard, int H, int64_t N, int64_t* labels, 
 /* acc[r][h] = number of pool positions p with hard[pool[r][p]][h] == labels[pool[r][p]] */
 int coda_b200_pool_accuracy(const uint16_t* hard, const int64_t* labels, int H, const int64_t* pool, int64_t R, int P,
                             int32_t* acc, coda_stream_t stream);
+/* a search's pool table from one N-range piece: for k < K, out_hard[slots[k]] = hard[items[k]] (rows of H u16),
+ * out_disagree[slots[k]] = disagree[items[k]], out_labels[slots[k]] = labels[items[k]].  items are local to the piece
+ * (in [0, N_i)), slots are rows of the output; hard and out_hard are 16-byte aligned, all arrays on the current device.
+ * K = 0 launches nothing.  Running the other entry points above on the table with pool[r][p] = the slot of position
+ * (r, p) gives the bits they give on the whole [N][H] table with global item ids. */
+int coda_b200_pool_gather(const uint16_t* hard, const uint8_t* disagree, const int64_t* labels, int H,
+                          const int64_t* slots, const int64_t* items, int64_t K, uint16_t* out_hard,
+                          uint8_t* out_disagree, int64_t* out_labels, coda_stream_t stream);
 
 /* ---- true losses of a slab held as N-range pieces (coda/oracle.py:9-21 with coda/options.py's accuracy loss) --------
  * counts[h] = number of items n of this piece with argmax_c preds[h][n][c] == labels[n], argmax as torch.argmax decides it

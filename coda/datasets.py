@@ -1,15 +1,15 @@
 import os
 
 from coda_b200.datasets import Dataset as _Dataset
-from coda_b200.datasets import (compact_load_count, host_load_wanted, host_piece_count, is_compact_file,
-                                shard_load_count)
+from coda_b200.datasets import load_route
 
 
 class Dataset(_Dataset):
-    """reference coda/datasets.py.  ``CODA_B200_KEEP_DTYPE=1`` keeps a stored fp16 / bf16 slab at its width (half the
-    device memory, the same results as the fp32 widening).  ``CODA_B200_SHARD_LOAD=1``, or a slab larger than the
-    target device's free memory with more than one GPU visible, loads it as N-range pieces over the GPUs
-    (``coda_b200.datasets.ShardedSlab``; ``CODA_B200_GPUS`` pieces, else one per visible GPU).
+    """reference coda/datasets.py, loaded the way ``coda_b200.datasets.load_route`` decides from the ``CODA_B200_*``
+    settings.  ``CODA_B200_KEEP_DTYPE=1`` keeps a stored fp16 / bf16 slab at its width (half the device memory, the same
+    results as the fp32 widening).  ``CODA_B200_SHARD_LOAD=1``, or a slab larger than the target device's free memory
+    with more than one GPU visible, loads it as N-range pieces over the GPUs (``coda_b200.datasets.ShardedSlab``;
+    ``CODA_B200_GPUS`` pieces, else one per visible GPU).
 
     A file written by ``coda_b200.CompactSlab.save`` loads as a compact slab, and ``CODA_B200_COMPACT_K=K`` compacts a
     dense task file to its top-K form as it loads (opt-in: the compact form approximates the tail classes, so results
@@ -24,22 +24,4 @@ class Dataset(_Dataset):
     else one per visible GPU).  Compact files and ``CODA_B200_COMPACT_K`` take precedence."""
 
     def __init__(self, filepath, device):
-        keep = os.environ.get("CODA_B200_KEEP_DTYPE", "0") == "1"
-        k = os.environ.get("CODA_B200_COMPACT_K")
-        k = int(k) if k else None
-        if k or is_compact_file(filepath):
-            shards = compact_load_count(filepath, device, k)
-            super().__init__(filepath, device, compact_k=k, shards=shards or None)
-            return
-        if host_load_wanted(filepath, device, keep):
-            super().__init__(filepath, device, keep_dtype=keep, host=True)
-            return
-        shards = host_piece_count(filepath, device, keep)
-        if shards:
-            super().__init__(filepath, device, keep_dtype=keep, host=True, shards=shards)
-            return
-        shards = shard_load_count(filepath, device, keep)
-        if shards:
-            super().__init__(filepath, device, keep_dtype=keep, shards=shards)
-        else:
-            super().__init__(filepath, device, keep_dtype=keep)
+        super().__init__(filepath, device, **load_route(filepath, device, os.environ))

@@ -44,7 +44,8 @@ import torch
 
 from . import _native as nat
 from .base import ModelSelector
-from .dist import InProcessGroup, ProcessGroup, SoloGroup, default_comm, labels_per_device, piece_layout, split_slab
+from .datasets import model_stride, walk
+from .dist import ProcessGroup, default_comm, labels_per_device, shard_layout
 from .selector import _Unlabeled
 
 _NO_CPU = ("coda_b200.baselines: dataset.preds must be a CUDA tensor on an sm_90a device; there is no CPU path in this "
@@ -319,12 +320,10 @@ class _DeviceState:
                 cs = self.compact
                 self._call("coda_b200_scan_compact", _ptr(cs.ids), _ptr(cs.probs), self.model_stride, H, N, C, cs.K,
                            _ptr(hard), _ptr(pseudo), _ptr(disagree), _ptr(e), _ptr(self.flags), self._s())
-            elif self.host is not None:                    # N-range chunks: the scan is per item
-                self.host.walk(lambda n0, n1, v: self._scan_dense(_ptr(v), (n1 - n0) * C, n1 - n0, _ptr(hard[n0:]),
-                                                                  _ptr(pseudo[n0:]), _ptr(disagree[n0:]),
-                                                                  _ptr(e[n0:]) if e is not None else None))
-            else:
-                self._scan_dense(_ptr(self.preds), self.model_stride, N, _ptr(hard), _ptr(pseudo), _ptr(disagree), _ptr(e))
+            else:                                          # a host slab in N-range chunks: the scan is per item
+                walk(self.preds, lambda n0, n1, v: self._scan_dense(_ptr(v), model_stride(v), n1 - n0, _ptr(hard[n0:]),
+                                                                    _ptr(pseudo[n0:]), _ptr(disagree[n0:]),
+                                                                    _ptr(e[n0:]) if e is not None else None))
             flags = int(self.flags.item())
         if flags & nat.FLAG_NONFINITE_INPUT:
             raise RuntimeError("[NUMERIC ERROR] preds has bad values (NaN/Inf)")
@@ -546,40 +545,35 @@ def _check_rank_ranges(preds, n_offset, N, n_global, comm):
         raise ValueError(f"coda_b200.baselines: the ranks' N-ranges cover {lo} of the task's {n_global} items")
 
 
-def _layout(dataset, gpus, shards, comm):
-    """-> (group, [(shard slab, n_offset)] of this process)."""
-    from .datasets import CompactSlab, HostSlab, ShardedCompactSlab, ShardedHostSlab, ShardedSlab
-    from .selector import host_slab_refusals
-    preds = getattr(dataset, "preds", None)
-    if isinstance(preds, HostSlab):                             # one shard on the slab's compute device
-        host_slab_refusals(gpus, shards, comm.world)
-        return SoloGroup(), [(preds, 0)]
-    if isinstance(preds, (ShardedSlab, ShardedCompactSlab, ShardedHostSlab)):    # the pieces are the shards
-        layout = piece_layout(preds, gpus, shards, comm.world)
-        if not preds.is_cuda:
-            raise NotImplementedError(_NO_CPU)
-        return (SoloGroup() if len(layout) == 1 else InProcessGroup(len(layout))), layout
-    if not ((isinstance(preds, torch.Tensor) or isinstance(preds, CompactSlab)) and preds.is_cuda):
-        raise NotImplementedError(_NO_CPU)
-    n_offset = int(getattr(dataset, "n_offset", 0))
-    N = int(preds.shape[1])
-    n_global = int(getattr(dataset, "n_global", N))
-    if comm.world > 1:                                     # one process per GPU: this is one shard of the task
-        if gpus or shards:
-            raise ValueError("coda_b200.baselines: gpus= / shards= split a task inside one process; under "
-                             "torch.distributed with world > 1 every rank is one shard (pass this rank's N-range)")
-        _check_rank_ranges(preds, n_offset, N, n_global, comm)
-        return ProcessGroup(comm), [(preds, n_offset)]
-    if n_global != N:
-        raise NotImplementedError("coda_b200.baselines: an N-range shard of a task needs its peers: run one process "
-                                  "per shard under torch.distributed, or pass the whole task with gpus= / shards=")
+def _default_pieces():
+    """The competing selectors split a task into ``CODA_B200_GPUS`` pieces, else keep it whole."""
     env = os.environ.get("CODA_B200_GPUS")
-    nshards = int(shards) if shards else (int(gpus) if gpus else (max(1, int(env)) if env else 1))
-    ngpus = int(gpus) if gpus else min(nshards, max(1, torch.cuda.device_count()))
-    nshards = max(1, min(nshards, N))
-    if nshards == 1:
-        return SoloGroup(), [(preds, n_offset)]
-    return InProcessGroup(nshards), split_slab(preds, nshards, ngpus)
+    return max(1, int(env)) if env else 1
+
+
+def _layout(dataset, gpus, shards, comm):
+    """-> (group, [(shard slab, n_offset)] of this process) (``dist.shard_layout``)."""
+    from .datasets import CompactSlab, HostSlab, PieceSlab
+    preds = getattr(dataset, "preds", None)
+    n_offset = int(getattr(dataset, "n_offset", 0))
+    if not isinstance(preds, (HostSlab, PieceSlab)):         # one device slab: this rank's shard, or a task to split
+        if not (isinstance(preds, (torch.Tensor, CompactSlab)) and preds.is_cuda):
+            raise NotImplementedError(_NO_CPU)
+        N = int(preds.shape[1])
+        n_global = int(getattr(dataset, "n_global", N))
+        if comm.world > 1:
+            if gpus or shards:
+                raise ValueError("coda_b200.baselines: gpus= / shards= split a task inside one process; under "
+                                 "torch.distributed with world > 1 every rank is one shard (pass this rank's N-range)")
+            _check_rank_ranges(preds, n_offset, N, n_global, comm)
+        elif n_global != N:
+            raise NotImplementedError("coda_b200.baselines: an N-range shard of a task needs its peers: run one "
+                                      "process per shard under torch.distributed, or pass the whole task with gpus= / "
+                                      "shards=")
+    group, layout = shard_layout(preds, gpus, shards, comm, n_offset, default=_default_pieces)
+    if not preds.is_cuda:                                    # pieces: after their own refusals
+        raise NotImplementedError(_NO_CPU)
+    return group, layout
 
 
 class _Baseline(ModelSelector):

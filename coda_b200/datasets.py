@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as ct
+import functools
 import os
 
 import torch
@@ -18,28 +19,18 @@ def _slab_dtype(t: torch.Tensor, keep_dtype: bool) -> torch.dtype:
     return t.dtype if keep_dtype and t.dtype in _KEPT_DTYPES else torch.float32
 
 
-class ShardedSlab:
-    """An (H, N, C) slab held as contiguous N-range pieces, one dense (H, N_i, C) tensor per piece, each on its own
-    device (consecutive pieces may share one).  The pieces ARE the shard layout: CODA and the competing selectors run
-    one shard per piece, in place.  Duck-types the tensor attributes the selectors and main.py read from
-    ``dataset.preds``; ``device`` is the first piece's."""
+class PieceSlab:
+    """An (H, N, C) slab held as contiguous N-range pieces, each on its own device (consecutive pieces may share one).
+    The pieces ARE the shard layout: CODA and the competing selectors run one shard per piece, in place.  Duck-types the
+    tensor attributes the selectors and main.py read from ``dataset.preds``; ``device`` is the first piece's.  The
+    subclasses check their pieces (``_check``)."""
 
     def __init__(self, pieces):
         pieces = list(pieces)
         if not pieces:
-            raise ValueError("ShardedSlab: at least one piece expected")
-        for p in pieces:
-            if isinstance(p, CompactSlab) or not isinstance(p, torch.Tensor):
-                raise TypeError("ShardedSlab: pieces must be dense (H, N_i, C) tensors; a compact ShardedSlab is not "
-                                "supported")
-            if p.dim() != 3 or p.dtype not in _KEPT_DTYPES:
-                raise TypeError(f"ShardedSlab: pieces must be float32, float16 or bfloat16 (H, N_i, C) tensors, got "
-                                f"{p.dtype} {tuple(p.shape)}")
-            if not p.is_contiguous() or p.shape[1] < 1:
-                raise ValueError("ShardedSlab: every piece must be a contiguous tensor with at least one item")
+            raise ValueError(f"{type(self).__name__}: at least one piece expected")
+        self._check(pieces)
         H, _, C = pieces[0].shape
-        if any(p.shape[0] != H or p.shape[2] != C or p.dtype != pieces[0].dtype for p in pieces):
-            raise TypeError("ShardedSlab: all pieces must share one dtype, H and C")
         self.pieces = pieces
         self.offsets = []
         n = 0
@@ -62,12 +53,37 @@ class ShardedSlab:
         return self.pieces[0].element_size()
 
     def item_column(self, idx) -> torch.Tensor:
-        """The (H, C) float32 scores of item ``idx``, on the device of the piece that holds it."""
+        """The (H, C) float32 scores of item ``idx``, on the (compute) device of the piece that holds it."""
         idx = int(idx)
         if not 0 <= idx < self.shape[1]:
-            raise IndexError(f"ShardedSlab: item {idx} outside [0, {self.shape[1]})")
+            raise IndexError(f"{type(self).__name__}: item {idx} outside [0, {self.shape[1]})")
         r = max(i for i, off in enumerate(self.offsets) if off <= idx)
-        return self.pieces[r][:, idx - self.offsets[r]].float()
+        p, i = self.pieces[r], idx - self.offsets[r]
+        return p[:, i].float() if isinstance(p, torch.Tensor) else p.item_column(i)
+
+
+def pieces_of(preds):
+    """[(piece, n_offset)] of a slab: a ``PieceSlab``'s pieces, else the slab itself as one piece."""
+    return preds.layout() if isinstance(preds, PieceSlab) else [(preds, 0)]
+
+
+class ShardedSlab(PieceSlab):
+    """A ``PieceSlab`` of dense (H, N_i, C) tensors."""
+
+    @staticmethod
+    def _check(pieces):
+        for p in pieces:
+            if isinstance(p, CompactSlab) or not isinstance(p, torch.Tensor):
+                raise TypeError("ShardedSlab: pieces must be dense (H, N_i, C) tensors; a compact ShardedSlab is not "
+                                "supported")
+            if p.dim() != 3 or p.dtype not in _KEPT_DTYPES:
+                raise TypeError(f"ShardedSlab: pieces must be float32, float16 or bfloat16 (H, N_i, C) tensors, got "
+                                f"{p.dtype} {tuple(p.shape)}")
+            if not p.is_contiguous() or p.shape[1] < 1:
+                raise ValueError("ShardedSlab: every piece must be a contiguous tensor with at least one item")
+        H, _, C = pieces[0].shape
+        if any(p.shape[0] != H or p.shape[2] != C or p.dtype != pieces[0].dtype for p in pieces):
+            raise TypeError("ShardedSlab: all pieces must share one dtype, H and C")
 
 
 HOST_CHUNK_BYTES = 1 << 30
@@ -161,111 +177,36 @@ class HostDataset:
         self.n_offset, self.n_global = 0, slab.shape[1]
 
 
-class ShardedHostSlab:
-    """An (H, N, C) slab kept in host memory as contiguous N-range pieces, one ``HostSlab`` per piece, each computed on
-    its own device (consecutive pieces may share one): the host-resident twin of ``ShardedSlab``, with its surface and
-    its rules.  The pieces ARE the shard layout: CODA and the competing selectors run one host-resident shard per piece,
-    each streaming its piece through its own device and staging its own host columns each step, and give the bits of
-    the whole slab.  ``device`` is the first piece's."""
+class ShardedHostSlab(PieceSlab):
+    """A ``PieceSlab`` kept in host memory, one ``HostSlab`` per piece, each computed on its own device: the
+    host-resident twin of ``ShardedSlab``.  CODA and the competing selectors run one host-resident shard per piece, each
+    streaming its piece through its own device and staging its own host columns each step, and give the bits of the
+    whole slab."""
 
-    def __init__(self, pieces):
-        pieces = list(pieces)
-        if not pieces:
-            raise ValueError("ShardedHostSlab: at least one piece expected")
+    @staticmethod
+    def _check(pieces):
         for p in pieces:
             if not isinstance(p, HostSlab):
                 raise TypeError("ShardedHostSlab: pieces must be HostSlab (device pieces make a ShardedSlab)")
         H, _, C = pieces[0].shape
         if any(p.shape[0] != H or p.shape[2] != C or p.dtype != pieces[0].dtype for p in pieces):
             raise TypeError("ShardedHostSlab: all pieces must share one dtype, H and C")
-        self.pieces = pieces
-        self.offsets = []
-        n = 0
-        for p in pieces:
-            self.offsets.append(n)
-            n += int(p.shape[1])
-        self.shape = torch.Size([int(H), n, int(C)])
-        self.device = pieces[0].device
-        self.dtype = pieces[0].dtype
-        self.is_cuda = True
-
-    def layout(self):
-        """[(piece, n_offset)]: the shard layout selectors build from."""
-        return list(zip(self.pieces, self.offsets))
-
-    def numel(self):
-        return self.shape[0] * self.shape[1] * self.shape[2]
-
-    def element_size(self):
-        return self.pieces[0].element_size()
-
-    def item_column(self, idx) -> torch.Tensor:
-        """The (H, C) float32 scores of item ``idx``, on the compute device of the piece that holds it."""
-        idx = int(idx)
-        if not 0 <= idx < self.shape[1]:
-            raise IndexError(f"ShardedHostSlab: item {idx} outside [0, {self.shape[1]})")
-        r = max(i for i, off in enumerate(self.offsets) if off <= idx)
-        return self.pieces[r].item_column(idx - self.offsets[r])
 
 
-def host_slab_wanted(held_bytes, free_bytes, device_count, env=None):
-    """The shim's rule for a ``HostSlab`` load: ``CODA_B200_HOST_SLAB=1``, or a slab that, at the width it would be
-    held, exceeds the target device's free memory while exactly one GPU is visible (with more, it is split into
-    per-GPU pieces instead).  ``CODA_B200_HOST_SLAB=0`` never loads one."""
-    env = os.environ if env is None else env
-    v = env.get("CODA_B200_HOST_SLAB")
-    if v is not None and v != "":
-        return v == "1"
-    return device_count == 1 and held_bytes > free_bytes
+def walk(preds, body):
+    """Read a dense piece on its device: ``body(n0, n1, view)`` enqueues the kernels that read ``view``, an
+    (H, n1 - n0, C) device tensor holding items [n0, n1).  A ``HostSlab`` streams through its device in chunks
+    (``HostSlab.walk``, which returns when they are done); a device tensor is one view of itself."""
+    if isinstance(preds, HostSlab):
+        preds.walk(body)
+    else:
+        body(0, int(preds.shape[1]), preds)
 
 
-def host_load_wanted(filepath, device, keep_dtype=False, env=None):
-    """Whether ``coda.datasets.Dataset`` loads ``filepath`` as a ``HostSlab`` (``host_slab_wanted`` on the slab's bytes
-    at the width it would be held and the target device's free memory)."""
-    env = os.environ if env is None else env
-    if env.get("CODA_B200_HOST_SLAB") not in (None, ""):
-        return host_slab_wanted(0, 0, 0, env)
-    dev = torch.device(device)
-    ngpus = torch.cuda.device_count()
-    if dev.type != "cuda" or ngpus != 1:
-        return False
-    try:
-        full = _open_mmap(filepath)
-    except Exception:                                              # legacy format: keep the plain load
-        return False
-    held = full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep_dtype)).element_size()
-    try:
-        index = dev.index if dev.index is not None else torch.cuda.current_device()
-        free = _free_bytes(index)
-    except RuntimeError:                                           # no usable device: keep the plain load
-        return False
-    return host_slab_wanted(held, free, ngpus, env)
-
-
-def host_piece_count(filepath, device, keep_dtype=False, env=None):
-    """How many host-resident pieces (``ShardedHostSlab``) ``coda.datasets.Dataset`` loads ``filepath`` into: 0 for
-    none.  With more than one GPU visible and neither ``CODA_B200_HOST_SLAB`` nor ``CODA_B200_SHARD_LOAD`` set, a slab
-    that, at the width it would be held, exceeds the summed free memory of the devices its pieces would use (a shared
-    device counted once) stays in host memory in ``CODA_B200_GPUS`` pieces, else one per visible GPU."""
-    env = os.environ if env is None else env
-    if env.get("CODA_B200_HOST_SLAB") or env.get("CODA_B200_SHARD_LOAD"):
-        return 0
-    dev = torch.device(device)
-    ngpus = torch.cuda.device_count()
-    if dev.type != "cuda" or ngpus < 2:
-        return 0
-    try:
-        full = _open_mmap(filepath)
-    except Exception:                                              # legacy format: keep the plain load
-        return 0
-    held = full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep_dtype)).element_size()
-    count = max(1, int(env["CODA_B200_GPUS"])) if env.get("CODA_B200_GPUS") else ngpus
-    try:
-        plan = _load_plan(int(full.shape[1]), dev, count, None)
-        free = sum(_free_bytes(d) for d in {d for _, _, d in plan})
-    except RuntimeError:                                           # no usable device: keep the plain load
-        return 0
-    return count if held > free else 0
+def model_stride(v):
+    """Elements between two models' rows of an (H, n, C) view with contiguous items, as the slab kernels take it."""
+    H, n, C = v.shape
+    return int(v.stride(0)) if H > 1 else int(n) * int(C)
 
 
 def load_host(filepath, device, keep_dtype=False, chunk_items=None, *, shards=None, gpus=None):
@@ -283,20 +224,25 @@ def load_host(filepath, device, keep_dtype=False, chunk_items=None, *, shards=No
 
 
 def piece_plan(N, nshards, ngpus, home, device_count):
-    """[(lo, hi, device index)] of ``nshards`` N-range pieces: the ranges ``shard_range(N, r, nshards)`` and the device
-    assignment of ``dist.split_slab`` -- the home device first, consecutive pieces sharing a device when there are more
-    pieces than GPUs."""
+    """[(lo, hi, device index)] of ``nshards`` N-range pieces over ``ngpus`` devices, as the loaders and
+    ``dist.split_slab`` make them: the ranges ``shard_range(N, r, nshards)``, the home device first, then the others in
+    order, consecutive pieces sharing a device when there are more pieces than GPUs."""
     devs = [home] + [d for d in range(device_count) if d != home]
     devs = devs[:max(1, ngpus)]
     return [(*shard_range(N, r, nshards), devs[r * len(devs) // nshards]) for r in range(nshards)]
 
 
-def _load_plan(N, device, shards, gpus):
-    """``piece_plan`` of a load into ``shards`` pieces (else ``gpus``) over ``gpus`` devices (else as many as there are
-    pieces, up to the visible GPUs), the first on ``device``."""
-    nshards = int(shards) if shards else int(gpus)
+def piece_counts(N, shards, gpus, default=lambda: 1):
+    """(pieces, GPUs) of a task of N items split by ``shards=`` / ``gpus=``: ``shards`` pieces (else ``gpus``, else
+    ``default()``, at most N) over ``gpus`` GPUs (else as many as there are pieces, up to the visible GPUs)."""
+    nshards = int(shards) if shards else (int(gpus) if gpus else int(default()))
     ngpus = int(gpus) if gpus else min(nshards, max(1, torch.cuda.device_count()))
-    nshards = max(1, min(nshards, N))
+    return max(1, min(nshards, N)), ngpus
+
+
+def _load_plan(N, device, shards, gpus):
+    """``piece_plan`` of a load split by ``shards=`` / ``gpus=`` (``piece_counts``), the first piece on ``device``."""
+    nshards, ngpus = piece_counts(N, shards, gpus)
     home = device.index if device.index is not None else torch.cuda.current_device()
     return piece_plan(N, nshards, ngpus, home, torch.cuda.device_count())
 
@@ -393,45 +339,89 @@ def _free_bytes(index):
     return torch.cuda.mem_get_info(index)[0]
 
 
-def _piece_count(held_bytes, device, env):
-    """The shim's piece-count rule: ``CODA_B200_GPUS`` (else the visible GPUs) pieces when ``CODA_B200_SHARD_LOAD=1``,
-    or when ``held_bytes()`` exceeds the free memory of the target device and more than one GPU is visible; else 0."""
-    env = os.environ if env is None else env
-    ngpus = torch.cuda.device_count()
-    count = max(1, int(env["CODA_B200_GPUS"])) if env.get("CODA_B200_GPUS") else max(1, ngpus)
-    if env.get("CODA_B200_SHARD_LOAD", "0") == "1":
-        return count
-    dev = torch.device(device)
-    if dev.type != "cuda" or ngpus < 2:
-        return 0
+def _map_contents(filepath):
+    """``torch.load`` of a zip file through a memory map; None for a legacy-format file or one it does not read."""
+    import zipfile
+    if not zipfile.is_zipfile(filepath):
+        return None
     try:
-        nbytes = held_bytes()
-    except Exception:                                              # legacy format: keep the plain load
-        return 0
-    index = dev.index if dev.index is not None else torch.cuda.current_device()
-    return count if nbytes > _free_bytes(index) else 0
+        return torch.load(filepath, map_location="cpu", mmap=True, weights_only=True)
+    except Exception:
+        return None
 
 
-def shard_load_count(filepath, device, keep_dtype=False, env=None):
-    """How many pieces ``coda.datasets.Dataset`` loads ``filepath`` into: 0 for a plain load.  Sharded when
-    ``CODA_B200_SHARD_LOAD=1``, or when the slab (at the width it would be held) exceeds the free memory of the target
-    device and more than one GPU is visible.  The count is ``CODA_B200_GPUS`` if set, else the visible GPUs."""
-    def held():
-        full = _open_mmap(filepath)
-        return full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep_dtype)).element_size()
-    return _piece_count(held, device, env)
+def load_route(filepath, device, env=None):
+    """The keyword arguments ``coda.datasets.Dataset`` loads ``filepath`` on ``device`` with, under the ``CODA_B200_*``
+    settings in ``env`` (default ``os.environ``; an empty value counts as unset).  A slab counts at the width it would
+    be held at; the file is opened once and each device's free memory read at most once.
 
+    * A ``CompactSlab.save`` file, or any file with ``CODA_B200_COMPACT_K=K``: a compact load, in device pieces by the
+      last rule below on its compact byte count.
+    * ``CODA_B200_HOST_SLAB=1``: one ``HostSlab``; any other value turns the host rules off.
+    * One GPU visible: a ``HostSlab`` when the slab exceeds the target device's free memory.
+    * More than one GPU visible and ``CODA_B200_SHARD_LOAD`` unset: ``CODA_B200_GPUS`` host pieces (else one per
+      visible GPU) when the slab exceeds the summed free memory of the devices they would use, a shared one counted
+      once.
+    * Device pieces, as many: with ``CODA_B200_SHARD_LOAD=1``, or with more than one GPU visible when the slab exceeds
+      the target device's free memory.
+    * Else the plain load.
 
-def compact_load_count(filepath, device, K=None, env=None):
-    """``shard_load_count``'s rule for a compact load of ``filepath`` (a ``CompactSlab.save`` file, or a dense file
-    compacted at ``K``), applied to the compact byte count: 0 means one piece."""
-    def held():
-        obj = _open_compact(filepath)
-        if obj is not None:
-            return obj["ids"].numel() * 6
-        H, N, _ = _open_mmap(filepath).shape
-        return int(H) * int(N) * int(K) * 6
-    return _piece_count(held, device, env)
+    A file that cannot be memory-mapped (the legacy format) keeps the plain load; so does a failure to read free
+    memory in the host rules, while in the device-piece rule it raises."""
+    env = os.environ if env is None else env
+    keep = env.get("CODA_B200_KEEP_DTYPE", "0") == "1"
+    k = int(env["CODA_B200_COMPACT_K"]) if env.get("CODA_B200_COMPACT_K") else None
+    dev = torch.device(device)
+    ngpus = torch.cuda.device_count()
+    free = functools.cache(_free_bytes)
+
+    def home():
+        return dev.index if dev.index is not None else torch.cuda.current_device()
+
+    def piece_count():
+        return max(1, int(env["CODA_B200_GPUS"])) if env.get("CODA_B200_GPUS") else max(1, ngpus)
+
+    def device_pieces(held):
+        count = piece_count()
+        if env.get("CODA_B200_SHARD_LOAD", "0") == "1":
+            return count
+        if dev.type != "cuda" or ngpus < 2 or held is None:
+            return 0
+        return count if held > free(home()) else 0
+
+    obj = _map_contents(filepath)
+    try:
+        comp = _compact_contents(obj, filepath)
+        compact = comp is not None
+    except ValueError:                                             # a compact file load_compact refuses, saying why
+        comp, compact = None, True
+    except Exception:
+        comp, compact = None, False
+    full = obj if isinstance(obj, torch.Tensor) and obj.dim() == 3 and obj.is_contiguous() else None
+    if k or compact:
+        held = (comp["ids"].numel() * 6 if comp is not None
+                else int(full.shape[0]) * int(full.shape[1]) * k * 6 if full is not None else None)
+        return {"compact_k": k, "shards": device_pieces(held) or None}
+    held = full.numel() * torch.empty(0, dtype=_slab_dtype(full, keep)).element_size() if full is not None else None
+    host = env.get("CODA_B200_HOST_SLAB")
+    if host:
+        if host == "1":
+            return {"keep_dtype": keep, "host": True}
+    elif dev.type == "cuda" and held is not None and ngpus == 1:
+        try:
+            if held > free(home()):
+                return {"keep_dtype": keep, "host": True}
+        except RuntimeError:                                       # no usable device: keep the plain load
+            pass
+    elif dev.type == "cuda" and held is not None and ngpus > 1 and not env.get("CODA_B200_SHARD_LOAD"):
+        count = piece_count()
+        try:
+            if held > sum(free(d) for d in {d for _, _, d in _load_plan(int(full.shape[1]), dev, count, None)}):
+                return {"keep_dtype": keep, "host": True, "shards": count}
+        except RuntimeError:                                       # no usable device: keep the plain load
+            pass
+    shards = device_pieces(held)
+    return {"keep_dtype": keep, "shards": shards} if shards else {"keep_dtype": keep}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -454,7 +444,11 @@ def _open_compact(filepath):
     import zipfile
     if not zipfile.is_zipfile(filepath):
         return None
-    obj = torch.load(filepath, map_location="cpu", mmap=True, weights_only=True)
+    return _compact_contents(torch.load(filepath, map_location="cpu", mmap=True, weights_only=True), filepath)
+
+
+def _compact_contents(obj, filepath):
+    """``obj``, the contents of ``filepath``, if it is a compact slab this loader reads; None for any other file."""
     if not (isinstance(obj, dict) and obj.get("format") == COMPACT_FORMAT):
         return None
     if obj.get("version") != COMPACT_VERSION:
@@ -580,12 +574,9 @@ def load_compact(filepath, device, K=None, *, shards=None, gpus=None, chunk_byte
         if full.dtype not in _KEPT_DTYPES:
             raise TypeError(f"{filepath}: compacting takes a float32, float16 or bfloat16 slab, got {full.dtype}")
         K = _check_k(K, C)
-    nshards = int(shards) if shards else (int(gpus) if gpus else 1)
-    ngpus = int(gpus) if gpus else min(nshards, max(1, torch.cuda.device_count()))
-    nshards = max(1, min(nshards, N))
     dev = torch.device(device)
     home = dev.index if dev.index is not None else torch.cuda.current_device()
-    plan = piece_plan(N, nshards, ngpus, home, torch.cuda.device_count())
+    plan = _load_plan(N, dev, shards, gpus)
     pieces, by_dev = [], {}
     for lo, hi, d in plan:
         dd = torch.device("cuda", d)
@@ -795,16 +786,18 @@ class CompactSlab:
         return col
 
 
-class ShardedCompactSlab:
-    """A compact slab held as contiguous N-range pieces, one ``CompactSlab`` per piece, each on its own device: the
-    compact twin of ``ShardedSlab``, with its surface and its rules.  The pieces ARE the shard layout: CODA and the
-    competing selectors run one shard per piece, in place, and give the bits of the whole ``CompactSlab`` with
-    ``shards=`` the piece count.  ``device`` is the first piece's."""
+class ShardedCompactSlab(PieceSlab):
+    """A ``PieceSlab`` of ``CompactSlab`` pieces: the compact twin of ``ShardedSlab``.  CODA and the competing selectors
+    give the bits of the whole ``CompactSlab`` with ``shards=`` the piece count."""
 
     def __init__(self, pieces):
-        pieces = list(pieces)
-        if not pieces:
-            raise ValueError("ShardedCompactSlab: at least one piece expected")
+        super().__init__(pieces)
+        self.shape = tuple(self.shape)
+        self.C, self.K = self.shape[2], self.pieces[0].K
+        self.compaction = None
+
+    @staticmethod
+    def _check(pieces):
         for p in pieces:
             if not isinstance(p, CompactSlab):
                 raise TypeError("ShardedCompactSlab: pieces must be CompactSlab (dense pieces make a ShardedSlab)")
@@ -814,33 +807,9 @@ class ShardedCompactSlab:
         K = pieces[0].K
         if any(p.shape[0] != H or p.C != C or p.K != K for p in pieces):
             raise TypeError("ShardedCompactSlab: all pieces must share H, C and K")
-        self.pieces = pieces
-        self.offsets = []
-        n = 0
-        for p in pieces:
-            self.offsets.append(n)
-            n += int(p.shape[1])
-        self.shape = (int(H), n, int(C))
-        self.C, self.K = int(C), int(K)
-        self.device = pieces[0].device
-        self.dtype = torch.float32
-        self.is_cuda = pieces[0].is_cuda
-        self.compaction = None
-
-    def layout(self):
-        """[(piece, n_offset)]: the shard layout selectors build from."""
-        return list(zip(self.pieces, self.offsets))
 
     def numel(self):
         return sum(p.numel() for p in self.pieces)
-
-    def item_column(self, idx) -> torch.Tensor:
-        """The dense (H, C) float32 scores of item ``idx`` (``CompactSlab.item_column``), on its piece's device."""
-        idx = int(idx)
-        if not 0 <= idx < self.shape[1]:
-            raise IndexError(f"ShardedCompactSlab: item {idx} outside [0, {self.shape[1]})")
-        r = max(i for i, off in enumerate(self.offsets) if off <= idx)
-        return self.pieces[r].item_column(idx - self.offsets[r])
 
 
 class CompactDataset:

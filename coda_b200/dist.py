@@ -25,6 +25,7 @@ import ctypes as ct
 import torch
 
 from . import _native as nat
+from .datasets import HostSlab, PieceSlab, piece_counts, piece_plan
 
 
 class LocalComm:
@@ -149,10 +150,19 @@ class Mailbox:
             pass
 
 
+def host_slab_refusals(gpus, shards, world):
+    """What a host-resident slab (``HostSlab``) does not offer: it runs as one shard on one GPU in one process."""
+    if (gpus and int(gpus) > 1) or (shards and int(shards) > 1) or world > 1:
+        raise NotImplementedError("coda_b200: a HostSlab runs as one shard on one GPU (gpus=1, shards=1, one process); "
+                                  "load the task as per-GPU pieces (ShardedHostSlab, ShardedSlab) to use several "
+                                  "GPUs")
+
+
 def piece_layout(slab, gpus, shards, world):
-    """A ``ShardedSlab`` (``ShardedCompactSlab``, ``ShardedHostSlab``) is its own shard layout: [(piece, n_offset)],
-    used in place (no peer copy, no re-split, and ``CODA_B200_GPUS`` is not consulted).  ``shards=`` (or ``gpus=``
-    alone) must equal the piece count, ``gpus=`` with ``shards=`` the number of devices the pieces are on."""
+    """A ``PieceSlab`` (``ShardedSlab``, ``ShardedCompactSlab``, ``ShardedHostSlab``) is its own shard layout:
+    [(piece, n_offset)], used in place (no peer copy, no re-split, and ``CODA_B200_GPUS`` is not consulted).
+    ``shards=`` (or ``gpus=`` alone) must equal the piece count, ``gpus=`` with ``shards=`` the number of devices the
+    pieces are on."""
     name = type(slab).__name__
     if world > 1:
         raise ValueError(f"coda_b200: a {name} holds the whole task in one process; under torch.distributed with "
@@ -168,20 +178,36 @@ def piece_layout(slab, gpus, shards, world):
     return slab.layout()
 
 
+def shard_layout(preds, gpus, shards, comm, n_offset=0, default=lambda: 1):
+    """-> (group, [(shard slab, n_offset)] of this process) of a selector over ``preds``:
+
+    * a ``HostSlab``: one shard on its compute device;
+    * a ``PieceSlab``: its pieces, one shard each (``piece_layout``);
+    * a tensor or ``CompactSlab`` under torch.distributed with world > 1: this rank's shard of the task;
+    * else a tensor or ``CompactSlab`` split into ``piece_counts`` N-range shards (``default()`` when neither
+      ``shards=`` nor ``gpus=`` is given), or kept whole as one."""
+    if isinstance(preds, HostSlab):
+        host_slab_refusals(gpus, shards, comm.world)
+        return SoloGroup(), [(preds, 0)]
+    if isinstance(preds, PieceSlab):
+        layout = piece_layout(preds, gpus, shards, comm.world)
+        return (SoloGroup() if len(layout) == 1 else InProcessGroup(len(layout))), layout
+    if comm.world > 1:
+        return ProcessGroup(comm), [(preds, n_offset)]
+    nshards, ngpus = piece_counts(preds.shape[1], shards, gpus, default)
+    if nshards == 1:
+        return SoloGroup(), [(preds, n_offset)]
+    return InProcessGroup(nshards), split_slab(preds, nshards, ngpus)
+
+
 def split_slab(preds, nshards, ngpus):
-    """N-range shards of a slab that lives on one device -> [(shard slab, n_offset)]: shards on the home device are
-    VIEWS of the caller's tensor (the kernels take the model stride), the others are contiguous copies on their device.
-    Consecutive shards share a device when there are more shards than GPUs.  Works for a dense tensor and a
-    ``CompactSlab``."""
-    from .synth import shard_range
-    n = preds.shape[1]
+    """N-range shards of a slab that lives on one device, as ``datasets.piece_plan`` places them -> [(shard slab,
+    n_offset)]: shards on the home device are VIEWS of the caller's tensor (the kernels take the model stride), the
+    others are contiguous copies on their device.  Works for a dense tensor and a ``CompactSlab``."""
     home = preds.device.index
-    devs = [home] + [d for d in range(torch.cuda.device_count()) if d != home]
-    devs = devs[:max(1, ngpus)]
+    plan = piece_plan(preds.shape[1], nshards, ngpus, home, torch.cuda.device_count())
     out = []
-    for r in range(nshards):
-        lo, hi = shard_range(n, r, nshards)
-        d = devs[r * len(devs) // nshards]
+    for lo, hi, d in plan:
         if isinstance(preds, torch.Tensor):
             view = preds[:, lo:hi]
             if d != home:
@@ -191,7 +217,7 @@ def split_slab(preds, nshards, ngpus):
             if d != home:
                 view = view.to(torch.device("cuda", d))
         out.append((view, lo))
-    for d in devs:                                      # the peer copies ran on the current streams; the shards use their own
+    for d in {d for _, _, d in plan}:                   # the peer copies ran on the current streams; the shards use their own
         torch.cuda.synchronize(d)
     return out
 

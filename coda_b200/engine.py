@@ -29,6 +29,7 @@ import numpy as np
 import torch
 
 from . import _native as nat
+from .datasets import model_stride, walk
 
 _CONST_SLOTS = {}          # device index -> set of constant-memory term-table slots in use (csrc/slab.cu c_terms_bank)
 _CONST_TERMS = 3584
@@ -391,10 +392,8 @@ class Engine:
                 self._build_compact_index()
                 return
             self._record_kernels()
-            if self.host is not None:                           # per chunk; the confusion sums are order-free integers
-                self.host.walk(lambda n0, n1, v: self._scan_range(_ptr(v), (n1 - n0) * C, n0, n1 - n0))
-            else:
-                self._scan_range(_ptr(self.preds), self.model_stride, 0, N)
+            # a host slab in chunks: the confusion sums are order-free integers
+            walk(self.preds, lambda n0, n1, v: self._scan_range(_ptr(v), model_stride(v), n0, n1 - n0))
 
     def _scan_range(self, base, model_stride, n0, n):
         """The slab scan and the confusion sums of items [n0, n0 + n), read from ``base`` (their first item)."""
@@ -493,10 +492,8 @@ class Engine:
             self._call("coda_b200_pi_full_compact", _ptr(cs.ids), _ptr(cs.probs), self.model_stride, _ptr(self.D), H, N, C,
                        self.K, _ptr(dt), _ptr(rs), _ptr(self.U), s, n=3)
             del dt, rs
-        elif self.host is not None:
-            self.host.walk(lambda n0, n1, v: self._pi_full(_ptr(v), (n1 - n0) * C, n0, n1 - n0))
         else:
-            self._pi_full()
+            walk(self.preds, lambda n0, n1, v: self._pi_full(_ptr(v), model_stride(v), n0, n1 - n0))
         self._call("coda_b200_pi_reduce", _ptr(self.U), N, C, self.fx_shift, None, _ptr(self.pisum),
                    _ptr(self.flags), s)
 

@@ -137,11 +137,10 @@ def hard_labels(dataset):
     raise as the selectors raise them."""
     import concurrent.futures as cf
     from .baselines import _DeviceState
-    from .datasets import ShardedCompactSlab, ShardedHostSlab, ShardedSlab
+    from .datasets import pieces_of
     preds = getattr(dataset, "preds", None)
     shape = _whole_task(dataset, preds)
-    sharded = isinstance(preds, (ShardedSlab, ShardedCompactSlab, ShardedHostSlab))
-    states = [_DeviceState(p, off) for p, off in (preds.layout() if sharded else [(preds, 0)])]
+    states = [_DeviceState(p, off) for p, off in pieces_of(preds)]
 
     def scan(sts):
         out = []
@@ -346,12 +345,12 @@ def modelpicker_eps_search(dataset, epsilons=DEFAULT_EPSILONS, iterations=1000, 
     ``picks`` / ``best`` / ``pick_tie`` / ``best_tie`` [E, R, B] arrays (pool positions and models of every step),
     ``realisations`` [R, P], ``pool_accuracies`` [R, H], ``labels`` [N], ``epsilons``, ``seed``."""
     eps = _check_epsilons(epsilons)
-    from .datasets import HostSlab, ShardedCompactSlab, ShardedHostSlab, ShardedSlab
+    from .datasets import HostSlab, PieceSlab
     if isinstance(dataset, HardLabels):
         H, N, C = dataset.shape
     else:
         preds = getattr(dataset, "preds", None)
-        if isinstance(preds, (ShardedSlab, ShardedCompactSlab, HostSlab, ShardedHostSlab)):
+        if isinstance(preds, (PieceSlab, HostSlab)):
             raise NotImplementedError(f"modelpicker_eps_search: a {type(preds).__name__} (a slab loaded as N-range "
                                       f"pieces or kept in host memory) is searched through its predicted-class table: "
                                       f"modelpicker_eps_search(coda_b200.eps_search.hard_labels(dataset), ...)")

@@ -14,10 +14,10 @@ class Oracle:
         assert self.labels is not None, "Oracle needs labels!"
 
     def true_losses(self, preds):
-        """Mean loss of every model, (H,) (coda/oracle.py:9-21).  A ``ShardedSlab``, ``CompactSlab`` or
-        ``ShardedCompactSlab`` takes the accuracy loss only, on the pieces' devices (``sharded_true_losses``)."""
-        from .datasets import CompactSlab, HostSlab, ShardedCompactSlab, ShardedHostSlab, ShardedSlab
-        if isinstance(preds, (ShardedSlab, CompactSlab, ShardedCompactSlab, HostSlab, ShardedHostSlab)):
+        """Mean loss of every model, (H,) (coda/oracle.py:9-21).  A ``CompactSlab``, ``HostSlab`` or ``PieceSlab``
+        takes the accuracy loss only, on the pieces' devices (``sharded_true_losses``)."""
+        from .datasets import CompactSlab, HostSlab, PieceSlab
+        if isinstance(preds, (CompactSlab, HostSlab, PieceSlab)):
             return sharded_true_losses(preds, self.labels, self.loss_fn, self.dataset.device)
         H, N, C = preds.shape
         return self.loss_fn(preds.reshape(-1, C), self.labels.repeat(H), reduction="none").view(H, N).mean(dim=1)
@@ -33,10 +33,10 @@ def mean_factor(H, N):
 
 
 def sharded_true_losses(slab, labels, loss_fn, device):
-    """``Oracle.true_losses`` of a ``ShardedSlab`` with the accuracy loss: one ``coda_b200_true_loss_counts`` launch per
-    piece, each on its device and a stream of its own, all in flight together.  The per-model wrong counts are exact
-    integers below 2^24, so they equal torch's fp32 sums; the result carries the bits of ``true_losses`` on the same
-    slab held as one tensor, on ``device``.
+    """``Oracle.true_losses`` of a slab in pieces (``datasets.pieces_of``) with the accuracy loss: one
+    ``coda_b200_true_loss_counts`` launch per device piece, each on its device and a stream of its own, all in flight
+    together.  The per-model wrong counts are exact integers below 2^24, so they equal torch's fp32 sums; the result
+    carries the bits of ``true_losses`` on the same slab held as one tensor, on ``device``.
 
     A ``CompactSlab`` (one piece) or ``ShardedCompactSlab`` counts the items whose ``ids[0]`` -- the hard prediction
     every selector sees -- is the label (``coda_b200_true_loss_counts_compact``).  For a slab compacted from a dense one
@@ -44,10 +44,10 @@ def sharded_true_losses(slab, labels, loss_fn, device):
     ``true_losses`` on the dense slab.  It can differ from ``true_losses(slab.densify())`` only in the rows counted in
     ``compaction["flat_rows"]``, where the uniform remainder reaches ``probs[0]``.
 
-    A ``HostSlab`` is counted chunk by chunk as it streams through its device (``HostSlab.walk``); a
-    ``ShardedHostSlab`` piece by piece, each through its own device."""
+    A ``HostSlab`` piece is counted chunk by chunk as it streams through its device (``HostSlab.walk``), after the
+    device pieces before it are in flight and before the pieces after it start."""
     from . import _native as nat
-    from .datasets import CompactSlab, HostSlab, ShardedHostSlab
+    from .datasets import CompactSlab, model_stride, pieces_of, walk
     name = type(slab).__name__
     try:
         from coda.options import accuracy_loss                # what LOSS_FNS["acc"] resolves to
@@ -66,29 +66,8 @@ def sharded_true_losses(slab, labels, loss_fn, device):
         raise NotImplementedError(f"coda_b200: the pieces of a {name} must be CUDA tensors; there is no CPU path")
     lib = nat.load()
     labels = labels.to(torch.int64)
-    if isinstance(slab, (HostSlab, ShardedHostSlab)):
-        correct = torch.zeros(H, dtype=torch.int64, device=device)
-        for piece, off in (slab.layout() if isinstance(slab, ShardedHostSlab) else [(slab, 0)]):
-            dev = piece.device
-            with torch.cuda.device(dev):
-                lab = labels[off:off + int(piece.shape[1])].to(dev)
-                part = torch.zeros(H, dtype=torch.int64, device=dev)
-
-                def body(n0, n1, v):
-                    cnt = torch.zeros(H, dtype=torch.int64, device=dev)
-                    nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(v.data_ptr()), nat.slab_format(v.dtype),
-                                                             (n1 - n0) * C, H, n1 - n0, C,
-                                                             ct.c_void_p(lab[n0:].data_ptr()),
-                                                             ct.c_void_p(cnt.data_ptr()),
-                                                             ct.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-                              "true_loss_counts")
-                    part.add_(cnt)
-                piece.walk(body)
-                correct += part.to(device)
-        wrong = (N - correct).to(torch.float32)
-        return wrong * torch.tensor(mean_factor(H, N), device=device)
     parts = []
-    for piece, off in (slab.layout() if hasattr(slab, "layout") else [(slab, 0)]):
+    for piece, off in pieces_of(slab):
         dev = piece.device
         n = int(piece.shape[1])
         with torch.cuda.device(dev):
@@ -96,19 +75,24 @@ def sharded_true_losses(slab, labels, loss_fn, device):
             st.wait_stream(torch.cuda.current_stream(dev))
             with torch.cuda.stream(st):
                 lab = labels[off:off + n].to(dev, non_blocking=False)
-                cnt = torch.empty(H, dtype=torch.int64, device=dev)
                 if isinstance(piece, CompactSlab):
-                    stride = int(piece.ids.stride(0)) if H > 1 else n * piece.K
+                    cnt = torch.empty(H, dtype=torch.int64, device=dev)
                     nat.check(lib.coda_b200_true_loss_counts_compact(
-                        ct.c_void_p(piece.ids.data_ptr()), stride, H, n, piece.K, ct.c_void_p(lab.data_ptr()),
-                        ct.c_void_p(cnt.data_ptr()), ct.c_void_p(st.cuda_stream)), "true_loss_counts_compact")
+                        ct.c_void_p(piece.ids.data_ptr()), model_stride(piece.ids), H, n, piece.K,
+                        ct.c_void_p(lab.data_ptr()), ct.c_void_p(cnt.data_ptr()), ct.c_void_p(st.cuda_stream)),
+                        "true_loss_counts_compact")
+                    parts.append((cnt, st))
                 else:
-                    nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(piece.data_ptr()), nat.slab_format(slab.dtype),
-                                                             int(piece.stride(0)), H, n, C, ct.c_void_p(lab.data_ptr()),
-                                                             ct.c_void_p(cnt.data_ptr()), ct.c_void_p(st.cuda_stream)),
-                              "true_loss_counts")
+                    def body(n0, n1, v):
+                        cnt = torch.empty(H, dtype=torch.int64, device=dev)
+                        nat.check(lib.coda_b200_true_loss_counts(ct.c_void_p(v.data_ptr()), nat.slab_format(v.dtype),
+                                                                 model_stride(v), H, n1 - n0, C,
+                                                                 ct.c_void_p(lab[n0:].data_ptr()),
+                                                                 ct.c_void_p(cnt.data_ptr()), ct.c_void_p(st.cuda_stream)),
+                                  "true_loss_counts")
+                        parts.append((cnt, st))
+                    walk(piece, body)          # a host piece returns when its chunks are counted
                 lab.record_stream(st)
-        parts.append((cnt, st))
     correct = torch.zeros(H, dtype=torch.int64, device=device)
     for cnt, st in parts:
         st.synchronize()

@@ -22,9 +22,7 @@ import numpy as np
 import torch
 
 from .base import ModelSelector
-from .datasets import HostSlab, ShardedCompactSlab, ShardedHostSlab, ShardedSlab
-from .dist import (InProcessGroup, ProcessGroup, SoloGroup, choose_among_ties, default_comm, labels_per_device,
-                   piece_layout, split_slab)
+from .dist import choose_among_ties, default_comm, labels_per_device, shard_layout
 from .engine import HIST_CAP, TIE_CAP, build_engines
 
 
@@ -107,14 +105,6 @@ def _auto_gpus(preds) -> int:
     return max(1, torch.cuda.device_count())
 
 
-def host_slab_refusals(gpus, shards, world):
-    """What a host-resident slab (``HostSlab``) does not offer: it runs as one shard on one GPU in one process."""
-    if (gpus and int(gpus) > 1) or (shards and int(shards) > 1) or world > 1:
-        raise NotImplementedError("coda_b200: a HostSlab runs as one shard on one GPU (gpus=1, shards=1, one process); "
-                                  "load the task as per-GPU pieces (ShardedHostSlab, ShardedSlab) to use several "
-                                  "GPUs")
-
-
 class CODA(ModelSelector):
     def __init__(self, dataset, prefilter_n=0, alpha=0.9, learning_rate=0.01, multiplier=2.0,
                  disable_diag_prior=False, q="eig", *, mode="incremental", comm=None, gpus=None, shards=None):
@@ -131,26 +121,7 @@ class CODA(ModelSelector):
         n_global = int(getattr(dataset, "n_global", preds.shape[1]))
         kw = dict(alpha=alpha, learning_rate=learning_rate, multiplier=multiplier,
                   uniform_prior=bool(disable_diag_prior), mode=mode, n_global=n_global, prefilter_n=prefilter_n, q=q)
-        if isinstance(preds, HostSlab):                     # one shard on the slab's compute device
-            host_slab_refusals(gpus, shards, comm.world)
-            self.group = SoloGroup()
-            layout = [(preds, 0)]
-        elif isinstance(preds, (ShardedSlab, ShardedCompactSlab, ShardedHostSlab)):    # the pieces are the shards
-            layout = piece_layout(preds, gpus, shards, comm.world)
-            self.group = SoloGroup() if len(layout) == 1 else InProcessGroup(len(layout))
-        elif comm.world > 1:                                # one process per GPU: this is one shard of the task
-            self.group = ProcessGroup(comm)
-            layout = [(preds, n_offset)]
-        else:
-            nshards = int(shards) if shards else (int(gpus) if gpus else _auto_gpus(preds))
-            ngpus = int(gpus) if gpus else min(nshards, max(1, torch.cuda.device_count()))
-            nshards = max(1, min(nshards, preds.shape[1]))
-            if nshards == 1:
-                self.group = SoloGroup()
-                layout = [(preds, n_offset)]
-            else:
-                self.group = InProcessGroup(nshards)
-                layout = self._split(preds, nshards, ngpus)
+        self.group, layout = shard_layout(preds, gpus, shards, comm, n_offset, default=lambda: _auto_gpus(preds))
         self.engines = build_engines(layout, self.group, **kw)
         self.engine = self.engines[0]
         self.H, self.C = self.engine.H, self.engine.C
@@ -164,10 +135,6 @@ class CODA(ModelSelector):
         self._hist_seen = 0                                 # device-loop steps already mirrored into the host lists
         self._labels_dev = None
         self._loop_dirty = False
-
-    @staticmethod
-    def _split(preds, nshards, ngpus):
-        return split_slab(preds, nshards, ngpus)
 
     @classmethod
     def from_args(cls, dataset, args):

@@ -213,14 +213,17 @@ def test_eps_search_and_true_losses_refuse_what_they_do_not_take():
 # the shim's choice of load
 # ---------------------------------------------------------------------------------------------------------------------
 def _count(monkeypatch, path, env, free, ngpus, K=None, device="cuda:0"):
+    """``load_route``'s piece count of a compact load (0 for one piece)."""
     import coda_b200.datasets as ds
     monkeypatch.setattr(ds, "_free_bytes", lambda index: free)
     monkeypatch.setattr(torch.cuda, "device_count", lambda: ngpus)
     monkeypatch.setattr(torch.cuda, "current_device", lambda: 0)
-    return ds.compact_load_count(path, device, K, env=env)
+    route = ds.load_route(path, device, {**env, **({"CODA_B200_COMPACT_K": str(K)} if K else {})})
+    assert route["compact_k"] == K
+    return route["shards"] or 0
 
 
-def test_compact_piece_count_rule(tmp_path, monkeypatch):
+def test_load_route_compact_piece_count(tmp_path, monkeypatch):
     dense = str(tmp_path / "task.pt")
     torch.save(torch.rand(4, 50, 10), dense)
     comp = str(tmp_path / "comp.pt")

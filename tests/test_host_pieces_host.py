@@ -1,4 +1,4 @@
-"""CPU tier of a host-resident slab in N-range pieces (``ShardedHostSlab``): the shim's piece-count rule and its
+"""CPU tier of a host-resident slab in N-range pieces (``ShardedHostSlab``): the load route's host-piece rule and its
 dispatch, the N-range ``HostSlab`` view, the pieces' surface and validation, the loader's plan and its one shared memory
 map, and the refusals that need no device."""
 import pytest
@@ -21,15 +21,17 @@ def _gpus(monkeypatch, free, current=0):
 
 
 def _count(monkeypatch, path, env, free, keep=False, device="cuda:0"):
+    """How many host pieces ``load_route`` loads ``path`` into: 0 for none."""
     import coda_b200.datasets as ds
     _gpus(monkeypatch, free)
-    return ds.host_piece_count(path, device, keep, env=env)
+    route = ds.load_route(path, device, {"CODA_B200_KEEP_DTYPE": "1" if keep else "0", **env})
+    return route["shards"] if route.get("host") and "shards" in route else 0
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # the shim's rule and its dispatch
 # ---------------------------------------------------------------------------------------------------------------------
-def test_host_piece_count_rule(tmp_path, monkeypatch):
+def test_load_route_host_piece_count(tmp_path, monkeypatch):
     p, t = _slab_file(tmp_path, dtype=torch.float16)
     b32, b16 = t.numel() * 4, t.numel() * 2
     # more than the summed free memory of the GPUs the pieces would use: one host piece per GPU
@@ -58,7 +60,7 @@ def test_host_piece_count_rule(tmp_path, monkeypatch):
     assert _count(monkeypatch, p, {"CODA_B200_HOST_SLAB": "", "CODA_B200_SHARD_LOAD": ""}, [0, 0]) == 2
 
 
-def test_host_piece_count_keeps_the_plain_load_for_a_legacy_file(tmp_path, monkeypatch):
+def test_load_route_host_pieces_keep_the_plain_load_for_a_legacy_file(tmp_path, monkeypatch):
     p = str(tmp_path / "legacy.pt")
     torch.save(torch.rand(3, 11, 4), p, _use_new_zipfile_serialization=False)
     assert _count(monkeypatch, p, {}, [0, 0]) == 0

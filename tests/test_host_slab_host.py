@@ -1,4 +1,4 @@
-"""CPU tier of the host-resident slab: the shim's decision rule, HostSlab's validation and chunking, and the ABI of the
+"""CPU tier of the host-resident slab: the load route's one-GPU rule, HostSlab's validation and chunking, and the ABI of the
 staging entry points (declared, bound with matching arity, step-struct fields appended at the end)."""
 import os
 import re
@@ -9,8 +9,19 @@ import torch
 from helpers import ROOT
 
 
-def test_host_slab_decision_rule():
-    from coda_b200.datasets import host_slab_wanted
+def test_load_route_host_slab_rule(tmp_path, monkeypatch):
+    import coda_b200.datasets as ds
+    path = str(tmp_path / "task.pt")
+    torch.save(torch.rand(3, 40, 5), path)
+    held = 3 * 40 * 5 * 4
+
+    def host_slab_wanted(held_bytes, free_bytes, device_count, env):
+        """Whether ``load_route`` loads the slab, scaled to ``held_bytes``, as one ``HostSlab``."""
+        monkeypatch.setattr(ds, "_free_bytes", lambda index: free_bytes * held // held_bytes)
+        monkeypatch.setattr(torch.cuda, "device_count", lambda: device_count)
+        monkeypatch.setattr(torch.cuda, "current_device", lambda: 0)
+        return ds.load_route(path, "cuda:0", env) == {"keep_dtype": False, "host": True}
+
     G = 1 << 30
     assert host_slab_wanted(100 * G, 80 * G, 1, {}) is True               # too large for the one GPU
     assert host_slab_wanted(10 * G, 80 * G, 1, {}) is False               # fits: the plain load

@@ -347,7 +347,7 @@ def test_device_zero_holds_only_its_piece_on_several_gpus(tmp_path, monkeypatch)
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    import coda_b200.selector as selector
+    import coda_b200.dist as dist
     from coda_b200 import CODA
     from coda_b200.datasets import Dataset
     H, N, C = 64, 40000, 10
@@ -359,7 +359,7 @@ def test_device_zero_holds_only_its_piece_on_several_gpus(tmp_path, monkeypatch)
     assert [x.device.index for x in pieces] == list(range(n))
     assert torch.cuda.memory_allocated(0) - base <= pieces[0].numel() * 4 + N * 8 + 4096     # its piece and the labels
     monkeypatch.setenv("CODA_B200_SHADOW", "0")              # no cache sized to the free memory
-    monkeypatch.setattr(selector, "split_slab", lambda *a: pytest.fail("a ShardedSlab must not be re-split"))
+    monkeypatch.setattr(dist, "split_slab", lambda *a: pytest.fail("a ShardedSlab must not be re-split"))
     torch.cuda.reset_peak_memory_stats(0)
     sel = CODA(ds)
     torch.cuda.synchronize(0)

@@ -62,14 +62,18 @@ def test_non_contiguous_file_is_refused_with_a_message(tmp_path):
 
 
 def _decide(monkeypatch, path, env, free, ngpus, keep=False, device="cuda:0"):
+    """``load_route``'s device-piece count (0 for a plain load), with the host rules off (``CODA_B200_HOST_SLAB=0``)."""
     import coda_b200.datasets as ds
     monkeypatch.setattr(ds, "_free_bytes", lambda index: free)
     monkeypatch.setattr(torch.cuda, "device_count", lambda: ngpus)
     monkeypatch.setattr(torch.cuda, "current_device", lambda: 0)
-    return ds.shard_load_count(path, device, keep, env=env)
+    env = {"CODA_B200_HOST_SLAB": "0", "CODA_B200_KEEP_DTYPE": "1" if keep else "0", **env}
+    route = ds.load_route(path, device, env)
+    assert route["keep_dtype"] == keep and "host" not in route
+    return route.get("shards", 0)
 
 
-def test_shim_decision_rule(tmp_path, monkeypatch):
+def test_load_route_device_piece_count(tmp_path, monkeypatch):
     p, t = _slab_file(tmp_path, H=4, N=50, C=10, dtype=torch.float16)
     b32 = t.numel() * 4
     b16 = t.numel() * 2
@@ -88,7 +92,7 @@ def test_shim_decision_rule(tmp_path, monkeypatch):
     assert _decide(monkeypatch, p, {"CODA_B200_SHARD_LOAD": "0"}, 1 << 40, 4) == 0
 
 
-def test_shim_keeps_the_plain_load_for_a_legacy_file(tmp_path, monkeypatch):
+def test_load_route_device_pieces_keep_the_plain_load_for_a_legacy_file(tmp_path, monkeypatch):
     p, _ = _slab_file(tmp_path, legacy=True)
     assert _decide(monkeypatch, p, {}, 0, 4) == 0
 
